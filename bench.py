@@ -1,6 +1,6 @@
-"""bench.py -- One-2-3-45 hot paths on B200: sec/mesh end to end, and volume-render M rays/sec.
+"""bench.py -- One-2-3-45 hot paths on H100: sec/mesh end to end, and volume-render M rays/sec.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
 
 Headline metric (BASELINE.json, configs[1]): "sec/mesh end-to-end (256x256 in)".  One step = one 256x256 input
 image -> Zero123 stage 1 + stage 2 (the reference's 10 DDIM sampler calls = 2x76 + 8x49 = 544 UNet passes over a CFG
@@ -16,6 +16,9 @@ pinned host image and ending with the mesh on the host (the pipeline itself move
 host as uint8, as the reference's PNG hand-off does).  The second BASELINE metric, "volume-render M rays/sec", is
 reported under "rays" with its own roofline (GenericTrainer mode='val' on 65 536 rays x (64+64) samples x 32 views).
 N > 1: one process per GPU, one independent image per rank (weak scaling, no data-path collective).
+--dump-outputs DIR: after the timed steps, fixed-shape seeded samples of the arrays the last step returned (mesh vertices,
+triangles, colours, SDF grid) go to DIR/<name>.npy, so that two builds can be compared output for output on the same seeded
+inputs.
 """
 from __future__ import annotations
 
@@ -55,11 +58,6 @@ UNET_FLOP_PER_SAMPLE = 176.3e9
 FLOP_SDF_FWD = 2 * 41856.0
 FLOP_SDF_BWD = 2 * (128 * 144 + 128 * 39)
 RAY_FLOP, RAY_GATHER_BYTES = 211e6, 4.0e6
-# ncu dram__bytes_read.sum + dram__bytes_write.sum over the GEMM launches of one eager UNet forward, by batch (profiles/)
-GEMM_DRAM_BYTES_PER_LAUNCH = {8: 2620.6e6 / 165, 16: 3722.2e6 / 190, 64: 13082.9e6 / 190}
-GEMM_DRAM_NOTE = ("ncu launch lists of one eager UNet iteration per batch (profiles/r2_unet_b64_launches_summary.txt: 13 082.9 MB over the "
-                  "190 gemm_tc launches at batch 64, 3 722.2 MB at batch 16; r2_unet_launches_summary.txt for batch 8): a committed "
-                  "measurement, ncu cannot run inside the bench")
 PUBLISHED_SEC_PER_MESH = 40.0   # BASELINE.md section 1 (reference README.md:154, A6000, whole run.py)
 
 
@@ -69,11 +67,12 @@ def peaks():
         p = json.load(open(path))
         return {"hbm_gbs": p["hbm_gbs"], "bf16_tflops": p["bf16_tflops"], "bf16_sustained": p.get("bf16_tflops_sustained"),
                 "source": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_sustained": 1400.0, "source": "fallback"}
+    # NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 / BF16
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_sustained": None, "source": "data sheet"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -190,6 +189,7 @@ def run_gpu(args):
         dist.barrier()
     clocks = ClockSampler(local)
     clocks.start()
+    torch.manual_seed(0)             # the timed steps draw the same sampler noise in every run with the same arguments
     _lib.reset_launches()
     torch.cuda.synchronize()
     t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -204,6 +204,8 @@ def run_gpu(args):
     wall_s = time.perf_counter() - w0
     launches = _lib.launches()
     clk = clocks.stop()
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs if world == 1 else os.path.join(args.dump_outputs, "rank%d" % rank), mesh)
     ms, e2e_ms = sharding.max_over_ranks([t0.elapsed_time(t1), wall_s * 1e3], dev)
     if rank == 0:
         sec_per_mesh = ms * 1e-3 / (args.steps * world)
@@ -261,7 +263,7 @@ class CpuBaselineJob:
 
 
 def stage_breakdown(z123, tr, dev, pk, world=1):
-    """Per-stage device times, the tensor-core roofline of the dominant kernel (the tcgen05 GEMM inside the UNet)
+    """Per-stage device times, the tensor-core roofline of the dominant kernel (the wgmma GEMM inside the UNet)
     and the volume-rendering throughput with its own roofline.  Untimed extras; every rank runs them (symmetric)."""
     beat("stage breakdown: UNet iterations")
     from o2345 import ops_a
@@ -361,15 +363,10 @@ def stage_breakdown(z123, tr, dev, pk, world=1):
     ms_dec = float(np.mean([ev_time(lambda: vae.decode(z))[0] for _ in range(3)]))
     flops = B_TOP * UNET_FLOP_PER_SAMPLE
     tf = flops_counted / (ms_gemm * 1e-3) / 1e12
-    # DRAM traffic of the same launches: ncu dram__bytes_read.sum + dram__bytes_write.sum summed over the GEMM launches of one
-    # eager UNet forward at this batch (profiles/r2_unet_b64_launches_summary.txt), divided by the launch count -- a committed
-    # measurement, not taken live (ncu cannot run inside the bench)
-    roofline = {"kernel": "gemm_tc_kernel<BN, STAGES, CTAS, MODE> (tcgen05.mma kind::f16, cta_group::2 pairs; all %d GEMM / implicit-conv "
+    roofline = {"kernel": "gemm_tc_kernel<BN, STAGES, MODE> (wgmma.mma_async m64nBNk16 f16, TMA operands; all %d GEMM / implicit-conv "
                           "launches of one UNet iteration at batch %d, the batch of the 49 stage-2 iterations)" % (n_gemm, B_TOP),
                 "bound": "tensor", "achieved": tf, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": tf / pk["bf16_tflops"],
-                "traffic": GEMM_DRAM_BYTES_PER_LAUNCH.get(B_TOP),
-                "traffic_unit": "bytes of DRAM traffic per launch (mean)",
-                "traffic_note": GEMM_DRAM_NOTE, "algorithmic_bytes_per_launch": algo_bytes / max(n_gemm, 1),
+                "algorithmic_bytes_per_launch": algo_bytes / max(n_gemm, 1),
                 "flops_per_step": flops_counted, "gemm_ms_per_unet_iteration": ms_gemm,
                 "other_batches": {str(B): {"unet_iteration_ms": prof[B][0], "gemm_ms": prof[B][1],
                                            "tflops": prof[B][2] / (prof[B][1] * 1e-3) / 1e12} for B, _ in UNET_SCHEDULE if B != B_TOP},
@@ -452,6 +449,33 @@ def render_throughput(tr, sample, imgs, fmaps, cond, sizeW, sizeH, dev, pk):
                 "render_blend_tc_kernel (mma.sync, default)" if prec == 1 else "render_blend_kernel precision %d" % prec: {"ms": ms_bl, "valid_pairs": pairs, "ms_fp32_kernel": ms_bl32,
                                            "max_colour_drift_vs_fp32_kernel": drift,
                                         "gather_gbs": (pairs * 960 + n_act * 544) / (ms_bl * 1e-3) / 1e9}}}
+
+
+DUMP_ROWS = 1 << 16        # rows kept of a row array (mesh vertices, triangles, colours)
+DUMP_ELEMENTS = 1 << 20    # elements kept of a grid (the SDF field)
+
+
+def dump_outputs(out_dir, outputs):
+    """Every array of `outputs` as out_dir/<name>.npy, float32 where that is exact (fp32 data, integers below 2^24), float64
+    otherwise, with a FIXED shape.  Runs of one build are bit-identical, but a mesh's size follows the last bits of the views
+    it was reconstructed from (125 stochastic DDIM steps amplify them), so two builds that round differently give meshes of
+    different sizes; to compare them array by array, each array is a fixed, seeded sample -- DUMP_ROWS rows of a row array,
+    DUMP_ELEMENTS elements of a grid -- taken at the same relative positions (rows in marching-cubes lattice order), with
+    the sampled indices in out_dir/<name>_index.npy.  About 20 MB in all."""
+    os.makedirs(out_dir, exist_ok=True)
+    rng = np.random.default_rng(0)
+    for name, v in sorted(outputs.items()):
+        v = v.detach().cpu().numpy() if torch.is_tensor(v) else v
+        if not isinstance(v, np.ndarray):
+            continue
+        exact32 = (v.dtype.kind == "f" and v.itemsize <= 4) or (v.dtype.kind in "iub" and (v.size == 0 or np.abs(v).max() < 2 ** 24))
+        rows = v.reshape(len(v), -1) if v.ndim == 2 else v.reshape(-1)
+        pos = np.sort(rng.random(DUMP_ROWS if v.ndim == 2 else DUMP_ELEMENTS))
+        idx = np.minimum((pos * len(rows)).astype(np.int64), max(len(rows) - 1, 0))
+        out = rows[idx] if len(rows) else rows
+        np.save(os.path.join(out_dir, name + ".npy"), out.astype(np.float32 if exact32 else np.float64))
+        np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+        beat("dump: %s %s of %s" % (name, out.shape, v.shape))
 
 
 def host_threads():
@@ -607,6 +631,8 @@ def main():
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="o2345", choices=["o2345", "reference"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write fixed-shape seeded samples of the arrays the last timed step computed to DIR/<name>.npy")
     ap.add_argument("--cpu-baseline-child", action="store_true", help=argparse.SUPPRESS)
     args = ap.parse_args()
     if args.cpu_baseline_child:      # child of CpuBaselineJob: the port's result as one JSON line on stdout

@@ -1,5 +1,5 @@
 /*
- * libo2345_sm100.so -- C-ABI of the B200-native (sm_100a) kernels behind One-2-3-45's
+ * libo2345_sm90.so -- C-ABI of the H100-native (sm_90a) kernels behind One-2-3-45's
  * SparseNeuS-style reconstruction hot path (SURVEY.md section 8, rows B1-B15).
  *
  * The reference has no FFI of its own for this path: its boundary is plain Python classes
@@ -40,7 +40,7 @@ typedef void* o2345_stream_t;
 int o2345_abi_version(void);
 /* Copies the last error message of the calling thread into buf (NUL terminated). */
 int o2345_last_error(char* buf, size_t n);
-/* Fills (major, minor, sm_count) of the current device; fails if it is not sm_100. */
+/* Fills (major, minor, sm_count) of the current device; fails if it is not sm_90. */
 int o2345_device_info(int* major, int* minor, int* sms);
 
 /* ------------------------------------------------------------------------------------------
@@ -243,7 +243,7 @@ typedef struct o2345_views {
  * matrix stored [in][out] in the order documented in csrc/render.cu. */
 #define O2345_BLEND_FP32 0     /* fp32 FMA mat-vecs in the reference's operation order (tight oracle parity)            */
 #define O2345_BLEND_TC_FP16 1  /* per-(sample, view) MLPs as mma.sync products: fp16 operands, fp32 accumulate / statistics */
-#define O2345_BLEND_TC5 2      /* the same MLPs as tcgen05.mma M = 128 tiles (4 samples x 32 views, a lane is a view), TMEM accumulators */
+#define O2345_BLEND_TC5 2      /* the same MLPs as wgmma M = 128 tiles (4 samples x 32 views, a lane is a view) */
 int o2345_render_blend(const o2345_points* src, int64_t n, const uint8_t* active, const float* vol_cl,
                        const float* occ, int D, const o2345_views* views, int dir_mode, const float* query_center,
                        const float* dirs, const float* rnet_pack, int precision, float* rgb, int32_t* nvalid,
@@ -258,7 +258,7 @@ int o2345_ray_composite(const float* rays_d, int64_t R, int S, const float* mid_
                         float* alpha_out, float* weights_sum_out, uint8_t* color_mask_out, o2345_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * Path A (rows A2-A4, A6): fp16 tensor-core GEMM, tcgen05.mma + TMEM accumulators + TMA operands.
+ * Path A (rows A2-A4, A6): fp16 tensor-core GEMM, wgmma.mma_async + register accumulators + TMA operands.
  * Replaces the cuBLAS / cuDNN calls behind nn.Linear, 1x1 and (im2col'd) 3x3 nn.Conv2d and the
  * attention einsums of the Zero123 UNet and VAE:
  *          ldm/modules/diffusionmodules/openaimodel.py:745-777, ldm/modules/attention.py:170-193,
@@ -292,7 +292,7 @@ int o2345_gemm_f16(const void* A, const void* B, void* C, int M, int N, int K, i
                    int64_t stride_b_b, int64_t stride_c_h, int64_t stride_c_b, const o2345_epilogue* ep /* NULL: plain */,
                    float* splitk_ws, int64_t ws_floats, o2345_stream_t stream);
 /* splitk_ws (optional, may be NULL): fp32 scratch of ws_floats elements, no initialisation needed.  When the output tiles
- * alone cannot fill the GPU the K range is split over up to min(8, ws_floats / (M*N)) CTA pairs per tile that run as one
+ * alone cannot fill the GPU the K range is split over up to min(8, ws_floats / (M*N)) CTAs per tile that run as one
  * thread-block cluster: each stores its partial tile in its own [M, N] plane of the scratch, a cluster barrier publishes the
  * planes, and every split sums them and applies the epilogue to its share of the tile.  One workspace serves one stream at
  * a time. */
@@ -304,17 +304,18 @@ int o2345_gemm_f16(const void* A, const void* B, void* C, int M, int N, int K, i
 int o2345_last_trap(char* buf, size_t n);
 
 /* Tuning hook (tools/gemm_sweep.py; not part of the data path): force the tile configuration of the following non-batched
- * GEMM / conv calls: ctas in {1, 2}, bn in {64, 128, 160, 256}, splits >= 1; 0 keeps the heuristic's choice of that field. */
+ * GEMM / conv calls: bn in {64, 128, 160, 256}, splits 1..8; 0 keeps the heuristic's choice of that field.  ctas is accepted and
+ * ignored: every tile is one CTA. */
 void o2345_debug_gemm_force(int ctas, int bn, int splits);
-/* Tuning hook: the persistent variant of the kernel (one CTA pair per SM pair walking many tiles, epilogue of tile i under
- * the main loop of tile i + 1).  mode 0: heuristic (at least min_tiles pair tiles; min_tiles 0 = default), 1: wherever it is
- * available (pair tiles of 128+ columns, staged fp16 epilogue, no split-K), 2: never. */
+/* Tuning hook: the persistent launch of the kernel (at most one CTA per SM walking the tiles; launch and prologue paid once
+ * per SM).  mode 0: heuristic (at least min_tiles tiles; min_tiles 0 = default),
+ * 1: wherever it is available (staged fp16 epilogue, no split-K, no head batches), 2: never. */
 void o2345_debug_gemm_persist(int mode, int min_tiles);
-/* Tuning hook: the seven constants of the tile-configuration cost model (per-SM ingest B/clk, two-CTA bonus, fabric B/clk,
+/* Tuning hook: the seven constants of the tile-configuration cost model (per-SM ingest B/clk, multi-wave bonus, fabric B/clk,
  * fixed us, epilogue us per 160 columns, split-K us, split-K us per split and 128 columns); see gemm_tc.cu predict_us. */
 void o2345_debug_gemm_model(const float* seven);
 
-/* Diagnostic hook (not part of the data path): when device_buf16 != NULL, CTA (0,0,0) of every following CTA-pair GEMM
+/* Diagnostic hook (not part of the data path): when device_buf16 != NULL, CTA (0,0,0) of every following GEMM
  * launch stores clock64() stamps of its phases into device_buf16[0..8] (entry, prologue done, first TMA issued, last TMA
  * issued, first operands landed, last MMA issued, accumulator ready, epilogue done, exit).  NULL switches it off. */
 void o2345_debug_gemm_trace(long long* device_buf16);

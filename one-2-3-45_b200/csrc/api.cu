@@ -1,4 +1,4 @@
-// Library-wide plumbing of libo2345_sm100.so: error string, device query.
+// Library-wide plumbing of libo2345_sm90.so: error string, device query.
 #include <stdarg.h>
 
 #include <stdlib.h>
@@ -31,7 +31,7 @@ int sm_count() {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0)
-      sms = 148;
+      sms = 132;
   }
   return sms;
 }
@@ -56,8 +56,8 @@ extern "C" int o2345_device_info(int* major, int* minor, int* sms) {
   if (major) *major = ma;
   if (minor) *minor = mi;
   if (sms) *sms = n;
-  if (ma != 10) {
-    o2345::set_error("o2345_device_info: device is sm_%d%d, this library is built for sm_100a only", ma, mi);
+  if (ma != 9 || mi != 0) {
+    o2345::set_error("o2345_device_info: device is sm_%d%d, this library is built for sm_90a only", ma, mi);
     return O2345_EUNSUPPORTED;
   }
   return O2345_OK;

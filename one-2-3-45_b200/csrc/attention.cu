@@ -1,10 +1,10 @@
 // Fused multi-head self-attention for the UNet's spatial transformers (SURVEY.md row A4): softmax(Q K^T * scale) V in one
 // kernel, scores never leave the SM.  Replaces reference ldm/modules/attention.py:170-193, which materialises the
-// [(b h), N, N] score tensor (134 MB per layer at N = 1024) three times; the r1 three-kernel version here (batched tcgen05
-// GEMM -> softmax -> batched GEMM) spent 0.43 ms per layer in 4096 one-k-block CTAs for QK^T alone.
+// [(b h), N, N] score tensor (134 MB per layer at N = 1024) three times; the three-kernel route (batched GEMM -> softmax
+// -> batched GEMM) runs 4096 one-k-block CTAs for QK^T alone.
 //
-// Head dims are 40 / 80 / 160 and sequences 16..1024 tokens: far too small per (batch, head) to fill a 128-row tcgen05
-// tile pipeline, so this kernel uses warp-level mma.sync.m16n8k16 (fp16 in, fp32 accumulate) in the FlashAttention-2
+// Head dims are 40 / 80 / 160 and sequences 16..1024 tokens: far too small per (batch, head) to fill a 128-row GEMM tile
+// pipeline, so this kernel uses warp-level mma.sync.m16n8k16 (fp16 in, fp32 accumulate) in the FlashAttention-2
 // arrangement: one CTA = 4 warps = 64 queries of one (b, h); K / V stream through a two-stage cp.async ring of 64-key tiles (both row-major;
 // the P V operand comes out of ldmatrix.trans); online softmax in fp32 registers with exp2; the S
 // accumulator fragments are re-used in place as the A fragments of the P V product.  The arithmetic is softmax-bound

@@ -1,4 +1,4 @@
-// Shared helpers for libo2345_sm100.so (sm_100a only).
+// Shared helpers for libo2345_sm90.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -46,14 +46,14 @@ struct PerDeviceOnce {
 };
 
 // Number of SMs of the current device (cached).  Grids of persistent kernels are sized
-// as a multiple of this (148 on B200).
+// as a multiple of this (132 on H100 SXM).
 int sm_count();
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
 // Programmatic dependent launch (PDL).  The ~660 kernels of a UNet pass are launched with programmatic stream
-// serialization: kernel N+1 may be scheduled while kernel N drains, runs its prologue (barrier init, TMEM allocation,
-// descriptor prefetch, index math) and then blocks in pdl_wait() until kernel N has completed and flushed its writes.
+// serialization: kernel N+1 may be scheduled while kernel N drains, runs its prologue (barrier init, descriptor prefetch,
+// index math) and then blocks in pdl_wait() until kernel N has completed and flushed its writes.
 // Every kernel launched this way calls pdl_wait() before its first access to memory another kernel may have written (or
 // may still read), so the chain stays transitively ordered; kernels launched normally are unaffected (wait is a no-op).
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }

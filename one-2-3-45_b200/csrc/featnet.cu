@@ -25,7 +25,7 @@ conv2d_kernel(const float* __restrict__ in, int Cin, int H, int W, const float* 
   constexpr int PT = (TILE - 1) * S + K;  // input patch side
   __shared__ float sIn[CCH][PT][PT + 1];
   __shared__ __align__(16) float sWt[CCH][K * K][COUT];
-  __shared__ float sRed[2][COUT];
+  __shared__ float sRed[2][TILE * TILE / 32][COUT];   // per-warp channel sums, added in warp order
   const int tx = threadIdx.x % TILE, ty = threadIdx.x / TILE;
   const int n = blockIdx.z;
   const int ox = blockIdx.x * TILE + tx, oy = blockIdx.y * TILE + ty;
@@ -72,18 +72,18 @@ conv2d_kernel(const float* __restrict__ in, int Cin, int H, int W, const float* 
     for (int c = 0; c < COUT; ++c) o[(int64_t)c * Ho * Wo] = acc[c];
   }
   if (stats) {
-    if (threadIdx.x < COUT) sRed[0][threadIdx.x] = 0.f, sRed[1][threadIdx.x] = 0.f;
-    __syncthreads();
 #pragma unroll
     for (int c = 0; c < COUT; ++c) {
       float s = valid ? acc[c] : 0.f, q = s * s;
       for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o), q += __shfl_xor_sync(0xffffffffu, q, o);
-      if ((threadIdx.x & 31) == 0) atomicAdd(&sRed[0][c], s), atomicAdd(&sRed[1][c], q);
+      if ((threadIdx.x & 31) == 0) sRed[0][threadIdx.x >> 5][c] = s, sRed[1][threadIdx.x >> 5][c] = q;
     }
     __syncthreads();
-    if (threadIdx.x < COUT) {
-      atomicAdd(stats + threadIdx.x, (double)sRed[0][threadIdx.x]);
-      atomicAdd(stats + COUT + threadIdx.x, (double)sRed[1][threadIdx.x]);
+    if (threadIdx.x < COUT) {   // fixed-order CTA sum; the CTAs' fp32 sums are added in fp64 (exact in practice)
+      float s = 0.f, q = 0.f;
+      for (int w = 0; w < TILE * TILE / 32; ++w) s += sRed[0][w][threadIdx.x], q += sRed[1][w][threadIdx.x];
+      atomicAdd(stats + threadIdx.x, (double)s);
+      atomicAdd(stats + COUT + threadIdx.x, (double)q);
     }
   }
 }

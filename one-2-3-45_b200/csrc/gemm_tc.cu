@@ -1,4 +1,4 @@
-// fp16 GEMM on the 5th-generation tensor cores (tcgen05 + TMEM accumulators), operands fed by TMA.
+// fp16 GEMM on the Hopper tensor cores (wgmma.mma_async, fp32 accumulators in registers), operands fed by TMA.
 // Path A of SURVEY.md section 8 (rows A2-A4, A6, A8): every Linear / 1x1 conv / 3x3 conv of the Zero123 UNet, the VAE and
 // the CLIP tower, and the QK^T / PV products of the unfused attention fallback, go through this file.
 //
@@ -6,31 +6,22 @@
 //
 // A and B are both K-major (row-major activations [rows, K]; nn.Linear / flattened conv weights [N, K]).
 //
-// ONE kernel template, gemm_tc_kernel<BN, STAGES, CTAS, MODE> (round 1 had two hand-copied kernels):
-//   CTAS = 2  a CTA PAIR (cluster of 2 on one TPC) computes a 256 x BN tile with tcgen05.mma.cta_group::2: each CTA stages
-//             its own 128 rows of A and HALF of the B tile, the tensor cores of both SMs read both halves (100-128 flop per
-//             operand byte instead of 64 for a lone 128 x 128 tile; the L2 -> SM fabric is the binding resource);
-//   CTAS = 1  a single CTA computes 128 x BN (M <= 128, and the 4-D batched per-head mode).
-// Warp roles (320 threads, two CTAs resident per SM so that one tile's prologue / epilogue overlaps the other's main loop):
-//   warp 0      TMA producer: cp.async.bulk.tensor (SWIZZLE_128B) into a STAGES-deep shared-memory ring guarded by full /
-//               empty mbarriers (pair: the bytes of both CTAs are counted on the leader's full barrier, stages are freed in
-//               both CTAs by a multicast tcgen05.commit);
-//   warp 1      allocates TMEM; one lane (of the leader) issues tcgen05.mma M = 128 * CTAS, N = BN, K = 16, four per stage;
-//   warps 2-9   EIGHT epilogue warps (round 1: four): warp w owns TMEM lane quarter w % 4 (a hardware rule) and one of two
-//               column ranges of the tile.  While the main loop runs they stage bias / row-group bias in shared memory and
-//               PREFETCH THE RESIDUAL into registers (round 1 fetched it after the accumulator was complete: 2 400 - 6 000
-//               cycles of exposed latency per tile); then tcgen05.ld -> alpha / bias / activation / GEGLU gate -> fp16 ->
-//               a shared-memory transpose in the idle operand ring -> coalesced row stores with the residual added.
-// MODE selects the epilogue at compile time (round 1 inlined every variant into one 9 600-instruction body):
+// ONE kernel template, gemm_tc_kernel<BN, STAGES, MODE>: a CTA computes a 128 x BN tile.
+// Warp roles (384 threads = three warpgroups, one CTA per SM):
+//   warpgroup 0   one thread is the TMA producer: cp.async.bulk.tensor (SWIZZLE_128B) into a STAGES-deep shared-memory ring
+//                 guarded by full / empty mbarriers;
+//   warpgroups 1-2  each issues wgmma.mma_async m64nBNk16 on its 64 rows of the tile, four per stage, one stage in flight
+//                 while the previous one is released; once the K loop is done the (now idle) operand ring receives the fp32
+//                 accumulator tile, and the same EIGHT warps run the epilogue: warp w owns 32 rows and one of two column
+//                 ranges of the tile; alpha / bias / activation / GEGLU gate -> fp16 -> a shared-memory transpose ->
+//                 coalesced row stores with the residual added.
+// MODE selects the epilogue at compile time:
 //   0 staged, no activation   1 staged, GEGLU gate   2 staged, SiLU / GELU / QuickGELU (runtime switch per tile)
 //   3 generic (fp32 output, batched, unaligned N) and SPLIT-K.
-// Split-K (tiles alone cannot fill 148 SMs): the `splits` CTAs (pairs) of a tile are launched as ONE thread-block cluster
-// (CTAS, 1, splits), so the hardware co-schedules them.  Each stores its partial accumulator into its own fp32 plane of the
+// Split-K (tiles alone cannot fill 132 SMs): the `splits` CTAs of a tile are launched as ONE thread-block cluster
+// (1, 1, splits), so the hardware co-schedules them.  Each stores its partial accumulator into its own fp32 plane of the
 // workspace, a cluster barrier (release / acquire) publishes the planes, and every split then sums the planes and applies
-// the epilogue to ITS share of the tile.  No atomics, no tickets, no zero-initialised scratch, no second kernel (round 1
-// added into one plane with L2 atomics -- they sustain only ~90 G elements/s -- and launched a finalize kernel: 92 extra
-// launches per UNet iteration; a first round-2 version let the last-arriving CTA finish the tile alone: 13-19 us of
-// serial L2 round trips, see profiles/r2_gemm_trace.txt).
+// the epilogue to ITS share of the tile.  No atomics, no tickets, no zero-initialised scratch, no second kernel.
 // Every mbarrier wait is bounded in TIME (4 s): a protocol bug or a lost arrival records which barrier of which CTA of
 // which problem stalled in a host-visible buffer (o2345_last_trap) and traps, instead of spinning for tens of minutes.
 #include <cuda.h>
@@ -38,6 +29,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace o2345 {
 namespace {
@@ -45,17 +37,16 @@ namespace {
 constexpr int BM = 128, BK = 64;
 constexpr int EPI_WARPS = 8;
 constexpr int EPI_THREADS = 32 * EPI_WARPS;
-constexpr int GEMM_THREADS = 64 + EPI_THREADS;
+constexpr int GEMM_THREADS = 128 + EPI_THREADS;
 constexpr uint64_t WAIT_LIMIT_NS = 4000000000ull;   // bounded waits: a protocol bug traps (with a record) instead of hanging the GPU
-constexpr uint32_t PEER_MASK = 0xFEFFFFFFu;         // clears the CTA-rank bit of a shared::cluster address: "the even CTA of my pair"
-constexpr int MAX_CLUSTER = 16;                     // CTAS * splits: one cluster per tile (non-portable size, opted into per kernel)
-constexpr int RES_PREFETCH = 8;                     // 16-byte residual pieces per lane fetched before the accumulator is ready
+constexpr int MAX_CLUSTER = 8;                      // splits: one cluster per tile (8 = the portable cluster size)
+constexpr int RES_PREFETCH = 8;                     // 16-byte residual pieces per lane fetched before the accumulator is read
 
-enum { WAIT_EMPTY = 1, WAIT_FULL = 2, WAIT_ACC = 3, WAIT_ACC_FREE = 4 };   // which wait timed out (o2345_last_trap)
+enum { WAIT_EMPTY = 1, WAIT_FULL = 2 };   // which wait timed out (o2345_last_trap)
 
 struct TrapRecord {
   unsigned long long magic;
-  int tag, stage, bx, by, bz, rank, M, N, K, bn, ctas, mode, splits, conv;
+  int tag, stage, bx, by, bz, rank, M, N, K, bn, mode, splits, conv;
 };
 constexpr unsigned long long TRAP_MAGIC = 0x6f32333435545250ull;
 
@@ -66,6 +57,9 @@ __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ uint32_t mbar_try(uint64_t* bar, uint32_t parity) {
   uint32_t done;
@@ -95,19 +89,6 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-// pair forms: the data lands in the executing CTA's shared memory, the bytes are counted on the leader CTA's barrier
-__device__ __forceinline__ void tma2_load_2d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tma2_load_4d(void* dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-      ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar) & PEER_MASK), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -116,60 +97,17 @@ __device__ __forceinline__ uint32_t cluster_ctarank() {
 __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
-__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the eight epilogue warps only
+__device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the eight MMA / epilogue warps only
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start >> 4,
-// LBO = 1 (ignored for swizzled K-major), SBO = 1024 B (8 rows x 128 B), version 1, layout type 2.
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-// kind::f16 instruction descriptor: D = f32, A = B = f16, both K-major, N >> 3 at bit 17, M >> 4 at bit 24.
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-template <int CTAS>
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  if (CTAS == 2)
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-  else
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// pair: arrives on the barrier at this shared-memory offset in BOTH CTAs of the pair (cluster ranks 2j and 2j + 1: `mask`)
-// once the pair's MMAs so far have finished
-template <int CTAS>
-__device__ __forceinline__ void umma_commit(uint64_t* bar, uint16_t mask) {
-  if (CTAS == 2)
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"(mask)
-                 : "memory");
-  else
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// the accumulator tile in shared memory: fp32 [128][BN + 4] (the pad spreads the row-per-thread reads over the banks)
+__host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }
+// 32 consecutive accumulator columns of one row
+__device__ __forceinline__ void acc_ld32(const float* src, uint32_t (&r)[32]) {
+#pragma unroll
+  for (int i = 0; i < 8; ++i) {
+    const float4 v = reinterpret_cast<const float4*>(src)[i];
+    r[4 * i] = __float_as_uint(v.x), r[4 * i + 1] = __float_as_uint(v.y), r[4 * i + 2] = __float_as_uint(v.z), r[4 * i + 3] = __float_as_uint(v.w);
+  }
 }
 
 struct GemmParams {
@@ -202,13 +140,14 @@ struct GemmParams {
   // the cluster barrier publishes the planes, then every split sums and finishes its share of the tile.
   int splits;
   float* ws;
+  int persist;                 // 1: a grid of at most one CTA per SM walks the tiles (staged epilogues only)
   // GroupNorm statistics of the OUTPUT: colstats[(g * 2 + 0) * N + col] += x and colstats[(g * 2 + 1) * N + col] += x^2 over the
   // final fp16 values of row group g = row / stats_rpg (the consumer turns them into mean / rstd); nullptr: off
   float* colstats;
   int stats_rpg, stats_groups;
   long long* trace;            // diagnostic: CTA (0,0,0) stores clock64() stamps of its phases (o2345_debug_gemm_trace), else nullptr
   TrapRecord* diag;            // host-mapped record written before a bounded wait traps (may be nullptr)
-  int bn, ctas, mode;          // for the trap record
+  int bn, mode;                // for the trap record
 };
 
 __device__ __forceinline__ void stamp(const GemmParams& p, int slot) {
@@ -230,7 +169,7 @@ __device__ __noinline__ void wait_timed_out(const GemmParams& p, int tag, int st
   if (p.diag) {
     TrapRecord* d = p.diag;
     d->tag = tag, d->stage = stage, d->bx = blockIdx.x, d->by = blockIdx.y, d->bz = blockIdx.z, d->rank = (int)cluster_ctarank();
-    d->M = p.M, d->N = p.N, d->K = p.K, d->bn = p.bn, d->ctas = p.ctas, d->mode = p.mode, d->splits = p.splits, d->conv = p.conv;
+    d->M = p.M, d->N = p.N, d->K = p.K, d->bn = p.bn, d->mode = p.mode, d->splits = p.splits, d->conv = p.conv;
     __threadfence_system();
     d->magic = TRAP_MAGIC;
     __threadfence_system();
@@ -502,17 +441,17 @@ __device__ __forceinline__ float act_fn(float x) {
   return x;
 }
 
-// Phase 1 of the staged epilogue for one thread (= one accumulator row) over tile columns [c_lo, c_hi): TMEM -> registers ->
+// Phase 1 of the staged epilogue for one thread (= one accumulator row) over tile columns [c_lo, c_hi): accumulator tile ->
 // alpha / bias / row-group bias / activation (ACT 3: GEGLU gate) -> fp16 -> this row of the warp's shared-memory slab.
 // rb: this row's row-group bias indexed by TILE column (nullptr: none); rb_smem: it is the shared-memory copy (no N tail).
 template <int ACT>
-__device__ __forceinline__ void stage_rows(const GemmParams& p, uint32_t tmem_row_base, uint8_t* mine, int n0, int c_lo, int c_hi,
+__device__ __forceinline__ void stage_rows(const GemmParams& p, const float* acc_row, uint8_t* mine, int n0, int c_lo, int c_hi,
                                            const float* sbias, const __half* rb, bool rb_smem) {
 #pragma unroll 1
   for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
-    uint32_t r[32];
-    tmem_ld32(tmem_row_base + c0, r);
     if (n0 + c0 >= p.N) break;                     // warp-uniform
+    uint32_t r[32];
+    acc_ld32(acc_row + c0, r);
     if (ACT == 3) {
       __half2 h[8];
 #pragma unroll
@@ -592,16 +531,16 @@ __device__ __forceinline__ uint4 add_h8(uint4 v, uint4 q) {
   return v;
 }
 
-// Staged epilogue of ONE warp: 32 accumulator rows (its TMEM lane quarter) x tile columns [c_lo, c_hi), fp16 output.
-//   phase 1   thread = row, as the TMEM load delivers it: alpha / bias / row-group bias / activation / GEGLU gate, rounded to
-//             fp16 (where autocast rounds the layer output) into this warp's slab of the (now idle) operand ring;
+// Staged epilogue of ONE warp: 32 accumulator rows x tile columns [c_lo, c_hi), fp16 output.
+//   phase 1   thread = row of the accumulator tile: alpha / bias / row-group bias / activation / GEGLU gate, rounded to
+//             fp16 (where autocast rounds the layer output) into this warp's slab;
 //   phase 2   the warp walks the slab in 16-byte pieces along rows, adds the residual (prefetched for the first
 //             RES_PREFETCH pieces of a lane) and writes whole rows: every global access is a run of full 32-byte sectors.
 // (r1 trace: with one 16-byte store per lane to 32 different rows the epilogue took 46 000 cycles per tile.)
 template <int BN, int MODE>
-__device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpOut& g, uint32_t tmem_row_base, uint8_t* slab, int lane,
+__device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpOut& g, const float* acc_row, uint8_t* slab, int lane,
                                                 int m0, int row0, int n0, int c_lo, int c_hi, const float* sbias, const __half* srb,
-                                                const uint4 (&resq)[RES_PREFETCH], uint32_t release_bar = 0) {
+                                                const uint4 (&resq)[RES_PREFETCH]) {
   const int row = row0 + lane;
   // row-group bias of this thread's row: from the smem copy when the tile spans few groups, else straight from global
   const __half* rb = nullptr;
@@ -614,20 +553,15 @@ __device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpO
   }
   uint8_t* mine = slab + lane * g.stride;
   if (MODE == 0) {
-    stage_rows<0>(p, tmem_row_base, mine, n0, c_lo, c_hi, sbias, rb, rb_smem);
+    stage_rows<0>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem);
   } else if (MODE == 1) {
-    stage_rows<3>(p, tmem_row_base, mine, n0, c_lo, c_hi, sbias, rb, rb_smem);
+    stage_rows<3>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem);
   } else {   // the activation switch is hoisted out of the element loops: one branch per tile
     switch (p.act) {
-      case 1: stage_rows<1>(p, tmem_row_base, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
-      case 2: stage_rows<2>(p, tmem_row_base, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
-      default: stage_rows<4>(p, tmem_row_base, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
+      case 1: stage_rows<1>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
+      case 2: stage_rows<2>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
+      default: stage_rows<4>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
     }
-  }
-  if (release_bar) {   // persistent kernel: this warp has read its part of the accumulator buffer -- hand it back to the MMA issuer
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncwarp();
-    if (lane == 0) asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(release_bar) : "memory");
   }
   __syncwarp();
   __half* C = reinterpret_cast<__half*>(p.C);
@@ -710,171 +644,154 @@ __device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpO
   }
 }
 
-__host__ __device__ constexpr int tmem_cols(int bn) { return bn <= 32 ? 32 : bn <= 64 ? 64 : bn <= 128 ? 128 : bn <= 256 ? 256 : 512; }
 __host__ __device__ constexpr int epi_slab_bytes(int bn) { return EPI_WARPS * 32 * (col_split(bn) * 2 + 16); }
-constexpr int smem_bytes(int bn, int stages, int ctas) {
-  return stages * (BM * BK * 2 + (bn / ctas) * BK * 2) + (2 * stages + 1) * 8 + 8 + 16 + epi_smem_bytes(bn) + 1024;
+constexpr int smem_bytes(int bn, int stages) {
+  return stages * (BM * BK * 2 + bn * BK * 2) + epi_slab_bytes(bn) + 2 * stages * 8 + 16 + epi_smem_bytes(bn) + 1024;
 }
 
-// One stage of the TMA producer: this CTA's 128 rows of A and its BROWS rows of the B tile for k-block kb of the tile at
-// (m0, n0).  Pair (CTAS = 2): the bytes of both CTAs are counted on the leader's full barrier.
-template <int CTAS, int BROWS>
+// One stage of the TMA producer: the 128 rows of A and the BN rows of B for k-block kb of the tile at (m0, n0).
+template <int BN>
 __device__ __forceinline__ void produce_stage(const GemmParams& p, const CUtensorMap* tmA, const CUtensorMap* tmB, uint8_t* a_dst,
-                                              uint8_t* b_dst, uint64_t* full_bar, int kb, int m0, int n0, uint32_t rank, int bz) {
-  constexpr int A_BYTES = BM * BK * 2, B_BYTES = BROWS * BK * 2;
-  if (CTAS == 2) {
-    if (rank == 0) mbar_expect_tx(full_bar, 2 * (A_BYTES + B_BYTES));   // the peer's bytes land on this barrier too
-    const int nb = n0 + (int)rank * BROWS;
-    if (p.conv) {
-      const int tap = kb / p.cblocks, c0 = (kb - tap * p.cblocks) * BK;
-      const int x0 = m0 % p.cW, y0 = (m0 / p.cW) % p.cH, b0 = m0 / (p.cW * p.cH);
-      tma2_load_4d(a_dst, tmA, full_bar, c0, x0 + tap % p.ctx + p.cox, y0 + tap / p.ctx + p.coy, b0);
-      tma2_load_2d(b_dst, tmB, full_bar, tap * p.cC + c0, nb);
-    } else {
-      tma2_load_2d(a_dst, tmA, full_bar, kb * BK, m0);
-      tma2_load_2d(b_dst, tmB, full_bar, kb * BK, nb);
-    }
+                                              uint8_t* b_dst, uint64_t* full_bar, int kb, int m0, int n0, int bz) {
+  mbar_expect_tx(full_bar, BM * BK * 2 + BN * BK * 2);
+  if (p.conv) {
+    const int tap = kb / p.cblocks, c0 = (kb - tap * p.cblocks) * BK;
+    const int x0 = m0 % p.cW, y0 = (m0 / p.cW) % p.cH, b0 = m0 / (p.cW * p.cH);
+    tma_load_4d(a_dst, tmA, full_bar, c0, x0 + tap % p.ctx + p.cox, y0 + tap / p.ctx + p.coy, b0);
+    tma_load_2d(b_dst, tmB, full_bar, tap * p.cC + c0, n0);
+  } else if (p.batched) {
+    tma_load_4d(a_dst, tmA, full_bar, kb * BK, m0, bz % p.nh, bz / p.nh);
+    tma_load_4d(b_dst, tmB, full_bar, kb * BK, n0, bz % p.nh, bz / p.nh);
   } else {
-    mbar_expect_tx(full_bar, A_BYTES + B_BYTES);
-    if (p.conv) {
-      const int tap = kb / p.cblocks, c0 = (kb - tap * p.cblocks) * BK;
-      const int x0 = m0 % p.cW, y0 = (m0 / p.cW) % p.cH, b0 = m0 / (p.cW * p.cH);
-      tma_load_4d(a_dst, tmA, full_bar, c0, x0 + tap % p.ctx + p.cox, y0 + tap / p.ctx + p.coy, b0);
-      tma_load_2d(b_dst, tmB, full_bar, tap * p.cC + c0, n0);
-    } else if (p.batched) {
-      tma_load_4d(a_dst, tmA, full_bar, kb * BK, m0, bz % p.nh, bz / p.nh);
-      tma_load_4d(b_dst, tmB, full_bar, kb * BK, n0, bz % p.nh, bz / p.nh);
-    } else {
-      tma_load_2d(a_dst, tmA, full_bar, kb * BK, m0);
-      tma_load_2d(b_dst, tmB, full_bar, kb * BK, n0);
-    }
+    tma_load_2d(a_dst, tmA, full_bar, kb * BK, m0);
+    tma_load_2d(b_dst, tmB, full_bar, kb * BK, n0);
+  }
+}
+
+// A warpgroup's m64nBN accumulator fragment -> rows [row0, row0 + 64) of the shared-memory accumulator tile
+template <int BN>
+__device__ __forceinline__ void acc_store(float* acc, const float (&d)[BN / 2], int row0, int t) {
+  const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    *reinterpret_cast<float2*>(acc + r * acc_ld(BN) + 8 * j + c) = make_float2(d[4 * j], d[4 * j + 1]);
+    *reinterpret_cast<float2*>(acc + (r + 8) * acc_ld(BN) + 8 * j + c) = make_float2(d[4 * j + 2], d[4 * j + 3]);
   }
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
-// Two CTAs per SM: their prologues / epilogues overlap each other's main loops.  (Measured alternative, dropped: one CTA per
-// SM with a ring twice as deep -- no gain on launches of <= 148 CTAs, 35 % slower on multi-wave launches: the main loops are
-// not bound by bytes in flight; ncu shows 5.9 TB/s of L2 -> SM operand traffic on the 8192 x 320 x 2880 conv.)
-template <int BN, int STAGES, int CTAS, int MODE>
-__global__ void __launch_bounds__(GEMM_THREADS, 2)
+template <int BN, int STAGES, int MODE>
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by SWIZZLE_128B
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int BROWS = BN / CTAS;                           // rows of B staged by this CTA (pair: half of the tile)
-  constexpr int A_BYTES = BM * BK * 2, B_BYTES = BROWS * BK * 2;
+  constexpr int A_BYTES = BM * BK * 2, B_BYTES = BN * BK * 2;
   static_assert(B_BYTES % 1024 == 0, "stage bases must stay 1024-byte aligned for SWIZZLE_128B");
-  static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "tile width: a multiple of 32 (GEGLU chunks, 32-column TMEM loads)");
-  static_assert(epi_slab_bytes(BN) <= STAGES * (A_BYTES + B_BYTES), "the output transpose must fit in the operand ring");
-  constexpr int TCOLS = tmem_cols(BN);
+  static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "tile width: a multiple of 32 (GEGLU chunks, 32-column epilogue reads)");
+  static_assert(BM * acc_ld(BN) * 4 <= STAGES * (A_BYTES + B_BYTES), "the accumulator tile must fit in the operand ring");
   constexpr int CSPLIT = col_split(BN);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(sB + STAGES * B_BYTES);
+  uint8_t* slabs = sB + STAGES * B_BYTES;
+  uint64_t* full = reinterpret_cast<uint64_t*>(slabs + epi_slab_bytes(BN));
   uint64_t* empty = full + STAGES;
-  uint64_t* tmem_full = empty + STAGES;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_full + 1);   // [0] TMEM base address, [1] split-K "this CTA is the last"
-  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 2) + 15) & ~(uintptr_t)15);
+  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(empty + STAGES) + 15) & ~(uintptr_t)15);
   __half* srb = reinterpret_cast<__half*>(sbias + BN);
+  float* acc = reinterpret_cast<float*>(smem);                // the operand ring, once the K loop is done
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) stamp(p, 0), stamp_ns(p, 16);
-  // cluster = (CTAS, 1, splits): ranks 2j and 2j + 1 are the pair of split j.  rank 0 = leader of its pair (issues the MMAs,
-  // owns the full barriers)
-  const uint32_t crank = cluster_ctarank();
-  const uint32_t rank = CTAS == 2 ? (crank & 1u) : 0u;
-  const uint16_t pair_mask = (uint16_t)(3u << (crank & ~1u));
-  const int m0 = CTAS == 2 ? (blockIdx.x >> 1) * (2 * BM) + (int)rank * BM : blockIdx.x * BM;
-  const int n0 = blockIdx.y * BN, bz = blockIdx.z;
+  const int bz = blockIdx.z;
   const int nk = p.conv ? p.ctaps * p.cblocks : (p.K + BK - 1) / BK;
-  // split-K: blockIdx.z owns k-blocks [kb0, kb1) and adds its partial tile into the fp32 workspace
+  // split-K: blockIdx.z owns k-blocks [kb0, kb1) and stores its partial tile into its plane of the fp32 workspace
+  const bool split = MODE == 3 && p.splits > 1;
   int kb0 = 0, kb1 = nk;
-  if (MODE == 3 && p.splits > 1) {
+  if (split) {
     kb0 = (int)((int64_t)nk * bz / p.splits);
     kb1 = (int)((int64_t)nk * (bz + 1) / p.splits);
   }
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    for (int s = 0; s < STAGES; ++s) mbar_init(full + s, 1), mbar_init(empty + s, 1);
-    mbar_init(tmem_full, 1);
+    for (int s = 0; s < STAGES; ++s) mbar_init(full + s, 1), mbar_init(empty + s, 2);   // empty: one arrival per MMA warpgroup
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {  // TMEM: TCOLS fp32 columns x 128 lanes (pair: the same warp of BOTH CTAs allocates the pair's columns)
-    if (CTAS == 2) {
-      asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TCOLS));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-    } else {
-      asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(TCOLS));
-      asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  if (CTAS == 2) cluster_sync_all();   // barrier inits of the leader must be visible before the peer's TMA can complete on them
-  else __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
+  __syncthreads();
   pdl_wait();      // everything above touched no global memory: it overlaps the tail of the previous kernel
   pdl_trigger();
   if (threadIdx.x == 0) stamp(p, 1);
 
-  if (warp == 0) {
-    if (lane == 0) {  // ---------------- TMA producer: own 128 rows of A, own BROWS rows of the B tile
+  // Tiles of this CTA: one (blockIdx.x, blockIdx.y), or -- persistent launch (p.persist, staged epilogues only) -- tiles
+  // blockIdx.x, blockIdx.x + gridDim.x, ... of the column-major tile order.  The ring's stage / phase counters run on across
+  // tiles, so the producer fills the next tile's first stages as soon as the epilogue has handed the ring back.
+  const int tiles_m = (p.M + BM - 1) / BM, tiles = tiles_m * ((p.N + BN - 1) / BN);
+  const bool persist = MODE != 3 && p.persist;
+  uint32_t cnt = 0;   // k-blocks consumed so far by this CTA
+  for (int t = persist ? blockIdx.x : blockIdx.y * tiles_m + blockIdx.x; t < tiles; t += persist ? gridDim.x : tiles) {
+  const int m0 = (t % tiles_m) * BM, n0 = (t / tiles_m) * BN;
+  if (warp < 4) {
+    if (threadIdx.x == 0) {  // ---------------- TMA producer
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the epilogue's generic accesses to the ring come first
       for (int kb = kb0; kb < kb1; ++kb) {
-        const int s = (kb - kb0) % STAGES;
-        const uint32_t ph = ((kb - kb0) / STAGES) & 1;
+        const uint32_t c = cnt + (kb - kb0);
+        const int s = c % STAGES;
+        const uint32_t ph = (c / STAGES) & 1;
         mbar_wait(empty + s, ph ^ 1, p, WAIT_EMPTY, s);
-        produce_stage<CTAS, BROWS>(p, &tmA, &tmB, sA + s * A_BYTES, sB + s * B_BYTES, full + s, kb, m0, n0, rank, bz);
+        produce_stage<BN>(p, &tmA, &tmB, sA + s * A_BYTES, sB + s * B_BYTES, full + s, kb, m0, n0, bz);
         if (kb == kb0) stamp(p, 2);
       }
       stamp(p, 3);
     }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {  // ---------------- MMA issuer (pair: the leader only, M = 256 across the pair)
-      constexpr uint32_t idesc = umma_idesc_f16(CTAS * BM, BN);
-      for (int kb = kb0; kb < kb1; ++kb) {
-        const int s = (kb - kb0) % STAGES;
-        const uint32_t ph = ((kb - kb0) / STAGES) & 1;
-        mbar_wait(full + s, ph, p, WAIT_FULL, s);
-        if (kb == kb0) stamp(p, 4);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t a0 = smem_u32(sA + s * A_BYTES), b0 = smem_u32(sB + s * B_BYTES);
-#pragma unroll
-        for (int k = 0; k < BK / 16; ++k)   // advancing 16 fp16 along K inside the 128-byte swizzle atom = +32 bytes on the start address
-          umma_f16<CTAS>(tmem_base, umma_desc_sw128(a0 + k * 32), umma_desc_sw128(b0 + k * 32), idesc, ((kb - kb0) | k) != 0);
-        umma_commit<CTAS>(empty + s, pair_mask);   // frees this stage (pair: in both CTAs) once these MMAs have read it
-      }
-      umma_commit<CTAS>(tmem_full, pair_mask);     // accumulator complete: the epilogue warps (pair: of both CTAs) may start
-      stamp(p, 5);
-    }
-  } else {  // ------------------------ epilogue warps 2..9 on this CTA's 128 accumulator rows
-    const int e = warp - 2, quarter = warp & 3, te = threadIdx.x - 64;
+    __syncwarp();
+  } else {  // ------------------------ warpgroups 1 and 2: MMAs on rows [64 wg, 64 wg + 64), then the epilogue
+    const int wg = (warp >> 2) - 1, e = warp - 4, quarter = e & 3, te = threadIdx.x - 128;
     const int c_lo = e < 4 ? 0 : CSPLIT, c_hi = e < 4 ? CSPLIT : BN;   // this warp's tile columns
     const int row0 = m0 + quarter * 32;
-    const uint32_t tmem_row_base = tmem_base + ((uint32_t)(quarter * 32) << 16);
+    if (MODE != 3) epilogue_preload<BN>(p, m0, n0, sbias, srb, te);
+    {
+      float d[BN / 2];
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+      for (int kb = kb0; kb < kb1; ++kb) {
+        const uint32_t c = cnt + (kb - kb0);
+        const int s = c % STAGES;
+        const uint32_t ph = (c / STAGES) & 1;
+        mbar_wait(full + s, ph, p, WAIT_FULL, s);
+        if (kb == kb0 && te == 0) stamp(p, 4);
+        const uint32_t a0 = smem_u32(sA + s * A_BYTES) + wg * (64 * 128), b0 = smem_u32(sB + s * B_BYTES);
+        wg::fence();
+#pragma unroll
+        for (int k = 0; k < BK / 16; ++k)   // advancing 16 fp16 along K inside the 128-byte swizzle atom = +32 bytes on the start address
+          wg::mma_f16<BN>(d, wg::desc_sw128(a0 + k * 32), wg::desc_sw128(b0 + k * 32), 1);
+        wg::commit();
+        wg::wait<1>();                      // the previous stage's MMAs are done: hand that stage back to the producer
+        if (kb > kb0 && (threadIdx.x & 127) == 0) mbar_arrive(empty + (c - 1) % STAGES);
+      }
+      wg::wait<0>();
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty + (cnt + kb1 - kb0 - 1) % STAGES);
+      if (te == 0) stamp(p, 5);
+      epi_bar();                            // both warpgroups are done reading the ring: it becomes the accumulator tile
+      acc_store<BN>(acc, d, 64 * wg, threadIdx.x & 127);
+    }
+    epi_bar();
+    if (te == 0) stamp(p, 6);
+    const float* acc_row = acc + (quarter * 32 + lane) * acc_ld(BN);
     if (MODE != 3) {
-      epilogue_preload<BN>(p, m0, n0, sbias, srb, te);
       const WarpOut g = warp_out<MODE>(p, n0, c_lo, c_hi);
       uint4 resq[RES_PREFETCH];
       prefetch_residual(p, g, lane, row0, resq);
-      mbar_wait(tmem_full, 0, p, WAIT_ACC, 0);
-      if (threadIdx.x == 64) stamp(p, 6);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      // the operand ring is idle once the accumulator is complete: it becomes the output transpose buffer
-      epilogue_staged<BN, MODE>(p, g, tmem_row_base, smem + e * 32 * (CSPLIT * 2 + 16), lane, m0, row0, n0, c_lo, c_hi, sbias, srb, resq);
+      epilogue_staged<BN, MODE>(p, g, acc_row, slabs + e * 32 * (CSPLIT * 2 + 16), lane, m0, row0, n0, c_lo, c_hi, sbias, srb, resq);
     } else {
-      mbar_wait(tmem_full, 0, p, WAIT_ACC, 0);
-      if (threadIdx.x == 64) stamp(p, 6);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
       const int row = row0 + lane;
-      if (p.splits > 1) {
+      if (split) {
         if (te == 0) stamp_ns(p, 17);
 #pragma unroll 1
         for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
           uint32_t r[32];
-          tmem_ld32(tmem_row_base + c0, r);
+          acc_ld32(acc_row + c0, r);
           if (row < p.M) splitk_partial(p, r, bz, row, n0 + c0);
         }
         if (te == 0) stamp_ns(p, 18);
@@ -884,169 +801,27 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 #pragma unroll 1
         for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
           uint32_t r[32];
-          tmem_ld32(tmem_row_base + c0, r);
+          acc_ld32(acc_row + c0, r);
           if (row < p.M) epilogue_chunk(p, r, row, crow, n0 + c0);
         }
       }
     }
-    if (threadIdx.x == 64) stamp(p, 7);
+    if (te == 0) stamp(p, 7);
   }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  // pair: neither CTA may free TMEM / exit while the pair's MMAs or the peer's TMEM reads are in flight.
-  // split-K: the `splits` CTAs (pairs) of a tile form ONE cluster (co-scheduled by the hardware), so this barrier -- release /
-  // acquire at cluster scope -- also publishes every split's partial plane to its siblings.
-  const bool split = MODE == 3 && p.splits > 1;
-  if (CTAS == 2 || split) cluster_sync_all();
-  else __syncthreads();
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    if (CTAS == 2) asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TCOLS));
-    else asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TCOLS));
+  cnt += kb1 - kb0;
+  __syncthreads();   // the epilogue is done with the accumulator tile, slabs and bias slices: the ring is free for the next tile
   }
-  if (MODE == 3) {
-    if (split && warp >= 2) {   // every split finalizes its share of the 128 x BN block: sum of the planes + epilogue
-      if (threadIdx.x == 64) stamp_ns(p, 21, true);
-      splitk_finalize<BN>(p, m0, n0, bz, threadIdx.x - 64, reinterpret_cast<float*>(smem));
-      if (threadIdx.x == 64) stamp_ns(p, 22, true);
+  if (split) {
+    // the `splits` CTAs of a tile form ONE cluster (co-scheduled by the hardware): this barrier -- release / acquire at
+    // cluster scope -- publishes every split's partial plane to its siblings
+    cluster_sync_all();
+    if (warp >= 4) {   // every split finalizes its share of the 128 x BN block: sum of the planes + epilogue
+      if (threadIdx.x == 128) stamp_ns(p, 21, true);
+      splitk_finalize<BN>(p, blockIdx.x * BM, blockIdx.y * BN, bz, threadIdx.x - 128, reinterpret_cast<float*>(smem));
+      if (threadIdx.x == 128) stamp_ns(p, 22, true);
     }
   }
   if (threadIdx.x == 0) stamp(p, 8);
-}
-
-
-// ------------------------------------------------------------------------------------------------ the persistent kernel
-// Problems with MANY tiles (the batched sampler calls: M = 16 384 ... 65 536 rows): one CTA pair per SM pair walks tiles
-// pair, pair + n_pairs, ... with TWO accumulator buffers in TMEM, so that
-//   * the epilogue of tile i (TMEM -> registers -> bias / activation / GEGLU -> shared-memory transpose -> global) runs
-//     under the main loop of tile i + 1 -- on short-K problems (K = 320: five k-blocks) the epilogue is as long as the main
-//     loop, and a CTA per tile serialises them (two resident CTAs per SM hide only part of it: 190 us against cuBLAS's 103
-//     on the 65536 x 2560 x 320 GEGLU projection);
-//   * the producer runs ahead across tile borders (the ring never drains), and barrier set-up, TMEM allocation, tensor-map
-//     fetch and tear-down are paid once per SM instead of once per tile.
-// Accumulator hand-over: acc_full[b] (tcgen05.commit, multicast to the pair) MMA -> epilogue warps of both CTAs;
-// acc_free[b] on the LEADER, 16 arrivals (eight epilogue warps x two CTAs, remote arrive from the peer) epilogue -> MMA.
-// The output transpose has its own shared memory (the ring is never idle), bias / row-bias slices are double-buffered.
-// Pair tiles only (CTAS = 2), staged fp16 epilogues only (MODE 0 / 1 / 2): everything else takes gemm_tc_kernel.
-constexpr int persist_smem_bytes(int bn, int stages) {
-  return stages * (BM * BK * 2 + (bn / 2) * BK * 2) + epi_slab_bytes(bn) + (2 * stages + 4) * 8 + 16 + 2 * epi_smem_bytes(bn) + 1024;
-}
-
-template <int BN, int STAGES, int MODE>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc_persistent_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                          const __grid_constant__ GemmParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
-  constexpr int BROWS = BN / 2;
-  constexpr int A_BYTES = BM * BK * 2, B_BYTES = BROWS * BK * 2;
-  static_assert(B_BYTES % 1024 == 0, "stage bases must stay 1024-byte aligned for SWIZZLE_128B");
-  static_assert(MODE != 3, "staged epilogues only");
-  constexpr int TCOLS = tmem_cols(BN);                       // one accumulator buffer; two are allocated
-  static_assert(2 * TCOLS <= 512, "two accumulator buffers must fit the 512 TMEM columns");
-  constexpr int CSPLIT = col_split(BN);
-  uint8_t* sA = smem;
-  uint8_t* sB = smem + STAGES * A_BYTES;
-  uint8_t* slabs = sB + STAGES * B_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(slabs + epi_slab_bytes(BN));
-  uint64_t* empty = full + STAGES;
-  uint64_t* acc_full = empty + STAGES;
-  uint64_t* acc_free = acc_full + 2;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_free + 2);
-  float* sbias0 = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(tmem_slot + 2) + 15) & ~(uintptr_t)15);
-  constexpr int EPI_FLOATS = epi_smem_bytes(BN) / 4;         // one bias + row-bias buffer, in floats
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const uint32_t rank = crank & 1u;
-  const uint16_t pair_mask = (uint16_t)(3u << (crank & ~1u));
-  const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  const int tiles_n = (p.N + BN - 1) / BN;
-  const int ntiles = ((p.M + 2 * BM - 1) / (2 * BM)) * tiles_n;
-  const int nk = p.conv ? p.ctaps * p.cblocks : (p.K + BK - 1) / BK;
-
-  if (warp == 0 && lane == 0) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
-    asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
-    for (int s = 0; s < STAGES; ++s) mbar_init(full + s, 1), mbar_init(empty + s, 1);
-    for (int b = 0; b < 2; ++b) mbar_init(acc_full + b, 1), mbar_init(acc_free + b, 2 * EPI_WARPS);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)), "n"(2 * TCOLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  cluster_sync_all();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
-  pdl_wait();
-  pdl_trigger();
-
-  if (warp == 0) {
-    if (lane == 0) {  // ---------------- TMA producer: runs ahead across tile borders, bounded only by the ring
-      uint32_t cnt = 0;
-      for (int t = pair; t < ntiles; t += npairs) {
-        const int tm = t / tiles_n, n0 = (t - tm * tiles_n) * BN, m0 = tm * (2 * BM) + (int)rank * BM;
-        for (int kb = 0; kb < nk; ++kb, ++cnt) {
-          const int s = cnt % STAGES;
-          mbar_wait(empty + s, ((cnt / STAGES) & 1) ^ 1, p, WAIT_EMPTY, s);
-          produce_stage<2, BROWS>(p, &tmA, &tmB, sA + s * A_BYTES, sB + s * B_BYTES, full + s, kb, m0, n0, rank, 0);
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0 && rank == 0) {  // ---------------- MMA issuer (leader CTA): tile i into accumulator buffer i & 1
-      constexpr uint32_t idesc = umma_idesc_f16(2 * BM, BN);
-      uint32_t cnt = 0, it = 0;
-      for (int t = pair; t < ntiles; t += npairs, ++it) {
-        const uint32_t buf = it & 1;
-        mbar_wait(acc_free + buf, ((it >> 1) & 1) ^ 1, p, WAIT_ACC_FREE, (int)buf);   // both CTAs' epilogue warps have drained tile it - 2
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t acc = tmem_base + buf * TCOLS;
-        for (int kb = 0; kb < nk; ++kb, ++cnt) {
-          const int s = cnt % STAGES;
-          mbar_wait(full + s, (cnt / STAGES) & 1, p, WAIT_FULL, s);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint32_t a0 = smem_u32(sA + s * A_BYTES), b0 = smem_u32(sB + s * B_BYTES);
-#pragma unroll
-          for (int k = 0; k < BK / 16; ++k)
-            umma_f16<2>(acc, umma_desc_sw128(a0 + k * 32), umma_desc_sw128(b0 + k * 32), idesc, (kb | k) != 0);
-          umma_commit<2>(empty + s, pair_mask);
-        }
-        umma_commit<2>(acc_full + buf, pair_mask);
-      }
-    }
-  } else {  // ------------------------ epilogue warps 2..9: this CTA's 128 accumulator rows of every tile
-    const int e = warp - 2, quarter = warp & 3, te = threadIdx.x - 64;
-    const int c_lo = e < 4 ? 0 : CSPLIT, c_hi = e < 4 ? CSPLIT : BN;
-    uint8_t* slab = slabs + e * 32 * (CSPLIT * 2 + 16);
-    // the leader's acc_free barriers, as shared::cluster addresses (the peer arrives remotely)
-    uint32_t free_bar0;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(free_bar0) : "r"(smem_u32(acc_free)), "r"(crank & ~1u));
-    uint32_t it = 0;
-    for (int t = pair; t < ntiles; t += npairs, ++it) {
-      const uint32_t buf = it & 1;
-      const int tm = t / tiles_n, n0 = (t - tm * tiles_n) * BN, m0 = tm * (2 * BM) + (int)rank * BM;
-      const int row0 = m0 + quarter * 32;
-      float* sbias = sbias0 + buf * EPI_FLOATS;
-      __half* srb = reinterpret_cast<__half*>(sbias + BN);
-      epilogue_preload<BN>(p, m0, n0, sbias, srb, te);
-      const WarpOut g = warp_out<MODE>(p, n0, c_lo, c_hi);
-      uint4 resq[RES_PREFETCH];
-      prefetch_residual(p, g, lane, row0, resq);
-      mbar_wait(acc_full + buf, (it >> 1) & 1, p, WAIT_ACC, (int)buf);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tmem_row_base = tmem_base + buf * TCOLS + ((uint32_t)(quarter * 32) << 16);
-      epilogue_staged<BN, MODE>(p, g, tmem_row_base, slab, lane, m0, row0, n0, c_lo, c_hi, sbias, srb, resq, free_bar0 + buf * 8);
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  cluster_sync_all();   // neither CTA may free TMEM / exit while the pair's MMAs or the peer's TMEM reads are in flight
-  if (warp == 1) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(2 * TCOLS));
-  }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -1105,14 +880,14 @@ TrapRecord* diag_buffer(cudaStream_t st) {
 }
 
 struct Config {
-  int ctas, bn, splits;
-  int persist;   // 1: gemm_tc_persistent_kernel (pair tiles, staged epilogue, many tiles)
+  int bn, splits;
+  int persist;   // 1: persistent launch (at most one CTA per SM walks the tiles)
 };
 
-// tuning / sweep hook: O2345_GEMM_FORCE="ctas,bn,splits" (0 = keep the heuristic's choice for that field); also settable
-// through o2345_debug_gemm_force (tools/gemm_sweep.py)
+// tuning / sweep hook: O2345_GEMM_FORCE="ctas,bn,splits" (0 = keep the heuristic's choice for that field; ctas is 1, one CTA
+// per tile); also settable through o2345_debug_gemm_force (tools/gemm_sweep.py)
 int g_force[3] = {-1, 0, 0};
-int g_persist = 0;          // 0: heuristic, 1: persistent kernel wherever it is available, 2: never (o2345_debug_gemm_persist)
+int g_persist = 0;             // 0: heuristic, 1: persistent launch wherever available, 2: never (o2345_debug_gemm_persist)
 int g_persist_min_tiles = 0;   // heuristic threshold override (0: default)
 void read_force_env() {
   if (g_force[0] >= 0) return;
@@ -1121,34 +896,32 @@ void read_force_env() {
   if (e) sscanf(e, "%d,%d,%d", &g_force[0], &g_force[1], &g_force[2]);
 }
 
-// Tile shape and k-splits for a problem of M x N with nk k-blocks of 64: the candidate with the lowest predicted time under a
-// small cost model fitted to tools/gemm_sweep.py (63 UNet shapes x ~40 forced configurations each on a B200, cold L2;
-// profiles/r2_gemm_sweep.txt: the model's picks total 3.23 ms against 3.18 ms for the per-shape optimum):
+// Tile width and k-splits for a problem of M x N with nk k-blocks of 64: the candidate with the lowest predicted time under a
+// small cost model (its constants are starting values, not yet fitted on an H100 with tools/gemm_sweep.py):
 //   * a launch costs ~5 us of fixed latency (launch, prologue, first TMA round trip, tear-down) + ~3 us of epilogue per
-//     160 columns of tile and wave of 296 CTAs;
-//   * the main loop is bound by operand delivery, not by the tensor pipe: an SM ingests ~40 B/clk (60 when two CTAs share it
-//     and cover each other's bubbles), the whole L2 -> SM fabric ~6 300 B/clk -- so few fat tiles starve (few SMs pull),
-//     many thin tiles re-read A (fabric), and long-K problems with few tiles want split-K;
+//     160 columns of tile and wave of CTAs;
+//   * the main loop is bound by operand delivery or by the tensor pipe (a 128 x BN x 64 k-block is 4 BN cycles of wgmma at
+//     ~2 048 fp16 FMA per clock and SM): an SM ingests ~40 B/clk, the whole L2 -> SM fabric ~6 300 B/clk -- so few fat tiles
+//     starve (few SMs pull), many thin tiles re-read A (fabric), and long-K problems with few tiles want split-K;
 //   * split-K adds ~4 us + ~1 us per split and 128 tile columns (partial planes through L2, cluster barrier, finalize).
 float g_model[7] = {40.f, 0.5f, 6300.f, 5.f, 3.f, 4.f, 1.f};   // bw_sm, alpha, cap, fixed, epi, so0, so1 (tools: o2345_debug_gemm_model)
-float predict_us(int M, int N, int nk, int ctas, int bn, int splits) {
+float predict_us(int M, int N, int nk, int bn, int splits) {
   const float bw_sm = g_model[0], alpha = g_model[1], cap = g_model[2], fixed = g_model[3], epi = g_model[4], so0 = g_model[5],
-              so1 = g_model[6], cyc_per_us = 1900.f;
-  const int mblocks = ctas == 2 ? 2 * cdiv(M, 2 * BM) : cdiv(M, BM);
-  const int tiles = mblocks * cdiv(N, bn);
+              so1 = g_model[6], cyc_per_us = 1750.f;
+  const int tiles = cdiv(M, BM) * cdiv(N, bn);
   const int n = tiles * splits;
   const int kb = cdiv(nk, splits);
-  const float bytes_cta = (float)kb * (float)(BM * BK * 2 + (bn / ctas) * BK * 2);
+  const float bytes_cta = (float)kb * (float)(BM * BK * 2 + bn * BK * 2);
   const int sms = sm_count();
   const int rounds = cdiv(n, sms);
   float f = (float)(n - sms) / (float)sms;
   f = f < 0.f ? 0.f : (f > 1.f ? 1.f : f);
   const float t_sm = (float)rounds * bytes_cta / (bw_sm * (1.f + alpha * f));
   const float t_fabric = (float)n * bytes_cta / cap;
-  const float t_mma = (float)rounds * (float)kb * 4.f * ((float)bn * 0.5f);
+  const float t_mma = (float)rounds * (float)kb * 4.f * (float)bn;
   float t = t_sm > t_fabric ? t_sm : t_fabric;
   if (t_mma > t) t = t_mma;
-  float us = fixed + t / cyc_per_us + epi * (float)bn / 160.f * (float)cdiv(n, 2 * sms);
+  float us = fixed + t / cyc_per_us + epi * (float)bn / 160.f * (float)cdiv(n, sms);
   if (splits > 1) us += so0 + so1 * (float)splits * (float)bn / 128.f;
   return us;
 }
@@ -1159,49 +932,35 @@ Config pick_config(const GemmParams& p, int nk, bool can_split, int64_t ws_float
   const int M = p.M, N = p.N;
   c.persist = 0;
   if (p.batched) {
-    c.ctas = 1, c.bn = N <= 64 ? 64 : 128, c.splits = 1;
+    c.bn = N <= 64 ? 64 : 128, c.splits = 1;
     return c;
   }
   static const int kBn[4] = {64, 128, 160, 256};
-  static const int kSplits[8] = {1, 2, 3, 4, 6, 8, 12, 16};
+  static const int kSplits[6] = {1, 2, 3, 4, 6, 8};
   const bool split_ok = can_split && p.act != 3 && p.ws && 2 * (int64_t)M * N <= ws_floats;
   const int max_planes = split_ok ? (int)(ws_floats / ((int64_t)M * N)) : 1;
   float best = 1e30f;
-  c.ctas = 2, c.bn = 128, c.splits = 1;
-  for (int ctas = 1; ctas <= 2; ++ctas) {
-    if (ctas == 1 && M > 2 * BM) continue;                      // single-CTA tiles only pay for short problems
-    if ((g_force[0] == 1 || g_force[0] == 2) && ctas != g_force[0]) continue;
-    for (int bi = 0; bi < 4; ++bi) {
-      const int bn = kBn[bi];
-      if (ctas == 1 && bn > 128) continue;
-      if (bn > 64 && N <= 64) continue;
-      if (g_force[1] > 0 && bn != g_force[1]) continue;
-      for (int si = 0; si < 8; ++si) {
-        const int sp = kSplits[si];
-        if (g_force[2] > 0 && sp != (g_force[2] > nk ? nk : g_force[2])) continue;
-        if (sp > 1 && (!split_ok || sp > max_planes || sp * ctas > MAX_CLUSTER || nk / sp < 3)) continue;
-        const float us = predict_us(M, N, nk, ctas, bn, sp);
-        if (us < best) best = us, c.ctas = ctas, c.bn = bn, c.splits = sp;
-      }
+  c.bn = 128, c.splits = 1;
+  for (int bi = 0; bi < 4; ++bi) {
+    const int bn = kBn[bi];
+    if (bn > 64 && N <= 64) continue;
+    if (g_force[1] > 0 && bn != g_force[1]) continue;
+    for (int si = 0; si < 6; ++si) {
+      const int sp = kSplits[si];
+      if (g_force[2] > 0 && sp != (g_force[2] > nk ? nk : g_force[2])) continue;
+      if (sp > 1 && (!split_ok || sp > max_planes || sp > MAX_CLUSTER || nk / sp < 3)) continue;
+      const float us = predict_us(M, N, nk, bn, sp);
+      if (us < best) best = us, c.bn = bn, c.splits = sp;
     }
   }
   if (best > 1e29f) {   // a forced configuration that is not available: fall back to the nearest valid one
-    c.ctas = (g_force[0] == 1) ? 1 : 2;
-    c.bn = (g_force[1] == 64 || g_force[1] == 128 || (c.ctas == 2 && (g_force[1] == 160 || g_force[1] == 256))) ? g_force[1] : 128;
+    c.bn = (g_force[1] == 64 || g_force[1] == 128 || g_force[1] == 160 || g_force[1] == 256) ? g_force[1] : 128;
     c.splits = 1;
   }
-  // Many tiles and a short K (the batched sampler calls: M = 16 384 ... 65 536): the epilogue of a tile is as long as its main
-  // loop, and the persistent kernel hides it under the next tile's.  Measured per shape (tools/gemm_persist_ab.py, B200):
-  // 65536 x 2560 x 320 GEGLU 184 -> 157 us, 65536 x 960 x 320 75 -> 59, 65536 x 320 x 1280 85 -> 63, 16384 x 1920 x 640 51 -> 38;
-  // with long K it LOSES (65536 x 320 x 2880 conv 111 -> 141 us): one CTA per SM keeps 128-156 KB of operands in flight
-  // against 192-208 KB for two resident per-tile CTAs, and the main loop is bound by bytes in flight.
-  if (g_persist == 0 && g_force[0] == 0 && g_force[1] == 0 && g_force[2] == 0 && !p.out_f32 && nk <= 20) {
-    // tile width: 256 where it divides the work well, 160 for the UNet's N = 320 / 640 / 960, 128 for N = 128 (the VAE's top level)
-    const int bn_p = (N >= 512 || N == 256) ? 256 : ((N % 160) == 0 || N > 128) ? 160 : 128;
-    const int tiles = cdiv(M, 2 * BM) * cdiv(N, bn_p);
-    const int min_tiles = g_persist_min_tiles > 0 ? g_persist_min_tiles : sm_count() / 2;
-    if (N >= 128 && tiles >= min_tiles && (N >= 512 || nk >= 8)) c.ctas = 2, c.bn = bn_p, c.splits = 1, c.persist = 1;
-  }
+  // Many waves of tiles: one CTA per SM walks them, so that launch, prologue and the wave tail are paid once per SM
+  const int tiles = cdiv(M, BM) * cdiv(N, c.bn);
+  const int min_tiles = g_persist_min_tiles > 0 ? g_persist_min_tiles : 4 * sm_count();
+  c.persist = c.splits == 1 && (g_persist == 1 || (g_persist == 0 && tiles >= min_tiles));
   return c;
 }
 
@@ -1209,104 +968,62 @@ Config pick_config(const GemmParams& p, int nk, bool can_split, int64_t ws_float
 int pick_mode(const GemmParams& p, const Config& c) {
   const int nout = p.act == 3 ? p.N / 2 : p.N;
   const bool staged = !p.out_f32 && c.splits <= 1 && !p.batched && (nout % 8) == 0 && (p.ldc % 8) == 0 && ((uintptr_t)p.C % 16) == 0 &&
-                      (!p.residual || ((uintptr_t)p.residual % 16) == 0) && !(c.ctas == 1 && p.act == 3);
+                      (!p.residual || ((uintptr_t)p.residual % 16) == 0);
   if (!staged) return 3;
   return p.act == 0 ? 0 : (p.act == 3 ? 1 : 2);
 }
 
-// The persistent kernel (mode 0 / 1 / 2 epilogues, pair tiles): chosen by pick_config for many-tile short-K problems, or forced
-// by the tuning hook wherever it is available.
-bool pick_persist(const Config& c, int mode) {
-  if (g_persist == 2 || mode == 3 || c.ctas != 2 || c.splits > 1 || c.bn < 128) return false;
-  return g_persist == 1 || c.persist == 1;
-}
-
 long long* g_trace = nullptr;
 
-template <int BN, int STAGES, int CTAS, int MODE>
-int launch(const CUtensorMap& a, const CUtensorMap& b, GemmParams p, int batch, cudaStream_t st) {
-  constexpr int SMEM = smem_bytes(BN, STAGES, CTAS);
-  static_assert(2 * SMEM <= 227 * 1024 + 2048, "two CTAs per SM");
-  static PerDeviceOnce attr;
-  if (attr.need()) {
-    O2345_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, CTAS, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-    if (MODE == 3)   // split-K clusters of up to 16 CTAs
-      O2345_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, CTAS, MODE>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
-  }
-  p.bn = BN, p.ctas = CTAS, p.mode = MODE;
-  p.diag = diag_buffer(st);
-  const int mblocks = CTAS == 2 ? 2 * cdiv(p.M, 2 * BM) : cdiv(p.M, BM);
-  const int splits = (MODE == 3 && batch == 0 && p.splits > 1) ? p.splits : 1;
-  p.splits = splits;
-  dim3 grid(mblocks, cdiv(p.N, BN), batch > 0 ? batch : splits);
-  O2345_CUDA(launch_pdl_cluster(gemm_tc_kernel<BN, STAGES, CTAS, MODE>, grid, dim3(GEMM_THREADS), (size_t)SMEM, st, CTAS, splits, a, b, p));
-  O2345_LAUNCH_CHECK();
-  return O2345_OK;
-}
-
 template <int BN, int STAGES, int MODE>
-int launch_persistent(const CUtensorMap& a, const CUtensorMap& b, GemmParams p, cudaStream_t st) {
-  constexpr int SMEM = persist_smem_bytes(BN, STAGES);
+int launch(const CUtensorMap& a, const CUtensorMap& b, GemmParams p, int batch, int persist, cudaStream_t st) {
+  constexpr int SMEM = smem_bytes(BN, STAGES);
   static_assert(SMEM <= 227 * 1024, "one CTA per SM");
   static PerDeviceOnce attr;
   if (attr.need())
-    O2345_CUDA(cudaFuncSetAttribute(gemm_tc_persistent_kernel<BN, STAGES, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
-  p.bn = BN, p.ctas = 2, p.mode = MODE + 10;
+    O2345_CUDA(cudaFuncSetAttribute(gemm_tc_kernel<BN, STAGES, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
+  p.bn = BN, p.mode = MODE;
   p.diag = diag_buffer(st);
-  p.splits = 1;
-  const int tiles = cdiv(p.M, 2 * BM) * cdiv(p.N, BN), pairs = sm_count() / 2;
-  dim3 grid(2 * (tiles < pairs ? tiles : pairs), 1, 1);
-  O2345_CUDA(launch_pdl_cluster(gemm_tc_persistent_kernel<BN, STAGES, MODE>, grid, dim3(GEMM_THREADS), (size_t)SMEM, st, 2, 1, a, b, p));
+  const int splits = (MODE == 3 && batch == 0 && p.splits > 1) ? p.splits : 1;
+  p.splits = splits;
+  dim3 grid(cdiv(p.M, BM), cdiv(p.N, BN), batch > 0 ? batch : splits);
+  p.persist = MODE != 3 && batch == 0 && splits == 1 && persist;
+  if (p.persist) {
+    const int tiles = (int)grid.x * (int)grid.y;
+    grid = dim3(tiles < sm_count() ? tiles : sm_count(), 1, 1);
+  }
+  O2345_CUDA(launch_pdl_cluster(gemm_tc_kernel<BN, STAGES, MODE>, grid, dim3(GEMM_THREADS), (size_t)SMEM, st, 1, splits, a, b, p));
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }
 
 template <int BN, int STAGES>
-int launch_persistent_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, cudaStream_t st) {
+int launch_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, int batch, int persist, cudaStream_t st) {
   switch (mode) {
-    case 0: return launch_persistent<BN, STAGES, 0>(a, b, p, st);
-    case 1: return launch_persistent<BN, STAGES, 1>(a, b, p, st);
-    default: return launch_persistent<BN, STAGES, 2>(a, b, p, st);
+    case 0: return launch<BN, STAGES, 0>(a, b, p, batch, persist, st);
+    case 1: return launch<BN, STAGES, 1>(a, b, p, batch, persist, st);
+    case 2: return launch<BN, STAGES, 2>(a, b, p, batch, persist, st);
+    default: return launch<BN, STAGES, 3>(a, b, p, batch, persist, st);
   }
 }
 
-template <int BN, int STAGES, int CTAS>
-int launch_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, int batch, cudaStream_t st) {
-  switch (mode) {
-    case 0: return launch<BN, STAGES, CTAS, 0>(a, b, p, batch, st);
-    case 1:
-      if constexpr (CTAS == 2) return launch<BN, STAGES, 2, 1>(a, b, p, batch, st);
-      else return launch<BN, STAGES, CTAS, 3>(a, b, p, batch, st);
-    case 2: return launch<BN, STAGES, CTAS, 2>(a, b, p, batch, st);
-    default: return launch<BN, STAGES, CTAS, 3>(a, b, p, batch, st);
-  }
-}
-
+// ring depth per tile width: as many stages as fit next to the epilogue slabs in 227 KB (one CTA per SM)
 int dispatch(const Config& c, int mode, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, int batch, cudaStream_t st) {
   if (p.colstats && mode == 3 && c.splits <= 1) {
     set_error("o2345_gemm_f16: column statistics need the staged fp16 epilogue (16-byte aligned C / residual) or split-K");
     return O2345_EUNSUPPORTED;
   }
-  if (pick_persist(c, mode)) {
-    if (c.bn == 128) return launch_persistent_mode<128, 6>(mode, a, b, p, st);
-    if (c.bn == 160) return launch_persistent_mode<160, 6>(mode, a, b, p, st);
-    return launch_persistent_mode<256, 4>(mode, a, b, p, st);
-  }
-  if (c.ctas == 2) {
-    if (c.bn == 64) return launch_mode<64, 5, 2>(mode, a, b, p, batch, st);
-    if (c.bn == 128) return launch_mode<128, 4, 2>(mode, a, b, p, batch, st);
-    if (c.bn == 160) return launch_mode<160, 4, 2>(mode, a, b, p, batch, st);
-    return launch_mode<256, 3, 2>(mode, a, b, p, batch, st);
-  }
-  if (c.bn == 64) return launch_mode<64, 4, 1>(mode, a, b, p, batch, st);
-  return launch_mode<128, 3, 1>(mode, a, b, p, batch, st);
+  if (c.bn == 64) return launch_mode<64, 6>(mode, a, b, p, batch, c.persist, st);
+  if (c.bn == 128) return launch_mode<128, 5>(mode, a, b, p, batch, c.persist, st);
+  if (c.bn == 160) return launch_mode<160, 4>(mode, a, b, p, batch, c.persist, st);
+  return launch_mode<256, 3>(mode, a, b, p, batch, c.persist, st);
 }
 
 int fill_epilogue(GemmParams& p, const o2345_epilogue* ep, int M, int N, int64_t ldc) {
   p.bias = nullptr, p.rowbias = nullptr, p.rowbias_ld = 0, p.rows_per_group = 1, p.residual = nullptr;
   p.out_f32 = 0, p.act = 0, p.alpha = 1.f, p.trace = g_trace;
   p.colstats = nullptr, p.stats_rpg = 1, p.stats_groups = 0;
-  p.diag = nullptr, p.bn = p.ctas = p.mode = 0;
+  p.diag = nullptr, p.bn = p.mode = 0;
   if (!ep) return O2345_OK;
   O2345_CHECK_ARG(ep->act >= 0 && ep->act <= 4, "unknown activation");
   O2345_CHECK_ARG(!ep->rowbias || (ep->rows_per_group > 0 && (ep->rowbias_ld % 8) == 0 && ((uintptr_t)ep->rowbias % 16) == 0),
@@ -1353,13 +1070,12 @@ extern "C" int o2345_last_trap(char* buf, size_t n) {
   const TrapRecord* d = g_diag;
   if (!d || d->magic != TRAP_MAGIC) return 0;
   static const char* names[] = {"?", "empty (producer waiting for the MMA to free a stage)", "full (MMA issuer waiting for TMA bytes)",
-                                "accumulator (epilogue waiting for the last MMA)",
-                                "accumulator buffer (MMA issuer waiting for the epilogue warps to drain it)"};
+                                };
   snprintf(buf, n,
-           "gemm_tc_kernel<BN=%d, CTAS=%d, MODE=%d> M=%d N=%d K=%d conv=%d splits=%d: CTA (%d,%d,%d) rank %d gave up after 4 s "
+           "gemm_tc_kernel<BN=%d, MODE=%d> M=%d N=%d K=%d conv=%d splits=%d: CTA (%d,%d,%d) rank %d gave up after 4 s "
            "on barrier '%s' stage %d",
-           d->bn, d->ctas, d->mode, d->M, d->N, d->K, d->conv, d->splits, d->bx, d->by, d->bz, d->rank,
-           names[d->tag >= 1 && d->tag <= 4 ? d->tag : 0], d->stage);
+           d->bn, d->mode, d->M, d->N, d->K, d->conv, d->splits, d->bx, d->by, d->bz, d->rank,
+           names[d->tag >= 1 && d->tag <= 2 ? d->tag : 0], d->stage);
   return 1;
 }
 
@@ -1394,7 +1110,7 @@ int conv_launch(const void* x, int B, int H, int W, int C, const void* weight, i
   set_workspace(p, splitk_ws, ws_floats);
   const Config c = pick_config(p, taps * p.cblocks, true, ws_floats);
   p.splits = c.splits;
-  rc = make_map(&mb, weight, N, taps * (int64_t)C, taps * (int64_t)C, 0, 0, 0, 0, c.bn / c.ctas);
+  rc = make_map(&mb, weight, N, taps * (int64_t)C, taps * (int64_t)C, 0, 0, 0, 0, c.bn);
   if (rc) return rc;
   return dispatch(c, pick_mode(p, c), ma, mb, p, 0, st);
 }
@@ -1464,7 +1180,7 @@ extern "C" int o2345_gemm_f16(const void* A, const void* B, void* C, int M, int 
   CUtensorMap ma, mb;
   rc = make_map(&ma, A, M, K, lda, nh, nb, stride_a_h, stride_a_b, BM);
   if (rc) return rc;
-  rc = make_map(&mb, B, N, K, ldb, nh, nb, stride_b_h, stride_b_b, c.bn / c.ctas);
+  rc = make_map(&mb, B, N, K, ldb, nh, nb, stride_b_h, stride_b_b, c.bn);
   if (rc) return rc;
   return dispatch(c, pick_mode(p, c), ma, mb, p, nh > 0 ? nh * nb : 0, st);
 }

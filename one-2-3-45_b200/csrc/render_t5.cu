@@ -1,17 +1,18 @@
-// View-blending network on the 5th-generation tensor cores (tcgen05.mma, accumulators in TMEM): precision = O2345_BLEND_TC5.
-// SURVEY.md rows B11 / B12, the hot kernel of the ray march (section 8(d)); same function as render_blend_kernel (render.cu,
-// reference reconstruction/models/rendering_network.py:75-129 fused with the Projector's per-view fetch, projector.py:96-228).
+// View-blending network on the Hopper warpgroup MMA (wgmma.mma_async, fp32 accumulators in registers): precision =
+// O2345_BLEND_TC5.  SURVEY.md rows B11 / B12, the hot kernel of the ray march (section 8(d)); same function as
+// render_blend_kernel (render.cu, reference reconstruction/models/rendering_network.py:75-129 fused with the Projector's
+// per-view fetch, projector.py:96-228).
 //
-// Round 1 ran the per-(sample, view) MLPs as register-chained mma.sync products (render_tc.cu): 4 580 warp instructions per
-// sample, 100 KB of SASS, instruction-fetch / issue bound at 15 % tensor pipe.  Here a CTA owns a 128-row tile = 4 samples x
-// 32 view slots: a warp is one sample and a LANE IS ONE SOURCE VIEW, which is also TMEM lane = accumulator row, so
+// The per-(sample, view) MLPs as register-chained mma.sync products (render_tc.cu) are instruction-fetch / issue bound.  Here a
+// CTA -- one warpgroup -- owns a 128-row tile = 4 samples x 32 view slots: a warp is one sample and a LANE IS ONE SOURCE VIEW,
+// which is also the accumulator row it reads back, so
 //   * the projection, the validity mask, the ray difference, the pooling weight and every per-sample reduction over the views
 //     (weighted mean / variance, soft-max) are plain per-lane values and warp shuffles -- no compaction, no fragment layouts;
 //   * each thread gathers the 59 channels of ITS view (4 bilinear taps x 240 contiguous bytes) into registers;
-//   * the seven wide layers (16->64, 64->64, 64->32, 32->32, 32->33, 32->32, 37->16) are tcgen05.mma M = 128 products: the
-//     thread writes its fp16 activation row into a SWIZZLE_128B shared-memory operand, one elected thread of a fifth warp
-//     issues the MMAs against weights resident in shared memory, tcgen05.commit signals an mbarrier, and each thread reads
-//     back ITS row of the accumulator with tcgen05.ld; the narrow layers (4->16, 32->1, 16->8->1) stay on the FMA pipe;
+//   * the seven wide layers (16->64, 64->64, 64->32, 32->32, 32->33, 32->32, 37->16) are M = 128 wgmma products (two m64
+//     instructions per k-step): the thread writes its fp16 activation row into a SWIZZLE_128B shared-memory operand, the
+//     warpgroup multiplies it by weights resident in shared memory, the accumulator fragments go to an fp32 row buffer and
+//     each thread reads back ITS row; the narrow layers (4->16, 32->1, 16->8->1) stay on the FMA pipe;
 //   * the per-sample part of base_fc ([geo | mean | var] -> 64, identical for the 32 views) is computed once per sample and
 //     added when the accumulator is read.
 // Numerics as render_tc.cu: features, statistics, soft-max and the colour blend in fp32, MMA operands rounded to fp16.
@@ -19,13 +20,14 @@
 
 #include "common.cuh"
 #include "render_pack.cuh"
+#include "wgmma.cuh"
 
 namespace o2345 {
 namespace {
 using namespace rpack;
 
-constexpr int T5_THREADS = 160;          // warps 0..3: one sample each (lane = view); warp 4: TMEM allocation + MMA issue
-constexpr int ST_LD = 61;                // floats per row of the fp32 feature staging (odd stride: conflict-free row writes)
+constexpr int T5_THREADS = 128;          // one warpgroup; warp = sample, lane = view
+constexpr int ST_LD = 65;                // floats per row of the fp32 accumulator / feature rows (odd stride: conflict-free row access)
 
 // ---- shared memory map (bytes from the 1024-byte aligned base)
 constexpr int W_D1 = 0;                      // ray_dir_fc[2]   [64 n][64 k] (k < 16 used)  SWIZZLE_128B K-major
@@ -42,14 +44,13 @@ constexpr int S_F32 = S_PS + 134 * 64 * 2;   // small fp32 vectors (below)
 constexpr int F_D0W = 0, F_D0B = 64, F_D1B = 80, F_B0B = 144, F_B1B = 208, F_V0B = 240, F_V1B = 272 /* 32 + visibility bias */,
               F_U0B = 320, F_U1W = 352, F_U1B = 384, F_R0B = 388, F_R1W = 404 /* [16][8] */, F_R1B = 532, F_R2W = 540, F_R2B = 548,
               F_S = 549, F_TOTAL = 552;
-constexpr int S_STAGE = S_F32 + F_TOTAL * 4;             // per-warp fp32 feature rows [32][ST_LD]
+constexpr int S_STAGE = S_F32 + F_TOTAL * 4;             // fp32 rows [128][ST_LD]: the accumulator of a round, a warp's features
 constexpr int S_VEC = S_STAGE + 4 * 32 * ST_LD * 4;      // per-warp [134] geo|mean|var + [64] per-sample base_fc part + [32] pooling weights
 constexpr int VEC_F = 134 + 64 + 32 + 2;
-constexpr int S_BAR = S_VEC + 4 * VEC_F * 4;             // mbarrier (8 bytes) + TMEM base (4 bytes)
-constexpr int T5_SMEM = S_BAR + 16 + 1024;               // + alignment slack
+constexpr int T5_SMEM = S_VEC + 4 * VEC_F * 4 + 1024;   // + alignment slack
 static_assert(A_BUF % 1024 == 0 && W_B0 % 1024 == 0 && W_B1 % 1024 == 0 && W_V0 % 1024 == 0 && W_V1 % 1024 == 0 && W_U0 % 1024 == 0 &&
               W_R0 % 1024 == 0, "SWIZZLE_128B operands start on 1024-byte boundaries");
-static_assert(S_F32 % 16 == 0 && S_STAGE % 4 == 0 && S_BAR % 8 == 0, "alignment");
+static_assert(S_F32 % 16 == 0 && S_STAGE % 4 == 0, "alignment");
 static_assert(2 * T5_SMEM <= 227 * 1024, "two CTAs per SM");
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -79,53 +80,11 @@ __device__ __forceinline__ float warp_max(float v) {
 __device__ __forceinline__ uint32_t sw128_off(int row, int k) {
   return (uint32_t)((row >> 3) * 1024 + (row & 7) * 128 + ((((k >> 3) ^ (row & 7))) << 4) + ((k & 7) << 1));
 }
-// UMMA shared-memory descriptor of such an operand (cute::UMMA::SmemDescriptor: start >> 4, LBO ignored, SBO 1024 B, version 1,
-// SWIZZLE_128B) and the kind::f16 instruction descriptor (D f32, A = B = f16, K-major, N >> 3 at bit 17, M >> 4 at bit 24)
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)1 << 16;
-  d |= (uint64_t)(1024 >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-  return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t r[32];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// the first NC columns of this thread's accumulator row
+template <int NC>
+__device__ __forceinline__ void acc_row(const float* row, float (&v)[NC]) {
 #pragma unroll
-  for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+  for (int i = 0; i < NC; ++i) v[i] = row[i];
 }
 
 // fp32 [in][out] pack -> fp16 [n][64] SWIZZLE_128B operand; rows >= n_used / columns >= k_used are zero
@@ -151,47 +110,30 @@ __device__ __forceinline__ void write_row(uint8_t* abuf, int row, const float (&
   }
 }
 
-struct Round {
-  uint64_t* bar;
-  uint32_t phase;
-};
-// sample warps: my operand row is written -> everybody's is -> the MMAs of this round have finished
-__device__ __forceinline__ void round_sync(Round& r) {
+// One layer for the whole tile: every thread has written its operand row -> accumulator [128 rows][N] = A . W^T over
+// KSTEPS x 16 inputs (two m64 halves) -> fragments into the fp32 row buffer -> every thread may read its row.
+template <int N, int KSTEPS>
+__device__ __forceinline__ void mma_round(uint32_t a_addr, uint32_t b_addr, float* rows, int tid) {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");          // generic-proxy stores -> visible to the tensor core's reads
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  asm volatile("bar.sync 1, 160;" ::: "memory");
-  uint32_t done = 0, spins = 0;
-  uint64_t t0 = 0;
-  while (!done) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(smem_u32(r.bar)), "r"(r.phase)
-        : "memory");
-    if (!done && ((++spins) & 1023u) == 0) {   // bounded: a protocol bug traps after 2 s instead of hanging the GPU
-      uint64_t t;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
-      if (t0 == 0) t0 = t;
-      else if (t - t0 > 2000000000ull) __trap();
-    }
+  __syncthreads();                                                      // every row written, every previous accumulator row read
+  float d0[N / 2], d1[N / 2];
+  wg::fence();
+#pragma unroll
+  for (int k = 0; k < KSTEPS; ++k) {
+    wg::mma_f16<N>(d0, wg::desc_sw128(a_addr + k * 32), wg::desc_sw128(b_addr + k * 32), k);
+    wg::mma_f16<N>(d1, wg::desc_sw128(a_addr + 64 * 128 + k * 32), wg::desc_sw128(b_addr + k * 32), k);
   }
-  r.phase ^= 1u;
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// MMA warp: wait for the rows, issue KSTEPS x (M = 128, N, K = 16) into TMEM columns [col, col + N), signal the mbarrier
-__device__ __forceinline__ void round_issue(uint64_t* bar, uint32_t tmem_base, int col, uint32_t a_addr, uint32_t b_addr, int N, int ksteps,
-                                            int lane) {
-  asm volatile("bar.sync 1, 160;" ::: "memory");
-  if (lane == 0) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t idesc = umma_idesc_f16(128, N);
-    for (int k = 0; k < ksteps; ++k)
-      umma_f16(tmem_base + col, umma_desc_sw128(a_addr + k * 32), umma_desc_sw128(b_addr + k * 32), idesc, k != 0);
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
+  wg::commit();
+  wg::wait<0>();
+  const int r = 16 * (tid >> 5) + ((tid & 31) >> 2), c = 2 * (tid & 3);
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    float* p = rows + r * ST_LD + 8 * j + c;
+    p[0] = d0[4 * j], p[1] = d0[4 * j + 1], p[8 * ST_LD] = d0[4 * j + 2], p[8 * ST_LD + 1] = d0[4 * j + 3];
+    p += 64 * ST_LD;
+    p[0] = d1[4 * j], p[1] = d1[4 * j + 1], p[8 * ST_LD] = d1[4 * j + 2], p[8 * ST_LD + 1] = d1[4 * j + 3];
   }
-  __syncwarp();
+  __syncthreads();
 }
 
 __device__ __forceinline__ void sample_point(const o2345_points& src, int64_t gi, float& x, float& y, float& z) {
@@ -216,8 +158,6 @@ render_blend_t5_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
   uint8_t* sm = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
   float* sF = reinterpret_cast<float*>(sm + S_F32);
   __half* sPS = reinterpret_cast<__half*>(sm + S_PS);
-  uint64_t* bar = reinterpret_cast<uint64_t*>(sm + S_BAR);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bar + 1);
   const int tid = threadIdx.x, nth = blockDim.x, lane = tid & 31, warp = tid >> 5;
 
   // ---- weights: the seven MMA operands, the per-sample part of base_fc[0], the small fp32 vectors
@@ -252,40 +192,16 @@ render_blend_t5_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
   __syncthreads();
   for (int k = tid; k < 32; k += nth)   // visibility row of vis_fc[2]
     *reinterpret_cast<__half*>(sm + W_V1 + sw128_off(32, k)) = __float2half_rn(__ldg(pack + P_V1V + k));
-  if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(bar)));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 4) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], 128;" ::"r"(smem_u32(tmem_slot)));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-  }
-  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   const uint32_t a_addr = smem_u32(sm + A_BUF);
   const int64_t groups = (n + 3) >> 2;
 
-  if (warp == 4) {
-    // ---------------- MMA issuer: seven rounds per group of four samples, alternating between two TMEM column ranges
-    for (int64_t grp = blockIdx.x; grp < groups; grp += gridDim.x) {
-      round_issue(bar, tmem_base, 0, a_addr, smem_u32(sm + W_D1), 64, 1, lane);
-      round_issue(bar, tmem_base, 64, a_addr, smem_u32(sm + W_B0), 64, 4, lane);
-      round_issue(bar, tmem_base, 0, a_addr, smem_u32(sm + W_B1), 32, 4, lane);
-      round_issue(bar, tmem_base, 64, a_addr, smem_u32(sm + W_V0), 32, 2, lane);
-      round_issue(bar, tmem_base, 0, a_addr, smem_u32(sm + W_V1), 48, 2, lane);
-      round_issue(bar, tmem_base, 64, a_addr, smem_u32(sm + W_U0), 32, 2, lane);
-      round_issue(bar, tmem_base, 0, a_addr, smem_u32(sm + W_R0), 16, 3, lane);
-    }
-  } else {
-    // ---------------- sample warps
-    Round rnd{bar, 0u};
-    const int row = warp * 32 + lane;                                   // operand row = TMEM lane
-    const uint32_t trow = tmem_base + ((uint32_t)(warp * 32) << 16);
+  {
+    // ---------------- seven wgmma rounds per group of four samples
+    const int row = warp * 32 + lane;                                   // operand row = accumulator row
+    float* rows = reinterpret_cast<float*>(sm + S_STAGE);
+    const float* myrow = rows + row * ST_LD;
     uint8_t* abuf = sm + A_BUF;
-    float* stage = reinterpret_cast<float*>(sm + S_STAGE) + warp * 32 * ST_LD;
+    float* stage = rows + warp * 32 * ST_LD;                            // this warp's rows (features between rounds 1 and 2)
     float* svec = reinterpret_cast<float*>(sm + S_VEC) + warp * VEC_F;  // [0,134) geo|mean|var, [134,198) per-sample base_fc part, [198,230) weights
     const int V = views.V, H = views.H, W = views.W;
     const float abs_s = sF[F_S];
@@ -423,13 +339,13 @@ render_blend_t5_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
         }
         if (run) write_row<16>(abuf, row, h16);
       }
-      round_sync(rnd);
+      mma_round<64, 1>(a_addr, smem_u32(sm + W_D1), rows, tid);
       {
         float d[32];
-        tmem_ld32(trow + 0, d);
+        acc_row<32>(myrow + 0, d);
 #pragma unroll
         for (int c = 0; c < 32; ++c) rf[c] = vmask ? rf[c] + elu_(d[c] + sF[F_D1B + c]) : 0.f;
-        tmem_ld32(trow + 32, d);
+        acc_row<32>(myrow + 32, d);
 #pragma unroll
         for (int c = 0; c < 27; ++c) rf[32 + c] = vmask ? rf[32 + c] + elu_(d[c] + sF[F_D1B + 32 + c]) : 0.f;
         rf[59] = 0.f;
@@ -471,54 +387,54 @@ render_blend_t5_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
         a64[60] = a64[61] = a64[62] = a64[63] = 0.f;
         write_row<64>(abuf, row, a64);
       }
-      round_sync(rnd);
+      mma_round<64, 4>(a_addr, smem_u32(sm + W_B0), rows, tid);
       // ---- base_fc: x1 = ELU(per-sample part + Wf f) -> round 3 operand
       {
         float a64[64];
         float d[32];
-        tmem_ld32(trow + 64, d);
+        acc_row<32>(myrow + 0, d);
 #pragma unroll
         for (int c = 0; c < 32; ++c) a64[c] = elu_(d[c] + svec[134 + c]);
-        tmem_ld32(trow + 96, d);
+        acc_row<32>(myrow + 32, d);
 #pragma unroll
         for (int c = 0; c < 32; ++c) a64[32 + c] = elu_(d[c] + svec[166 + c]);
         if (run) write_row<64>(abuf, row, a64);
       }
-      round_sync(rnd);
+      mma_round<32, 4>(a_addr, smem_u32(sm + W_B1), rows, tid);
       float x[32];
       {
         float d[32];
-        tmem_ld32(trow + 0, d);
+        acc_row<32>(myrow + 0, d);
         float a32[32];
 #pragma unroll
         for (int c = 0; c < 32; ++c) x[c] = elu_(d[c] + sF[F_B1B + c]), a32[c] = x[c] * wv;   // vis_fc input: x * pooling weight
         if (run) write_row<32>(abuf, row, a32);
       }
-      round_sync(rnd);
+      mma_round<32, 2>(a_addr, smem_u32(sm + W_V0), rows, tid);
       {
         float d[32];
-        tmem_ld32(trow + 64, d);
+        acc_row<32>(myrow + 0, d);
 #pragma unroll
         for (int c = 0; c < 32; ++c) d[c] = elu_(d[c] + sF[F_V0B + c]);
         if (run) write_row<32>(abuf, row, d);
       }
-      round_sync(rnd);
+      mma_round<48, 2>(a_addr, smem_u32(sm + W_V1), rows, tid);
       float vis;
       {
         float d[32];
-        tmem_ld32(trow + 0, d);
+        acc_row<32>(myrow + 0, d);
         float e16[16];
-        tmem_ld16(trow + 32, e16);
+        acc_row<16>(myrow + 32, e16);
         vis = vmask ? sigm_(elu_(e16[0] + sF[F_V1B + 32])) : 0.f;
         float a32[32];
 #pragma unroll
         for (int c = 0; c < 32; ++c) x[c] += elu_(d[c] + sF[F_V1B + c]), a32[c] = x[c] * vis;       // vis_fc2 input: x * visibility
         if (run) write_row<32>(abuf, row, a32);
       }
-      round_sync(rnd);
+      mma_round<32, 2>(a_addr, smem_u32(sm + W_U0), rows, tid);
       {
         float d[32];
-        tmem_ld32(trow + 64, d);
+        acc_row<32>(myrow + 0, d);
         float u = sF[F_U1B];
 #pragma unroll
         for (int c = 0; c < 32; ++c) u = fmaf(elu_(d[c] + sF[F_U0B + c]), sF[F_U1W + c], u);
@@ -531,10 +447,10 @@ render_blend_t5_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
         for (int c = 37; c < 48; ++c) a48[c] = 0.f;
         if (run) write_row<48>(abuf, row, a48);
       }
-      round_sync(rnd);
+      mma_round<16, 3>(a_addr, smem_u32(sm + W_R0), rows, tid);
       {
         float q1[16];
-        tmem_ld16(trow + 0, q1);
+        acc_row<16>(myrow + 0, q1);
 #pragma unroll
         for (int c = 0; c < 16; ++c) q1[c] = elu_(q1[c] + sF[F_R0B + c]);
         float logit = sF[F_R2B];
@@ -553,14 +469,7 @@ render_blend_t5_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
         const float r = warp_sum(e * rgb_in[0]), g = warp_sum(e * rgb_in[1]), b = warp_sum(e * rgb_in[2]);
         if (run && lane == 0) rgb_out[3 * gi] = r / den, rgb_out[3 * gi + 1] = g / den, rgb_out[3 * gi + 2] = b / den;
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 4) {
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, 128;" ::"r"(tmem_base));
   }
 }
 
@@ -570,7 +479,7 @@ int launch_render_blend_t5(const o2345_points* src, int64_t n, const uint8_t* ac
                            const o2345_views* views, int dir_mode, const float* query_center, const float* dirs,
                            const float* rnet_pack, float* rgb, int32_t* nvalid, cudaStream_t st) {
   if (views->V > 32) {
-    set_error("o2345_render_blend (tcgen05): at most 32 source views (a lane is a view)");
+    set_error("o2345_render_blend (wgmma): at most 32 source views (a lane is a view)");
     return O2345_EUNSUPPORTED;
   }
   static PerDeviceOnce attr_done;

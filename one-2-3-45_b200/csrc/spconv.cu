@@ -92,14 +92,13 @@ sp_conv_kernel(const float* __restrict__ in, const int32_t* __restrict__ in_inde
   __shared__ __align__(16) float sW[CIN * COUT];
   __shared__ int sIdx[TR];
   __shared__ int sCell[TR];
-  __shared__ float sSum[COUT], sSq[COUT];
+  __shared__ float sPart[2][RG][COUT];  // per-row-group channel sums, added in row-group order
 
   const int n_out = *out_count;
   const int row0 = blockIdx.x * TR;
   if (row0 >= n_out) return;
   const int tid = threadIdx.x;
   const int ct = tid % CQ, rg = tid / CQ;
-  if (tid < COUT) sSum[tid] = 0.f, sSq[tid] = 0.f;
   for (int r = tid; r < TR; r += CT) sCell[r] = (row0 + r < n_out) ? out_rows[row0 + r] : -1;
   float acc[4][4];
 #pragma unroll
@@ -158,11 +157,13 @@ sp_conv_kernel(const float* __restrict__ in, const int32_t* __restrict__ in_inde
     }
   }
 #pragma unroll
-  for (int j = 0; j < 4; ++j) atomicAdd(&sSum[ct * 4 + j], ps[j]), atomicAdd(&sSq[ct * 4 + j], pq[j]);
+  for (int j = 0; j < 4; ++j) sPart[0][rg][ct * 4 + j] = ps[j], sPart[1][rg][ct * 4 + j] = pq[j];
   __syncthreads();
-  if (tid < COUT) {
-    atomicAdd(stats + tid, (double)sSum[tid]);
-    atomicAdd(stats + COUT + tid, (double)sSq[tid]);
+  if (tid < COUT) {   // fixed-order CTA sum; the CTAs' fp32 sums are added in fp64 (exact in practice)
+    float s = 0.f, q = 0.f;
+    for (int r = 0; r < RG; ++r) s += sPart[0][r][tid], q += sPart[1][r][tid];
+    atomicAdd(stats + tid, (double)s);
+    atomicAdd(stats + COUT + tid, (double)q);
   }
 }
 

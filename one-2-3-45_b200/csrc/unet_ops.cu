@@ -1,4 +1,4 @@
-// Path A glue kernels around the tcgen05 GEMM: everything in the Zero123 UNet / VAE that is not a matrix
+// Path A glue kernels around the wgmma GEMM: everything in the Zero123 UNet / VAE that is not a matrix
 // product.  Activations are channel-last fp16 ([B, H*W, C]); normalisation statistics, softmax and the
 // DDIM update are computed in fp32, matching the reference's autocast policy (GroupNorm32 / LayerNorm /
 // softmax in fp32: ldm/modules/diffusionmodules/util.py:214-216, SURVEY.md section 8 header).
@@ -24,23 +24,48 @@ namespace {
 
 __device__ __forceinline__ float silu(float x) { return x / (1.f + __expf(-x)); }
 
+// Per-group sums of a CTA in a FIXED order (no atomics, so a run is bit-reproducible): thread (prow, slot) holds the partial
+// sums s[8] / sums of squares q[8] of channels slot * 8 .. slot * 8 + 7 over its pixels; the pixel rows are added channel by
+// channel in row order into chan [2 C], then the channels of a group in channel order into out[2 g], out[2 g + 1].
+// blockDim must be rows * C / 8; every thread calls it.
+__device__ void block_group_sums(const float (&s)[8], const float (&q)[8], int slot, int prow, int rows, int C, int G,
+                                 float* chan, float* out) {
+  for (int r = 0; r < rows; ++r) {
+    if (prow == r) {
+#pragma unroll
+      for (int e = 0; e < 8; ++e) {
+        const int c = slot * 8 + e;
+        chan[2 * c] = (r ? chan[2 * c] : 0.f) + s[e];
+        chan[2 * c + 1] = (r ? chan[2 * c + 1] : 0.f) + q[e];
+      }
+    }
+    __syncthreads();
+  }
+  const int cg = C / G;
+  for (int g = threadIdx.x; g < G; g += blockDim.x) {
+    float a = 0.f, b = 0.f;
+    for (int c = g * cg; c < (g + 1) * cg; ++c) a += chan[2 * c], b += chan[2 * c + 1];
+    out[2 * g] = a, out[2 * g + 1] = b;
+  }
+  __syncthreads();
+}
+
 // GroupNorm statistics folded into a per-(image, channel) affine: y = x * scale[b, c] + shift[b, c] with
 // scale = rstd * gamma, shift = beta - mean * rstd * gamma.  x [B, HW, C] fp16 channel-last.
 // grid (chunks, B): a CTA reads a slab of pixels with 16-byte loads (thread = fixed 8-channel slot, so the partial sums
-// stay in registers), folds them into per-group shared-memory sums, adds those to the global scratch, and the LAST CTA
-// of each image (ticket counter) turns the totals into scale / shift and leaves the scratch zeroed for the next call.
+// stay in registers), folds them into per-group sums (block_group_sums), stores those in its own slot of the scratch, and the
+// LAST CTA of each image (ticket counter) adds the chunks' sums in chunk order, turns them into scale / shift and resets the
+// ticket for the next call.  Scratch: B ticket ints, then [B][chunks][2 G] floats.
 __global__ void groupnorm_stats_kernel(const __half* __restrict__ x, int HW, int C, int G, float eps,
                                        const float* __restrict__ gamma, const float* __restrict__ beta,
                                        float* __restrict__ scratch, int B, int P,
                                        float* __restrict__ scale, float* __restrict__ shift) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ float gsm[];           // [2 G] sums, then [2 G] mean / rstd
+  extern __shared__ float gsm[];           // [2 G] sums, then [2 G] mean / rstd, then [2 C] channel sums
   __shared__ int is_last;
   const int b = blockIdx.y, c8n = C >> 3, cg = C / G;
   const int slot = threadIdx.x % c8n, prow = threadIdx.x / c8n, rows = blockDim.x / c8n;
-  for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) gsm[i] = 0.f;
-  __syncthreads();
   float s[8], q[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) s[e] = 0.f, q[e] = 0.f;
@@ -57,20 +82,11 @@ __global__ void groupnorm_stats_kernel(const __half* __restrict__ x, int HW, int
         s[2 * e + 1] += f.y, q[2 * e + 1] = fmaf(f.y, f.y, q[2 * e + 1]);
       }
     }
-    int g = (slot * 8) / cg;
-    float rs = 0.f, rq = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      int ge = (slot * 8 + e) / cg;
-      if (ge != g) { atomicAdd(gsm + 2 * g, rs), atomicAdd(gsm + 2 * g + 1, rq), rs = rq = 0.f, g = ge; }
-      rs += s[e], rq += q[e];
-    }
-    atomicAdd(gsm + 2 * g, rs), atomicAdd(gsm + 2 * g + 1, rq);
   }
-  __syncthreads();
-  float* tot = scratch + (int64_t)b * 2 * G;
-  int* ticket = reinterpret_cast<int*>(scratch + (int64_t)B * 2 * G) + b;
-  for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) atomicAdd(tot + i, gsm[i]);
+  block_group_sums(s, q, slot, prow, rows, C, G, gsm + 4 * G, gsm);
+  int* ticket = reinterpret_cast<int*>(scratch) + b;
+  float* parts = scratch + B + (int64_t)b * gridDim.x * 2 * G;           // this image's [chunks][2 G]
+  for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) parts[(int64_t)blockIdx.x * 2 * G + i] = gsm[i];
   __threadfence();
   __syncthreads();
   if (threadIdx.x == 0) is_last = atomicAdd(ticket, 1) == (int)gridDim.x - 1;
@@ -78,12 +94,13 @@ __global__ void groupnorm_stats_kernel(const __half* __restrict__ x, int HW, int
   if (!is_last) return;
   __threadfence();
   for (int g = threadIdx.x; g < G; g += blockDim.x) {
-    float n = (float)HW * cg, m = __ldcg(tot + 2 * g) / n;
-    float var = fmaxf(__ldcg(tot + 2 * g + 1) / n - m * m, 0.f);
+    float ts = 0.f, tq = 0.f;
+    for (int k = 0; k < (int)gridDim.x; ++k) ts += __ldcg(parts + (int64_t)k * 2 * G + 2 * g), tq += __ldcg(parts + (int64_t)k * 2 * G + 2 * g + 1);
+    float n = (float)HW * cg, m = ts / n;
+    float var = fmaxf(tq / n - m * m, 0.f);
     gsm[2 * g] = m, gsm[2 * g + 1] = rsqrtf(var + eps);
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) tot[i] = 0.f;
   if (threadIdx.x == 0) *ticket = 0;
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     float m = gsm[2 * (c / cg)], r = gsm[2 * (c / cg) + 1];
@@ -265,16 +282,15 @@ __global__ void groupnorm_apply_cluster_kernel(const __half* __restrict__ x, int
                                                __half* __restrict__ out) {
   pdl_wait();
   pdl_trigger();
-  extern __shared__ __align__(16) float gsm[];           // [2 G] this CTA's sums, [2 G] the image's sums, then (KEEP) the slab
+  extern __shared__ __align__(16) float gsm[];           // [2 G] this CTA's sums, [2 G] the image's sums, [2 C] channel sums,
+                                                          // then (KEEP) the slab
   constexpr int U = 4;
   uint32_t rank, csize;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(rank));
   asm volatile("mov.u32 %0, %%cluster_nctarank;" : "=r"(csize));
   const int b = blockIdx.y, cg = C / G, c8n = C >> 3;
   const int slot = threadIdx.x % c8n, prow = threadIdx.x / c8n, rows = blockDim.x / c8n;   // blockDim is a multiple of c8n
-  uint4* slab = reinterpret_cast<uint4*>(gsm + ((4 * G + 3) & ~3));
-  for (int i = threadIdx.x; i < 4 * G; i += blockDim.x) gsm[i] = 0.f;
-  __syncthreads();
+  uint4* slab = reinterpret_cast<uint4*>(gsm + ((4 * G + 2 * C + 3) & ~3));
   const int P = (HW + (int)csize - 1) / (int)csize;
   const int p0 = (int)rank * P, p1 = min(HW, p0 + P);
   const __half* base = x + (int64_t)b * HW * C + slot * 8;
@@ -298,17 +314,7 @@ __global__ void groupnorm_apply_cluster_kernel(const __half* __restrict__ x, int
       }
     }
   }
-  {
-    int g = (slot * 8) / cg;
-    float rs = 0.f, rq = 0.f;
-#pragma unroll
-    for (int e = 0; e < 8; ++e) {
-      const int ge = (slot * 8 + e) / cg;
-      if (ge != g) { atomicAdd(gsm + 2 * g, rs), atomicAdd(gsm + 2 * g + 1, rq), rs = rq = 0.f, g = ge; }
-      rs += s[e], rq += q[e];
-    }
-    atomicAdd(gsm + 2 * g, rs), atomicAdd(gsm + 2 * g + 1, rq);
-  }
+  block_group_sums(s, q, slot, prow, rows, C, G, gsm + 4 * G, gsm);
   // every CTA's partial sums become visible to the cluster
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
   for (int i = threadIdx.x; i < 2 * G; i += blockDim.x) {
@@ -639,7 +645,8 @@ __global__ void clip_add_positions_kernel(__half* __restrict__ tok, const float*
 using namespace o2345;
 #define ST ((cudaStream_t)stream)
 
-extern "C" int64_t o2345_groupnorm_scratch_floats(int B, int G) { return (int64_t)B * 2 * G + B; }
+// B ticket ints, then [B][chunks][2 G] per-CTA sums; o2345_groupnorm_stats launches at most cdiv(2 * SMs, B) chunks per image
+extern "C" int64_t o2345_groupnorm_scratch_floats(int B, int G) { return (int64_t)B + (int64_t)B * cdiv(2 * sm_count(), B) * 2 * G; }
 
 extern "C" int o2345_groupnorm_stats(const void* x, int B, int HW, int C, int G, float eps, const float* gamma,
                                      const float* beta, float* scratch, float* scale, float* shift, o2345_stream_t stream) {
@@ -653,7 +660,10 @@ extern "C" int o2345_groupnorm_stats(const void* x, int B, int HW, int C, int G,
   if (chunks < 1) chunks = 1;
   const int P = cdiv(HW, chunks);
   chunks = cdiv(HW, P);
-  O2345_CUDA(launch_pdl(groupnorm_stats_kernel, dim3(dim3(chunks, B)), dim3(threads), (size_t)(4 * G * sizeof(float)), ST, (const __half*)x, HW, C, G, eps, gamma, beta,
+  const size_t smem = (size_t)(4 * G + 2 * C) * sizeof(float);
+  static PerDeviceOnce attr;
+  if (attr.need()) O2345_CUDA(cudaFuncSetAttribute(groupnorm_stats_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 4 * (4 * 256 + 2 * 8192)));
+  O2345_CUDA(launch_pdl(groupnorm_stats_kernel, dim3(dim3(chunks, B)), dim3(threads), smem, ST, (const __half*)x, HW, C, G, eps, gamma, beta,
                                                                                   scratch, B, P, scale, shift));
   O2345_LAUNCH_CHECK();
   return O2345_OK;
@@ -670,19 +680,18 @@ extern "C" int o2345_groupnorm_apply(const void* x, int B, int HW, int C, int G,
   const int c8n = C / 8;
   const int rows = c8n >= 512 ? 1 : 512 / c8n;
   const int threads = c8n * rows;
-  // CTAs per image = cluster size (a power of two <= 16, a non-portable size).  Measured on a B200 (tools/gn_bench.py,
-  // profiles/r2_gn_cluster_sweep.txt): the kernel is fastest when the whole launch is about ONE CTA per SM -- clusters of 16
-  // over a batch of 64 images (1 024 small CTAs, few 16-wide clusters schedulable at a time) took 2-3x longer than clusters
-  // of 2 -- except that slabs beyond ~400 KB per CTA want one more doubling.  Never more CTAs than the image has pixel rows.
+  // CTAs per image = cluster size (a power of two <= 8, the portable size: a cluster of CTAs that park up to 200 KB each
+  // must fit one GPC).  The rule aims at about ONE CTA per SM for the whole launch (tools/gn_bench.py sweeps it), except
+  // that slabs beyond ~400 KB per CTA want one more doubling.  Never more CTAs than the image has pixel rows.
   int cl = 1;
-  while (cl < 16 && (int64_t)2 * cl * B <= (int64_t)sm_count()) cl <<= 1;
-  if (cl < 16 && (int64_t)HW * C * 2 / cl > 400 * 1024) cl <<= 1;
+  while (cl < 8 && (int64_t)2 * cl * B <= (int64_t)sm_count()) cl <<= 1;
+  if (cl < 8 && (int64_t)HW * C * 2 / cl > 400 * 1024) cl <<= 1;
   while (cl > 1 && HW < cl * rows) cl >>= 1;
   if (g_gn_cluster > 0) {
-    cl = g_gn_cluster;
+    cl = g_gn_cluster < 8 ? g_gn_cluster : 8;
     while (cl > 1 && HW < cl * rows) cl >>= 1;
   }
-  const size_t sums = (size_t)((4 * G + 3) & ~3) * sizeof(float);
+  const size_t sums = (size_t)((4 * G + 2 * C + 3) & ~3) * sizeof(float);
   const size_t slab = (size_t)cdiv(HW, cl) * C * 2;
   const bool keep = sums + slab <= 200 * 1024;
   static PerDeviceOnce attr;
@@ -690,6 +699,7 @@ extern "C" int o2345_groupnorm_apply(const void* x, int B, int HW, int C, int G,
     O2345_CUDA(cudaFuncSetAttribute(groupnorm_apply_cluster_kernel<true>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     O2345_CUDA(cudaFuncSetAttribute(groupnorm_apply_cluster_kernel<false>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1));
     O2345_CUDA(cudaFuncSetAttribute(groupnorm_apply_cluster_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 201 * 1024));
+    O2345_CUDA(cudaFuncSetAttribute(groupnorm_apply_cluster_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 201 * 1024));
   }
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));

@@ -1,4 +1,4 @@
-"""ctypes binding of libo2345_sm100.so (the C-ABI declared in include/o2345.h).
+"""ctypes binding of libo2345_sm90.so (the C-ABI declared in include/o2345.h).
 
 There is deliberately NO fallback: if the shared library is missing or a call fails this module
 raises, it never routes work to PyTorch or to the CPU oracle.
@@ -10,7 +10,7 @@ import functools
 import os
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get("O2345_LIB") or os.path.join(os.path.dirname(HERE), "lib", "libo2345_sm100.so")   # O2345_LIB: A/B against another build (tools/)
+LIB_PATH = os.environ.get("O2345_LIB") or os.path.join(os.path.dirname(HERE), "lib", "libo2345_sm90.so")   # O2345_LIB: A/B against another build (tools/)
 
 c_fp = C.c_void_p  # device pointers travel as integers
 c_i64 = C.c_int64

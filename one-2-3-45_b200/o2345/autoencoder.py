@@ -5,7 +5,7 @@ for the first_stage_config of configs/sd-objaverse-finetune-c_concat-256.yaml:45
 two ResnetBlocks per level, attention only in the middle, z_channels 4, double_z).  The module tree reproduces the
 reference state-dict keys (`encoder.down.0.block.0.norm1.weight`, `decoder.up.3.upsample.conv.weight`, ...).
 `encode(x)` returns a DiagonalGaussianDistribution-like object (`.mode()`, `.mean`), `decode(z)` an image batch.
-Same primitives as the UNet: GroupNorm(eps 1e-6)+swish fused into the conv patch gather, tcgen05 GEMMs, and a
+Same primitives as the UNet: GroupNorm(eps 1e-6)+swish fused into the conv patch gather, wgmma GEMMs, and a
 single-head 512-channel attention in the middle block.
 """
 from __future__ import annotations

@@ -10,7 +10,7 @@ names (`model.visual.conv1.weight`, `model.visual.transformer.resblocks.{i}.attn
 checkpoint's `cond_stage_model.*` keys load directly.
 
 Execution: one kernel resizes, normalises and patchifies (the A operand of the patch-embedding GEMM); every Linear is
-the tcgen05 GEMM (QuickGELU / residual in the epilogue); attention is the fused mma.sync kernel at head dim 64;
+the wgmma GEMM (QuickGELU / residual in the epilogue); attention is the fused mma.sync kernel at head dim 64;
 LayerNorms are fp32-statistics row kernels; activations fp16 (the reference runs this tower in fp16 under
 --half_precision as well).
 """

@@ -83,7 +83,7 @@ class LatentSDFLayer(nn.Module):
     def __init__(self, d_in=3, d_out=129, d_hidden=128, n_layers=4, multires=6, d_conditional_feature=16, **_):
         super().__init__()
         if (d_hidden, n_layers, multires, d_conditional_feature) != (128, 4, 6, 16):
-            raise NotImplementedError("the sm_100a SDF kernel is specialised for hidden 128, 4 layers, multires 6, latent 16")
+            raise NotImplementedError("the sm_90a SDF kernel is specialised for hidden 128, 4 layers, multires 6, latent 16")
         d_pe = d_in * (2 * multires + 1)
         self.lin0 = _WeightNormLinear(d_pe, d_hidden)
         self.lin1 = _WeightNormLinear(d_hidden + d_conditional_feature, d_hidden)

@@ -8,7 +8,7 @@ legacy=False): the module tree below reproduces the reference's state-dict keys
 signature and returns the epsilon prediction [N,4,H,W] in fp32 (values rounded through fp16 exactly where
 autocast would round them).
 
-Execution: activations are channel-last fp16 [N*H*W, C].  Every Linear / 1x1 conv is one tcgen05 GEMM and every
+Execution: activations are channel-last fp16 [N*H*W, C].  Every Linear / 1x1 conv is one wgmma GEMM and every
 3x3 stride-1 conv an implicit GEMM whose nine shifted windows are fetched by TMA (csrc/gemm_tc.cu: CTA-pair
 `cta_group::2` tiles, split-K for small grids); the strided / up-sampling convs gather patches first
 (csrc/unet_ops.cu).  GroupNorm is a per-(image, channel) affine computed by one statistics kernel and applied together
@@ -213,9 +213,8 @@ class UNetModel(nn.Module):
         self._graphs = {}
         self._ctx_ref, self._ctx_ver, self._ctx_pk, self._cross_out = None, None, None, {}
         # GroupNorm statistics tables filled by the producing GEMMs' epilogues (one arena, zeroed once per pass).  OFF by
-        # default: measured on a B200 the fused pass is SLOWER (captured UNet graph 5.69 ms with 324 kernels against 4.88 ms
-        # with 370): the epilogues' red.add.f32 hit each (image, channel) address from 32 row slabs, and the L2 atomic units
-        # serialise same-address updates (~13 us per producing GEMM, more than the 46 statistics kernels it removes).
+        # default: the epilogues' red.add.f32 hit each (image, channel) address from 32 row slabs, and the L2 atomic units
+        # serialise same-address updates, which can cost more than the 46 statistics kernels it removes (not measured on H100).
         # Kept as a tested option (tests/test_gpu_gemm.py::test_epilogue_groupnorm_statistics_feed_the_next_norm).
         self.fuse_gn_stats = False
         self.gn_one_kernel = True    # GroupNorm statistics + apply in one cluster kernel (o2345_groupnorm_apply)

@@ -302,6 +302,16 @@ def build_zero123(device, seed=0, clip=False):
         m.cond_stage_model.load_state_dict({k: torch.from_numpy(v) for k, v in S.clip_state(seed + 20).items()})
     m.model.diffusion_model.load_state_dict({k: torch.from_numpy(v) for k, v in S.unet_state(seed).items()})
     m.first_stage_model.load_state_dict({k: torch.from_numpy(v) for k, v in S.vae_state(seed + 10).items()})
+    # cc_projection is seeded too (nn.Linear's own initialisation draws from the unseeded global generator: every process would
+    # build a different model): the reference's initialisation (ddpm.py:526-528: identity on the CLIP embedding, zero bias)
+    # and nn.Linear's uniform bound for the four pose columns
+    g = torch.Generator().manual_seed(seed + 30)
+    with torch.no_grad():
+        w = m.cc_projection.weight
+        w.zero_()
+        w[:, :768] = torch.eye(768)
+        w[:, 768:] = (torch.rand(768, 4, generator=g) * 2 - 1) / 772 ** 0.5
+        m.cc_projection.bias.zero_()
     for p in m.parameters():
         p.requires_grad_(False)
     return m.to(device)

@@ -34,7 +34,7 @@ def load_input(path):
 
 
 def main(argv=None):
-    ap = argparse.ArgumentParser(description="single image -> textured mesh on the o2345 (sm_100a) kernels")
+    ap = argparse.ArgumentParser(description="single image -> textured mesh on the o2345 (sm_90a) kernels")
     ap.add_argument('--img_path', type=str, default="./demo/demo_examples/01_wild_hydrant.png", help='Path to the input image')
     ap.add_argument('--gpu_idx', type=int, default=0, help='GPU index')
     ap.add_argument('--half_precision', action='store_true', help='accepted for compatibility: the UNet / VAE kernels are fp16')

@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "one-2-3-45_b200")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100, sm_90a; select with -m gpu)")
 
 
 @pytest.fixture(scope="session")

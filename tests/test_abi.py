@@ -38,7 +38,7 @@ def test_ctypes_table_matches_header():
 def test_missing_library_fails_loudly(monkeypatch):
     from o2345 import _lib
     monkeypatch.setattr(_lib, "_lib", None)
-    monkeypatch.setattr(_lib, "LIB_PATH", "/nonexistent/libo2345_sm100.so")
+    monkeypatch.setattr(_lib, "LIB_PATH", "/nonexistent/libo2345_sm90.so")
     with pytest.raises(_lib.O2345Error):
         _lib.load()
 

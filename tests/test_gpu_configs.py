@@ -219,7 +219,7 @@ def test_two_scenes_through_one_renderer(c1):
 
 
 def test_real_unet_ddim_trajectory_against_oracle():
-    """Five DDIM iterations (S = 5, eta = 1, CFG 3) of the real UNet on the tcgen05 path against ldm_oracle.ddim_sample
+    """Five DDIM iterations (S = 5, eta = 1, CFG 3) of the real UNet on the wgmma path against ldm_oracle.ddim_sample
     running the fp32 oracle UNet on the host, same weights, same injected noise.  fp16 rounding of ~60 layers re-enters the
     loop four times: measured max |x - x_oracle| 6e-3 on latents of std ~1 (bar: 2e-2 max, 3e-3 mean)."""
     from o2345.ddim import DDIMSampler

@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 GEMM against torch.matmul in fp32 on the same fp16 inputs (fp32 accumulate on both sides)."""
+"""GPU: the wgmma GEMM against torch.matmul in fp32 on the same fp16 inputs (fp32 accumulate on both sides)."""
 import pytest
 import torch
 
@@ -93,7 +93,7 @@ def test_implicit_conv3x3_matches_conv2d(B, H, W, C, N):
                                    (8192, 960, 320), (2048, 1920, 640), (4096, 512, 1152), (1000, 256, 192), (300, 192, 72),
                                    (257, 160, 64), (129, 3840, 1280)])
 def test_pair_kernel_shapes(M, N, K):
-    """Every tile width of the CTA-pair kernel (160 / 256 / 128), M tails inside the second CTA, split-K shapes."""
+    """Every tile width of the kernel (160 / 256 / 128 / 64), M tails inside the second warpgroup, split-K shapes."""
     from o2345 import ops_a
     g = torch.Generator(device="cuda").manual_seed(M + N + K)
     a = (torch.randn(M, K, device="cuda", generator=g) * 0.5).half()
@@ -207,8 +207,8 @@ def test_epilogue_groupnorm_statistics_feed_the_next_norm(B, H, W, C, N, split):
 
 @pytest.fixture
 def persistent_everywhere():
-    """Forces the persistent variant of the GEMM kernel wherever it is available (pair tiles >= 128 columns, staged fp16
-    epilogue), whatever the tile count; restores the heuristic afterwards."""
+    """Forces the persistent launch of the GEMM kernel wherever it is available (staged fp16 epilogue, no split-K), whatever
+    the tile count; restores the heuristic afterwards."""
     from o2345 import _lib
     lib = _lib.load()
     lib.o2345_debug_gemm_persist(1, 0)
@@ -221,9 +221,9 @@ def persistent_everywhere():
 @pytest.mark.parametrize("M,N,K", [(65536, 320, 320), (16384, 640, 640), (40000, 960, 328), (300, 192, 72), (8192, 2560, 64),
                                    (33000, 1280, 1280)])
 def test_persistent_kernel_matches_matmul(persistent_everywhere, bn, M, N, K):
-    """One CTA pair per SM pair walking many tiles with two TMEM accumulator buffers: every tile width, one to ~40 tiles per
-    pair, M tails inside a pair and inside the first CTA, N tails, K tails, a single k-block (the accumulator hand-over is
-    then the only thing between two tiles), bias + residual + activation and GEGLU epilogues."""
+    """At most one CTA per SM walking many tiles, the operand ring's stages and phases running on across tiles: every tile
+    width, one to ~8 tiles per CTA, M tails inside the second warpgroup, N tails, K tails, a single k-block (then only the
+    ring hand-over is between two tiles), bias + residual + activation and GEGLU epilogues."""
     from o2345 import ops_a
     persistent_everywhere.o2345_debug_gemm_force(2, bn, 1)
     g = torch.Generator(device="cuda").manual_seed(M + N + K + bn)
@@ -248,7 +248,7 @@ def test_persistent_kernel_matches_matmul(persistent_everywhere, bn, M, N, K):
 
 @pytest.mark.parametrize("B,H,W,C,N", [(64, 32, 32, 320, 320), (16, 16, 16, 640, 640), (64, 8, 8, 1280, 1280), (3, 64, 64, 128, 128)])
 def test_persistent_kernel_implicit_conv(persistent_everywhere, B, H, W, C, N):
-    """The implicit 3x3 convolution (nine shifted TMA boxes per channel block) through the persistent kernel, with the
+    """The implicit 3x3 convolution (nine shifted TMA boxes per channel block) through the persistent launch, with the
     ResBlock epilogue: bias + per-image embedding row bias, then the skip connection."""
     from o2345 import ops_a
     g = torch.Generator(device="cuda").manual_seed(B + H + C)

@@ -48,12 +48,12 @@ def maxerr(a, b):
     return float((torch.as_tensor(a).double().cpu() - torch.as_tensor(b).double().cpu()).abs().max())
 
 
-def test_device_is_sm100():
+def test_device_is_sm90():
     import ctypes as C
     from o2345 import _lib
     ma, mi, sms = C.c_int(), C.c_int(), C.c_int()
     _lib.call("o2345_device_info", C.byref(ma), C.byref(mi), C.byref(sms))
-    assert ma.value == 10 and sms.value >= 100
+    assert (ma.value, mi.value) == (9, 0) and sms.value >= 100
 
 
 def test_feature_net(om, gpu, golden):
@@ -416,7 +416,7 @@ def test_full_size_blend_kernels_agree(full, dev):
                 w2cs=sample["w2cs"][0], intrinsics=sample["intrinsics"][0], img_wh=[256, 256], query_c2w=sample["query_c2w"])
     finally:
         tr.sdf_renderer_lod0.blend_precision = old
-    for prec, name in ((1, "mma.sync"), (2, "tcgen05")):
+    for prec, name in ((1, "mma.sync"), (2, "wgmma")):
         a, b = outs[0]["color_fine"], outs[prec]["color_fine"]
         assert torch.equal(outs[0]["z_vals"], outs[prec]["z_vals"])                 # the sampler does not depend on the colours
         assert torch.equal(outs[0]["color_fine_mask"], outs[prec]["color_fine_mask"])

@@ -1,4 +1,4 @@
-"""GPU: Zero123 UNet on the tcgen05 path and the DDIM sampler, against the reference goldens.
+"""GPU: Zero123 UNet on the wgmma path and the DDIM sampler, against the reference goldens.
 
 Tolerance: the reference itself runs this model in fp16 under autocast (fp32 GroupNorm / LayerNorm / softmax); the
 golden vector is the reference's fp32 CPU output.  fp16 storage of ~60 layers gives ~1e-2 relative deviations, so

@@ -1,4 +1,4 @@
-"""GPU: VAE decode / encode on the tcgen05 path against the reference goldens (fp16 storage: see test_gpu_unet.py)."""
+"""GPU: VAE decode / encode on the wgmma path against the reference goldens (fp16 storage: see test_gpu_unet.py)."""
 import os
 
 import numpy as np

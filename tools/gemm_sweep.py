@@ -1,4 +1,4 @@
-"""Tile-configuration sweep of the tcgen05 GEMM over every distinct GEMM / implicit-conv shape of one UNet forward
+"""Tile-configuration sweep of the wgmma GEMM over every distinct GEMM / implicit-conv shape of one UNet forward
 (CFG batch 8): for each shape, the device time of the heuristic's choice, of every forced (ctas, bn, splits) candidate
 (o2345_debug_gemm_force) and of cuBLAS on the same shape, all under the protocol the captured UNet graph runs under
 (cold L2, no host launch gaps): a CUDA graph of REPS x (L2 flush, call) minus a graph of REPS flushes.
@@ -97,18 +97,18 @@ for k, calls in groups.items():
     lib.o2345_debug_gemm_force(0, 0, 0)
     t_h = max(graph_ms(lambda: fn(*a, **kw)) - base, 1e-4)
     cands = []
-    for ctas in ((1, 2) if M <= 256 else (2,)):
-        for bn in ((64, 128) if ctas == 1 else (64, 128, 160, 256)):
+    for ctas in (1,):
+        for bn in (64, 128, 160, 256):
             if bn > 64 and N <= 64:
                 continue
             if act == 3 and N % bn:
                 continue
-            for sp in (1, 2, 3, 4, 6, 8, 12, 16):
+            for sp in (1, 2, 3, 4, 6, 8):
                 if sp > 1 and (act == 3 or nk // sp < 3):
                     continue
-                mblocks = (M + 127) // 128 if ctas == 1 else 2 * ((M + 255) // 256)
+                mblocks = (M + 127) // 128
                 tiles = mblocks * ((N + bn - 1) // bn)
-                if sp > 1 and (tiles * sp > 700 or sp * ctas > 16):
+                if sp > 1 and tiles * sp > 700:
                     continue
                 if QUICK and sp not in (1, 2, 4, 8):
                     continue

@@ -1,4 +1,4 @@
-"""Phase timeline of the tcgen05 GEMM for a few UNet shapes (o2345_debug_gemm_trace).
+"""Phase timeline of the wgmma GEMM for a few UNet shapes (o2345_debug_gemm_trace).
 SM-cycle stamps (clock64) of CTA (0,0,0): entry, prologue done, first / last TMA issued, first operands landed, last MMA
 issued, accumulator ready, epilogue done, exit.  For split-K launches also wall-clock stamps (globaltimer, ns, relative to
 the entry of CTA (0,0,0)) of tile (0,0): accumulator ready, partial stores issued (split 0); finalize start / end (the

@@ -1,4 +1,4 @@
-"""One reconstruction step at the bench configuration, for ncu (see profiles/README.md).
+"""One reconstruction step at the bench configuration, for ncu.
 
     ncu --metrics gpu__time_duration.sum --clock-control none --csv --log-file gpurun_out/launches.csv \
         python tools/profile_step.py --chunks 8

@@ -1,13 +1,13 @@
-"""Counts the SASS mnemonics that identify the Blackwell paths per kernel of the shipped library:
-    cuobjdump -sass one-2-3-45_b200/lib/libo2345_sm100.so | python tools/sass_evidence.py > profiles/rN_sass_evidence.txt
-UTCHMMA = tcgen05.mma, LDTM = tcgen05.ld, UTMALDG = TMA (cp.async.bulk.tensor), UTCBAR = tcgen05.commit, UTCATOMSWS = tcgen05.alloc /
-dealloc, UCGABAR = cluster barrier, HMMA = mma.sync (legacy tensor path), LDSM / STSM = ldmatrix / stmatrix, LDGSTS = cp.async."""
+"""Counts the SASS mnemonics that identify the Hopper paths per kernel of the shipped library:
+    cuobjdump -sass one-2-3-45_b200/lib/libo2345_sm90.so | python tools/sass_evidence.py > sass_evidence.txt
+HGMMA = wgmma.mma_async, WARPGROUP = wgmma fence / wait, UTMALDG = TMA (cp.async.bulk.tensor), SYNCS = mbarrier, UCGABAR = cluster
+barrier, HMMA = mma.sync, LDSM / STSM = ldmatrix / stmatrix, LDGSTS = cp.async."""
 import collections
 import re
 import subprocess
 import sys
 
-OPS = ('UTCHMMA', 'UTCQMMA', 'UTMALDG', 'UTMASTG', 'UBLKCP', 'LDTM', 'STTM', 'HMMA', 'UTCATOMSWS', 'UTCBAR', 'LDGSTS', 'LDSM', 'STSM', 'REDG',
+OPS = ('HGMMA', 'WARPGROUP', 'UTMALDG', 'UTMASTG', 'UBLKCP', 'SYNCS', 'HMMA', 'LDGSTS', 'LDSM', 'STSM', 'REDG',
        'UCGABAR_ARV', 'UCGABAR_WAIT')
 cur, counts, n = None, collections.defaultdict(collections.Counter), collections.Counter()
 for line in sys.stdin:
@@ -28,12 +28,12 @@ agg = collections.defaultdict(lambda: [0, collections.Counter(), 0])
 for k, name in zip(n, names):
     name = re.sub(r'o2345::\(anonymous namespace\)::', '', name)
     base = re.sub(r'^void ', '', re.sub(r'\(.*$', '', name))
-    key = re.sub(r'gemm_tc_kernel<(\d+), (\d+), (\d+), (\d+)>', r'gemm_tc_kernel<BN, STAGES, CTAS=\3, MODE=\4>', base)
+    key = re.sub(r'gemm_tc_kernel<(\d+), (\d+), (\d+)>', r'gemm_tc_kernel<BN, STAGES, MODE=\3>', base)
     a = agg[key]
     a[0] += 1
     a[1].update(counts[k])
     a[2] = max(a[2], n[k])
-print("cuobjdump -sass one-2-3-45_b200/lib/libo2345_sm100.so | python tools/sass_evidence.py   (sm_100a; instantiations merged: 'xN' of them,")
+print("cuobjdump -sass one-2-3-45_b200/lib/libo2345_sm90.so | python tools/sass_evidence.py   (sm_90a; instantiations merged: 'xN' of them,")
 print("counts summed over them, instruction count of the largest)\n")
 for key, (ni, c, mx) in sorted(agg.items(), key=lambda kv: -sum(kv[1][1].values())):
     if c:

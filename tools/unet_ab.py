@@ -14,7 +14,7 @@ from o2345.unet import UNetModel
 lib = _lib.load()
 net = UNetModel().cuda().requires_grad_(False)
 CASES = [("default", {}), ("up-sampling convs by gather", {"up2x": False}), ("GEMM never persistent", {"persist": (2, 0)}),
-         ("GroupNorm clusters of 16", {"gn_cl": 16}), ("default again", {})]
+         ("GroupNorm clusters of 8", {"gn_cl": 8}), ("default again", {})]
 if os.environ.get("UNET_AB_CASES"):
     CASES = eval(os.environ["UNET_AB_CASES"])
 for B in [int(a) for a in sys.argv[1:]] or [16, 64]:
