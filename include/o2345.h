@@ -32,8 +32,9 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 3   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
-                                 3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force */
+#define O2345_ABI_VERSION 4   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+                                 3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
+                                 4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...) */
 
 typedef void* o2345_stream_t;
 
@@ -134,6 +135,49 @@ int o2345_dense_scatter(const float* feat, const int32_t* rows, const int32_t* c
  * (reference sparse_neus_renderer.py:153-169).  out[i] = 1 iff occ at the nearest voxel > 0. */
 int o2345_occ_nearest(const o2345_points* src, int64_t n, const float* occ, int D, uint8_t* out,
                       o2345_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Lod-1 refinement (num_lods = 2): lod-0 SDF volume, pruning, children, cost rows with parent features.
+ * Replaces SparseSdfNetwork.get_sdf_volume            reconstruction/models/sparse_sdf_network.py:441-474
+ *          get_valid_sparse_coords_by_sdf             reconstruction/models/sparse_neus_renderer.py:822-879
+ *          SparseSdfNetwork.upsample + lod>0 branch   reconstruction/models/sparse_sdf_network.py:198-219,336-374
+ * ------------------------------------------------------------------------------------------ */
+
+/* sdf_vol[i] = SDF MLP at voxel i of the D^3 lattice for every i with occ[i] > 0, else 1.0.  The point is
+ * coord * voxel_size + origin (rounded fp32 multiply, then add) and the latent is row i of vol_cl [D^3,16] as it is
+ * (no trilinear fetch).  precision: O2345_SDF_FP32 or O2345_SDF_TC_SPLIT, as in o2345_sdf_query. */
+int o2345_sdf_voxels(const float* occ, const float* vol_cl, int D, const float* origin, float voxel_size,
+                     const float* wpack, int precision, float* sdf_vol, o2345_stream_t stream);
+
+/* minabs[i] = occ[i] > 0 ? min |sdf| over the 7^3 window around i (clipped at the border) : +inf, so that
+ * avg_pool3d(|sdf| < t, 7, 1, 3) > 0 && occ > 0  <=>  minabs < t for every t.  counts[r] (device int32) = number of
+ * voxels with minabs < ladder[r]; ladder is a HOST array of 1..16 fp32 thresholds.  scratch: float [D^3].
+ * sdf, scratch and minabs must be three distinct buffers (O2345_EINVAL otherwise). */
+int o2345_prune_by_sdf(const float* sdf, const float* occ, int D, const float* ladder, int n_ladder, float* scratch,
+                       float* minabs, int32_t* counts, o2345_stream_t stream);
+/* keep[i] = minabs[i] < threshold. */
+int o2345_prune_select(const float* minabs, int64_t n, float threshold, uint8_t* keep, o2345_stream_t stream);
+/* flags[rows[idx[i]]] = 0 for i < n (drops chosen survivors of a compaction). */
+int o2345_clear_flags(const int32_t* rows, const int32_t* idx, int64_t n, uint8_t* flags, o2345_stream_t stream);
+/* For the n lattice indices rows[i] of a D^3 lattice: coords[i] = (0, x, y, z) as floats, feats[i] = the C channels of
+ * vol_cf [C, D^3] at rows[i]. */
+int o2345_gather_rows(const int32_t* rows, int64_t n, int D, const float* vol_cf, int C, float* coords, float* feats,
+                      o2345_stream_t stream);
+
+/* pre_coords [n,4] float (batch, x, y, z), already in D1 lattice units: marks the 8 children (x+a, y+b, z+c),
+ * a,b,c in {0,1}, keep[lin] = frustum_keep[lin] (o2345_frustum_mask at D1 with min_views = 1, i.e. > 1 views), and
+ * parent[lin] = i (-1 elsewhere).  keep [D1^3] and parent [D1^3] are overwritten.  Returns O2345_EINVAL for a
+ * coordinate that is not an integer with both children in [0, D1), or for duplicate parents: this call synchronises
+ * the stream to read the device-side check (err_scratch: one int32 on the device). */
+int o2345_lod_children(const float* pre_coords, int64_t n, int D1, const uint8_t* frustum_keep, uint8_t* keep,
+                       int32_t* parent, int32_t* err_scratch, o2345_stream_t stream);
+
+/* o2345_costvol_gather for C = 8 or 16 channels per view; cost rows are [var(C), mean(C)] or, with parent / pre_feats
+ * (both or neither), [var(C), mean(C), pre_feats[parent[rows[k]]] (16)].  o2345_costvol_gather is C = 16 without parent. */
+int o2345_costvol_gather_lod(const float* feats_nhwc, int C, int V, int h, int w, int sizeH, int sizeW, const float* proj,
+                             const float* origin, float voxel_size, int D, const int32_t* rows, const int32_t* count,
+                             int64_t max_rows, const uint32_t* mask_bits, const int32_t* parent, const float* pre_feats,
+                             float* cost, o2345_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * B6: sparse 3-D convolution stack (torchsparse v1.4.0 semantics) + BatchNorm(batch stats) + ReLU.

@@ -99,6 +99,23 @@ __device__ __forceinline__ void load_point(const o2345_points& src, int64_t gi, 
   }
 }
 
+// Point and latent source of o2345_sdf_voxels (kernels instantiated with VOX = true): point i is lattice voxel
+// i = (x*D + y)*D + z at coord * vs + origin (one rounded multiply, one rounded add, as `coords * voxel_size + origin`
+// in fp32), its latent is row i of the channel-last volume as it is (no trilinear fetch), and it is evaluated iff
+// occ[i] > 0 (reference SparseSdfNetwork.get_sdf_volume, sparse_sdf_network.py:441-474).
+struct VoxelSrc {
+  const float* occ;
+  const float* origin;
+  float vs;
+};
+
+__device__ __forceinline__ void voxel_point(const VoxelSrc& vx, int64_t gi, int D, float& x, float& y, float& z) {
+  const int iz = (int)(gi % D), iy = (int)((gi / D) % D), ix = (int)(gi / ((int64_t)D * D));
+  x = __fadd_rn(__fmul_rn((float)ix, vx.vs), __ldg(vx.origin));
+  y = __fadd_rn(__fmul_rn((float)iy, vx.vs), __ldg(vx.origin + 1));
+  z = __fadd_rn(__fmul_rn((float)iz, vx.vs), __ldg(vx.origin + 2));
+}
+
 // acc[i][j] += sum_k A[k][m0+i] * B[k][n0+j];  A k-major with row stride TM, B row stride 128.
 template <int K>
 __device__ __forceinline__ void gemm_fwd(const float* __restrict__ sA, const float* __restrict__ sB,

@@ -19,12 +19,13 @@ namespace {
 
 using namespace sdfk;
 
-template <bool GRAD>
+// VOX: the points and latents come from VoxelSrc (o2345_sdf_voxels) instead of `src` + the trilinear fetch.
+template <bool GRAD, bool VOX>
 __global__ void __launch_bounds__(NT, 1)
 sdf_query_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, int D,
                  const float* __restrict__ wp, const uint8_t* __restrict__ active, float inactive_sdf,
                  float sign, float* __restrict__ o_sdf, float* __restrict__ o_feat,
-                 float* __restrict__ o_lat, float* __restrict__ o_grad) {
+                 float* __restrict__ o_lat, float* __restrict__ o_grad, VoxelSrc vx) {
   extern __shared__ __align__(16) float smem[];
   float* sAct = smem;                       // [144][TM]
   float* sW = sAct + SM_ACT;                // weights of the current layer / output staging
@@ -44,7 +45,7 @@ sdf_query_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, int
     const int64_t g0 = tile * TM;
     const int64_t gi = g0 + pm;
     // ---------------- stage 0: point, latent, embedding --------------------------------
-    bool act = gi < n && (active == nullptr || active[gi] != 0);
+    bool act = gi < n && (VOX ? __ldg(vx.occ + gi) > 0.f : (active == nullptr || active[gi] != 0));
     int any = __syncthreads_or(act ? 1 : 0);
     if (!any) {  // nothing to evaluate in this tile: defaults only (block-uniform branch)
       if (half == 0 && gi < n) {
@@ -57,7 +58,10 @@ sdf_query_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, int
       continue;
     }
     float px = 0.f, py = 0.f, pz = 0.f;
-    if (act) load_point(src, gi, px, py, pz);
+    if (act) {
+      if (VOX) voxel_point(vx, gi, D, px, py, pz);
+      else load_point(src, gi, px, py, pz);
+    }
     if (half == 0) {
       sPts[pm] = px, sPts[TM + pm] = py, sPts[2 * TM + pm] = pz;
       sFlag[pm] = act ? 1 : 0;
@@ -68,7 +72,12 @@ sdf_query_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, int
       float lat[8];
 #pragma unroll
       for (int c = 0; c < 8; ++c) lat[c] = 0.f;
-      if (act && t.inb) {
+      if (VOX) {
+        if (act) {
+          float4 v0 = ldg4(vol + gi * LAT + 8 * half), v1 = ldg4(vol + gi * LAT + 8 * half + 4);
+          lat[0] = v0.x, lat[1] = v0.y, lat[2] = v0.z, lat[3] = v0.w, lat[4] = v1.x, lat[5] = v1.y, lat[6] = v1.z, lat[7] = v1.w;
+        }
+      } else if (act && t.inb) {
 #pragma unroll
         for (int corner = 0; corner < 8; ++corner) {
           int dx = corner >> 2, dy = (corner >> 1) & 1, dz = corner & 1;
@@ -236,7 +245,8 @@ extern "C" int o2345_sdf_pack_weights(const float* w0, const float* b0, const fl
 
 namespace o2345 {
 int launch_sdf_query_tc(const o2345_points* src, int64_t n, const float* vol_cl, int D, const float* wpack, const uint8_t* active,
-                        float inactive_sdf, float sign, float* sdf, float* feat, float* latent, float* grad, cudaStream_t st);
+                        float inactive_sdf, float sign, float* sdf, float* feat, float* latent, float* grad, cudaStream_t st,
+                        const sdfk::VoxelSrc* vx);
 }
 
 extern "C" int o2345_sdf_query(const o2345_points* src, int64_t n, const float* vol_cl, int D,
@@ -253,19 +263,42 @@ extern "C" int o2345_sdf_query(const o2345_points* src, int64_t n, const float* 
   else O2345_CHECK_ARG(false, "unknown point source mode");
   if (precision == O2345_SDF_TC_SPLIT)
     return launch_sdf_query_tc(src, n, vol_cl, D, wpack, active, inactive_sdf, negate ? -1.f : 1.f, sdf, feat, latent, grad,
-                               (cudaStream_t)stream);
+                               (cudaStream_t)stream, nullptr);
   static PerDeviceOnce attr_done;
   if (attr_done.need()) {
-    O2345_CUDA(cudaFuncSetAttribute(sdf_query_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_FWD));
-    O2345_CUDA(cudaFuncSetAttribute(sdf_query_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_GRAD));
+    O2345_CUDA(cudaFuncSetAttribute(sdf_query_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_FWD));
+    O2345_CUDA(cudaFuncSetAttribute(sdf_query_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_GRAD));
   }
   int64_t ntiles = (n + TM - 1) / TM;
   int grid = (int)(ntiles < (int64_t)sm_count() ? ntiles : (int64_t)sm_count());
   float sign = negate ? -1.f : 1.f;
+  const VoxelSrc vx{};
   if (grad)
-    sdf_query_kernel<true><<<grid, NT, SMEM_GRAD, (cudaStream_t)stream>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat, latent, grad);
+    sdf_query_kernel<true, false><<<grid, NT, SMEM_GRAD, (cudaStream_t)stream>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat, latent, grad, vx);
   else
-    sdf_query_kernel<false><<<grid, NT, SMEM_FWD, (cudaStream_t)stream>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat, latent, grad);
+    sdf_query_kernel<false, false><<<grid, NT, SMEM_FWD, (cudaStream_t)stream>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat, latent, grad, vx);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+extern "C" int o2345_sdf_voxels(const float* occ, const float* vol_cl, int D, const float* origin, float voxel_size,
+                                const float* wpack, int precision, float* sdf_vol, o2345_stream_t stream) {
+  O2345_CHECK_ARG(occ && vol_cl && origin && wpack && sdf_vol, "null pointer");
+  O2345_CHECK_ARG(D >= 2 && D <= 1024, "volume side out of range");
+  O2345_CHECK_ARG(precision == O2345_SDF_FP32 || precision == O2345_SDF_TC_SPLIT, "unknown precision");
+  const int64_t n = (int64_t)D * D * D;
+  const VoxelSrc vx{occ, origin, voxel_size};
+  const o2345_points none{};
+  if (precision == O2345_SDF_TC_SPLIT)
+    return launch_sdf_query_tc(&none, n, vol_cl, D, wpack, nullptr, 1.f, 1.f, sdf_vol, nullptr, nullptr, nullptr,
+                               (cudaStream_t)stream, &vx);
+  static PerDeviceOnce attr_done;
+  if (attr_done.need())
+    O2345_CUDA(cudaFuncSetAttribute(sdf_query_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_FWD));
+  int64_t ntiles = (n + TM - 1) / TM;
+  int grid = (int)(ntiles < (int64_t)sm_count() ? ntiles : (int64_t)sm_count());
+  sdf_query_kernel<false, true><<<grid, NT, SMEM_FWD, (cudaStream_t)stream>>>(none, n, vol_cl, D, wpack, nullptr, 1.f, 1.f, sdf_vol,
+                                                                              nullptr, nullptr, nullptr, vx);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

@@ -188,11 +188,12 @@ __device__ __forceinline__ void store_activations(float (&acc)[2][8][4], __half*
     }
 }
 
-template <bool GRAD>
+// VOX: the points and latents come from VoxelSrc (o2345_sdf_voxels) instead of `src` + the trilinear fetch.
+template <bool GRAD, bool VOX>
 __global__ void __launch_bounds__(NT, 1)
 sdf_query_tc_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, int D, const float* __restrict__ wp,
                     const uint8_t* __restrict__ active, float inactive_sdf, float sign, float* __restrict__ o_sdf,
-                    float* __restrict__ o_feat, float* __restrict__ o_lat, float* __restrict__ o_grad) {
+                    float* __restrict__ o_feat, float* __restrict__ o_lat, float* __restrict__ o_grad, VoxelSrc vx) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sAh = reinterpret_cast<__half*>(smem_raw);
   __half* sAl = sAh + PLANE;
@@ -214,7 +215,7 @@ sdf_query_tc_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, 
     const int64_t g0 = tile * TM;
     const int64_t gi = g0 + pm;
     // ---------------- stage 0: point, latent, embedding (as sdf_query_kernel, written as hi / lo halves) -----------
-    bool act = gi < n && (active == nullptr || active[gi] != 0);
+    bool act = gi < n && (VOX ? __ldg(vx.occ + gi) > 0.f : (active == nullptr || active[gi] != 0));
     int any = __syncthreads_or(act ? 1 : 0);
     if (!any) {
       if (half == 0 && gi < n) {
@@ -227,7 +228,10 @@ sdf_query_tc_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, 
       continue;
     }
     float px = 0.f, py = 0.f, pz = 0.f;
-    if (act) load_point(src, gi, px, py, pz);
+    if (act) {
+      if (VOX) voxel_point(vx, gi, D, px, py, pz);
+      else load_point(src, gi, px, py, pz);
+    }
     if (half == 0) {
       sPts[pm] = px, sPts[TM + pm] = py, sPts[2 * TM + pm] = pz;
       sFlag[pm] = act ? 1 : 0;
@@ -242,7 +246,12 @@ sdf_query_tc_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, 
       float lat[8];
 #pragma unroll
       for (int c = 0; c < 8; ++c) lat[c] = 0.f;
-      if (act && t.inb) {
+      if (VOX) {
+        if (act) {
+          float4 v0 = ldg4(vol + gi * LAT + 8 * half), v1 = ldg4(vol + gi * LAT + 8 * half + 4);
+          lat[0] = v0.x, lat[1] = v0.y, lat[2] = v0.z, lat[3] = v0.w, lat[4] = v1.x, lat[5] = v1.y, lat[6] = v1.z, lat[7] = v1.w;
+        }
+      } else if (act && t.inb) {
 #pragma unroll
         for (int corner = 0; corner < 8; ++corner) {
           int dx = corner >> 2, dy = (corner >> 1) & 1, dz = corner & 1;
@@ -418,19 +427,27 @@ sdf_query_tc_kernel(o2345_points src, int64_t n, const float* __restrict__ vol, 
 
 }  // namespace
 
+// vx != nullptr: o2345_sdf_voxels (forward only; points and latents from *vx, `src` and `active` unused)
 int launch_sdf_query_tc(const o2345_points* src, int64_t n, const float* vol_cl, int D, const float* wpack, const uint8_t* active,
-                        float inactive_sdf, float sign, float* sdf, float* feat, float* latent, float* grad, cudaStream_t st) {
+                        float inactive_sdf, float sign, float* sdf, float* feat, float* latent, float* grad, cudaStream_t st,
+                        const VoxelSrc* vx) {
   static PerDeviceOnce attr_done;
   if (attr_done.need()) {
-    O2345_CUDA(cudaFuncSetAttribute(sdf_query_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TC_FWD));
-    O2345_CUDA(cudaFuncSetAttribute(sdf_query_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TC_GRAD));
+    O2345_CUDA(cudaFuncSetAttribute(sdf_query_tc_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TC_FWD));
+    O2345_CUDA(cudaFuncSetAttribute(sdf_query_tc_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TC_GRAD));
+    O2345_CUDA(cudaFuncSetAttribute(sdf_query_tc_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_TC_FWD));
   }
   int64_t tiles = (n + TM - 1) / TM;
   int grid = (int)(tiles < (int64_t)sm_count() ? tiles : (int64_t)sm_count());
-  if (grad)
-    sdf_query_tc_kernel<true><<<grid, NT, SMEM_TC_GRAD, st>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat, latent, grad);
+  if (vx)
+    sdf_query_tc_kernel<false, true><<<grid, NT, SMEM_TC_FWD, st>>>(*src, n, vol_cl, D, wpack, nullptr, inactive_sdf, sign, sdf, feat,
+                                                                    latent, nullptr, *vx);
+  else if (grad)
+    sdf_query_tc_kernel<true, false><<<grid, NT, SMEM_TC_GRAD, st>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat,
+                                                                     latent, grad, VoxelSrc{});
   else
-    sdf_query_tc_kernel<false><<<grid, NT, SMEM_TC_FWD, st>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat, latent, grad);
+    sdf_query_tc_kernel<false, false><<<grid, NT, SMEM_TC_FWD, st>>>(*src, n, vol_cl, D, wpack, active, inactive_sdf, sign, sdf, feat,
+                                                                     latent, grad, VoxelSrc{});
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

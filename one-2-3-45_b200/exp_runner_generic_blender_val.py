@@ -1,9 +1,11 @@
 """`python exp_runner_generic_blender_val.py --specific_dataset_name <exp_dir> --mode export_mesh --conf C --resolution R`
 
 Command-line mirror of the reference's reconstruction/exp_runner_generic_blender_val.py:596-640 for the two inference
-modes of the lod-0 demo configuration:
+modes of the demo configuration:
   export_mesh   <exp_dir>/{pose.json, stage1_8, stage2_8} -> <exp_dir>/mesh.ply   (what run.py's reconstruct() shells out to)
   val           volume-renders the query view -> <exp_dir>/val_color.png, val_depth.npy, val_normal.npy
+A conf with `model.num_lods = 2` adds the lod-1 level (`model.sdf_network_lod1`, `model.rendering_network_lod1`):
+export_mesh writes the lod-1 mesh, and val also writes val_color_lod1.png, val_depth_lod1.npy and val_normal_lod1.npy.
 `--conf` is parsed (o2345/checkpoints.py: the HOCON subset the reference's confs use; pyhocon is not needed) and supplies
 `model.sdf_network_lod0` (voxel_size, vol_dims, ...), `model.variance_network`, `model.rendering_network`, `model.trainer`
 (samples, perturb) and `general.base_exp_dir`; if the file does not exist the constants of
@@ -51,14 +53,17 @@ def main(argv=None):
     conf = load_conf(args.conf) if os.path.exists(args.conf) else None
     if conf is None:
         note(f"conf {args.conf!r} not found: using the built-in constants of confs/one2345_lod0_val_demo.conf")
+    num_lods = conf.get_int('model.num_lods') if conf is not None else 1
     states = S.all_states(0)
+    if num_lods > 1:
+        states.update(S.lod1_states(0))
     ckpt = args.checkpoint_path
     if ckpt is None and conf is not None and args.is_continue:
         ckpt = latest_checkpoint(conf['general.base_exp_dir'])
         if ckpt is not None:
             note(f"Find checkpoint: {os.path.basename(ckpt)}")
     if ckpt is not None:
-        states.update(recon_states(torch.load(ckpt, map_location="cpu"), report=note))
+        states.update(recon_states(torch.load(ckpt, map_location="cpu"), report=note, num_lods=num_lods))
     else:
         note("no checkpoint: seeded synthetic reconstruction weights")
     trainer = build_networks(dev, states=states, base_exp_dir=exp_dir, conf=conf,
@@ -72,12 +77,14 @@ def main(argv=None):
     # the reference's validate(); white background and alpha_inter_ratio 1.0 as at iter_step 215 000 (:412-418,528-540)
     # (512-ray chunks as in the reference: the host generator's draws -- jitter, then 1024 random points per chunk -- interleave
     # the same way)
-    out = trainer(sample, mode="val", background_rgb=1.0, alpha_inter_ratio_lod0=1.0)
+    out = trainer(sample, mode="val", background_rgb=1.0, alpha_inter_ratio_lod0=1.0, alpha_inter_ratio_lod1=1.0)
     W, H = int(sample['img_wh'][0][0]), int(sample['img_wh'][0][1])
     from PIL import Image
-    Image.fromarray((np.clip(out["color"].reshape(H, W, 3), 0, 1) * 255).astype(np.uint8)).save(os.path.join(exp_dir, "val_color.png"))
-    np.save(os.path.join(exp_dir, "val_depth.npy"), out["depth"].reshape(H, W))
-    np.save(os.path.join(exp_dir, "val_normal.npy"), out["normal"].reshape(H, W, 3))
+    for suffix in ("", "_lod1")[:num_lods]:
+        Image.fromarray((np.clip(out["color" + suffix].reshape(H, W, 3), 0, 1) * 255).astype(np.uint8)).save(
+            os.path.join(exp_dir, f"val_color{suffix}.png"))
+        np.save(os.path.join(exp_dir, f"val_depth{suffix}.npy"), out["depth" + suffix].reshape(H, W))
+        np.save(os.path.join(exp_dir, f"val_normal{suffix}.npy"), out["normal" + suffix].reshape(H, W, 3))
     print("val outputs written to", exp_dir)
     return out
 

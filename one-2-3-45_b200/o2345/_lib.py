@@ -56,6 +56,14 @@ _SIGS = {
     "o2345_costvol_gather": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp, C.c_float,
                                        C.c_int, c_fp, c_fp, c_i64, c_fp, c_fp, c_fp]),
     "o2345_dense_scatter": (C.c_int, [c_fp, c_fp, c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp]),
+    "o2345_sdf_voxels": (C.c_int, [c_fp, c_fp, C.c_int, c_fp, C.c_float, c_fp, C.c_int, c_fp, c_fp]),
+    "o2345_prune_by_sdf": (C.c_int, [c_fp, c_fp, C.c_int, C.POINTER(C.c_float), C.c_int, c_fp, c_fp, c_fp, c_fp]),
+    "o2345_prune_select": (C.c_int, [c_fp, c_i64, C.c_float, c_fp, c_fp]),
+    "o2345_clear_flags": (C.c_int, [c_fp, c_fp, c_i64, c_fp, c_fp]),
+    "o2345_gather_rows": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, C.c_int, c_fp, c_fp, c_fp]),
+    "o2345_lod_children": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp]),
+    "o2345_costvol_gather_lod": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp, C.c_float,
+                                           C.c_int, c_fp, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp, c_fp]),
     "o2345_occ_nearest": (C.c_int, [C.POINTER(Points), c_i64, c_fp, C.c_int, c_fp, c_fp]),
     "o2345_sp_coarsen": (C.c_int, [c_fp, C.c_int, c_fp, c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp]),
     "o2345_sp_conv": (C.c_int, [c_fp, c_fp, C.c_int, c_fp, c_fp, c_i64, C.c_int, C.c_int, c_fp, C.c_int, C.c_int,
@@ -121,7 +129,7 @@ _SIGS = {
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 3          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 4          # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 
@@ -160,7 +168,7 @@ def last_error() -> str:
 
 
 # kernels launched per successful entry-point call (memsets are not counted)
-_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4}
+_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4}
 _launches = 0
 
 

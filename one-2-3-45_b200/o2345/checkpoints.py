@@ -207,18 +207,27 @@ def latest_checkpoint(base_exp_dir):
 
 RECON_NETWORKS = {"pyramid_feature_network": "pyramid_feature_network", "sdf_network_lod0": "sdf_network_lod0",
                   "rendering_network_lod0": "rendering_network_lod0", "variance_network_lod0": "variance_network_lod0"}
+RECON_NETWORKS_LOD1 = {k: k for k in ("pyramid_feature_network_lod1", "sdf_network_lod1", "rendering_network_lod1",
+                                      "variance_network_lod1")}
 
 
-def recon_states(checkpoint: dict, report=None):
+def recon_states(checkpoint: dict, report=None, num_lods=1):
     """{network name -> state dict} for the four lod-0 networks of a `ckpt_*.pth` (the keys save_checkpoint writes,
     reference :480-503).  A network the file does not hold is reported ("<name> load fails", as the reference prints) and
-    left out, so that the caller keeps its initialisation -- the reference's behaviour, made visible."""
+    left out, so that the caller keeps its initialisation -- the reference's behaviour, made visible.  The four lod-1
+    networks are passed through when the file holds them; with num_lods = 2 a file that lacks one is refused (KeyError):
+    a lod-1 level with initial weights would refine the surface with noise."""
     out = {}
     for name, key in RECON_NETWORKS.items():
         if key in checkpoint and checkpoint[key] is not None:
             out[name] = checkpoint[key]
         elif report is not None:
             report(f"{key} load fails")
+    for name, key in RECON_NETWORKS_LOD1.items():
+        if checkpoint.get(key) is not None:
+            out[name] = checkpoint[key]
+        elif num_lods > 1:
+            raise KeyError(f"num_lods = 2 but the checkpoint has no {key!r}")
     return out
 
 

@@ -138,6 +138,76 @@ def costvol_gather(feats_nhwc, proj, origin, voxel_size, D, sizeH, sizeW, rows, 
     return cost
 
 
+def costvol_gather_lod(feats_nhwc, proj, origin, voxel_size, D, sizeH, sizeW, rows, count, bits, max_rows, parent, pre_feats):
+    """Cost rows [max_rows, 2C + 16] = [var(C), mean(C), pre_feats[parent[lin]]] for C = feats_nhwc.shape[-1] (8 or 16)."""
+    V, h, w, c = feats_nhwc.shape
+    cost = torch.empty(max_rows, 2 * c + 16, dtype=_f32, device=proj.device)
+    L.call("o2345_costvol_gather_lod", _f(feats_nhwc), c, V, h, w, int(sizeH), int(sizeW), _f(proj), _f(origin),
+           float(voxel_size), D, _p(rows, _i32), _p(count, _i32), max_rows, _p(bits, _i32), _p(parent, _i32), _f(pre_feats),
+           _f(cost), _stream())
+    return cost
+
+
+def sdf_voxels(occ, vol_cl, origin, voxel_size, pack, precision=None):
+    """[D^3] SDF of every occupied voxel (own latent row, no trilinear fetch), 1.0 elsewhere."""
+    precision = SDF_PRECISION if precision is None else precision
+    D = vol_cl.shape[0]
+    out = torch.empty(D ** 3, dtype=_f32, device=vol_cl.device)
+    L.call("o2345_sdf_voxels", _f(occ), _f(vol_cl), D, _f(origin), float(voxel_size), _f(pack), int(precision), _f(out),
+           _stream())
+    return out
+
+
+MAX_RUNGS = 16
+
+
+def prune_by_sdf(sdf, occ, D, ladder):
+    """-> minabs [D^3] (window minimum of |sdf|, +inf where occ == 0) and the host list of survivor counts per rung of
+    `ladder` (fp32 thresholds; one device-to-host copy per 16 rungs)."""
+    dev = sdf.device
+    minabs = torch.empty(D ** 3, dtype=_f32, device=dev)
+    scratch = torch.empty(D ** 3, dtype=_f32, device=dev)
+    counts = []
+    for k in range(0, len(ladder), MAX_RUNGS):
+        part = ladder[k:k + MAX_RUNGS]
+        arr = (C.c_float * len(part))(*part)
+        dcounts = torch.empty(len(part), dtype=_i32, device=dev)
+        L.call("o2345_prune_by_sdf", _f(sdf), _f(occ), D, arr, len(part), _f(scratch), _f(minabs), _p(dcounts, _i32),
+               _stream())
+        counts += dcounts.tolist()
+    return minabs, counts
+
+
+def prune_select(minabs, threshold):
+    keep = torch.empty(minabs.numel(), dtype=_u8, device=minabs.device)
+    L.call("o2345_prune_select", _f(minabs), minabs.numel(), float(threshold), _p(keep, _u8), _stream())
+    return keep
+
+
+def clear_flags(flags, rows, idx):
+    L.call("o2345_clear_flags", _p(rows, _i32), _p(idx, _i32), idx.numel(), _p(flags, _u8), _stream())
+
+
+def gather_rows(rows, n, D, vol_cf):
+    """coords [n,4] (0, x, y, z) and the channels of vol_cf [C, D^3] at the first n lattice indices of rows."""
+    Cc = vol_cf.shape[0]
+    coords = torch.empty(n, 4, dtype=_f32, device=rows.device)
+    feats = torch.empty(n, Cc, dtype=_f32, device=rows.device)
+    L.call("o2345_gather_rows", _p(rows, _i32), n, D, _f(vol_cf), Cc, _f(coords), _f(feats), _stream())
+    return coords, feats
+
+
+def lod_children(pre_coords, D1, frustum_keep):
+    """-> keep uint8 [D1^3] (children seen by > 1 views), parent int32 [D1^3].  Synchronises (argument check)."""
+    dev = pre_coords.device
+    keep = torch.empty(D1 ** 3, dtype=_u8, device=dev)
+    parent = torch.empty(D1 ** 3, dtype=_i32, device=dev)
+    err = torch.empty(1, dtype=_i32, device=dev)
+    L.call("o2345_lod_children", _f(pre_coords), pre_coords.shape[0], D1, _p(frustum_keep, _u8), _p(keep, _u8),
+           _p(parent, _i32), _p(err, _i32), _stream())
+    return keep, parent
+
+
 def dense_scatter(feat, rows, count, D, max_rows, want_cf=True):
     dev = feat.device
     vol_cl = torch.empty(D, D, D, 16, dtype=_f32, device=dev)

@@ -3,7 +3,7 @@
 `load_sample` mirrors BlenderPerView.__getitem__ (reference data/One2345_eval_new_data.py:139-377)
 for a folder written by run.py (pose.json, stage1_8/0.png, stage2_8/*.png); `synthetic_sample`
 builds the same dict from seeded inputs.  `build_networks` mirrors Runner.__init__ (reference
-exp_runner_generic_blender_val.py:93-151) for the lod-0 demo configuration.
+exp_runner_generic_blender_val.py:93-151) for the demo configuration, with one level (num_lods = 1) or two.
 """
 from __future__ import annotations
 
@@ -24,20 +24,35 @@ from .checkpoints import Conf  # noqa: E402,F401
 
 
 def build_networks(device, vol_dim=96, states=None, n_samples=64, n_importance=64, perturb=1.0, base_exp_dir=None,
-                   variance_init=0.3, conf=None):
+                   variance_init=0.3, conf=None, num_lods=None):
     """FeatureNet, SparseSdfNetwork, SingleVarianceNetwork, GeneralRenderingNetwork, GenericTrainer on `device`, assembled
     like Runner.__init__ (reference exp_runner_generic_blender_val.py:93-132).  With `conf` (a parsed
     confs/one2345_lod0_val_demo.conf) the constructor arguments come from it, exactly as the reference passes
     `**conf['model.sdf_network_lod0']` etc. -- including its 8-digit voxel_size 0.02105263; without it the same
-    constants are built in (voxel_size = 2 / (D - 1) in full precision)."""
-    fnet = FeatureNet()
+    constants are built in (voxel_size = 2 / (D - 1) in full precision).
+
+    num_lods = 2 (from the conf's model.num_lods, or the keyword without a conf) adds the lod-1 FeatureNet, SDF network,
+    variance network (built from model.variance_network, as the reference does) and rendering network; without a conf
+    the lod-1 volume has 2 D cells per side, voxel_size 2 / (2 D - 1) and 8 compressed channels (the demo conf's
+    sdf_network_lod1).  `states` must then also hold the lod-1 networks (o2345.synthetic.lod1_states)."""
     if conf is not None:
-        if conf.get_int('model.num_lods') != 1:
-            raise NotImplementedError("num_lods > 1 (the lod-1 refinement networks) is a 'next' row, SURVEY.md 8(f) item 3")
+        if num_lods is not None and num_lods != conf.get_int('model.num_lods'):
+            raise ValueError(f"num_lods={num_lods} contradicts the conf's model.num_lods={conf.get_int('model.num_lods')}")
+        num_lods = conf.get_int('model.num_lods')
+    num_lods = 1 if num_lods is None else num_lods
+    if num_lods not in (1, 2):
+        raise NotImplementedError(f"num_lods={num_lods}: 1 or 2 levels are on the accelerated path")
+    fnet = FeatureNet()
+    lod1 = {}
+    if conf is not None:
         sdf = SparseSdfNetwork(**conf['model.sdf_network_lod0'])
         var = SingleVarianceNetwork(**conf['model.variance_network'])
         rnet = GeneralRenderingNetwork(**conf['model.rendering_network'])
         tk = dict(conf['model.trainer'])
+        if num_lods > 1:
+            lod1 = {"sdf_network_lod1": SparseSdfNetwork(**conf['model.sdf_network_lod1']),
+                    "variance_network_lod1": SingleVarianceNetwork(**conf['model.variance_network']),
+                    "rendering_network_lod1": GeneralRenderingNetwork(**conf['model.rendering_network_lod1'])}
     else:
         sdf = SparseSdfNetwork(lod=0, ch_in=56, voxel_size=2.0 / (vol_dim - 1), vol_dims=[vol_dim] * 3, hidden_dim=128,
                                cost_type='variance_mean', d_pyramid_feature_compress=16, regnet_d_out=16,
@@ -46,20 +61,37 @@ def build_networks(device, vol_dim=96, states=None, n_samples=64, n_importance=6
         rnet = GeneralRenderingNetwork(in_geometry_feat_ch=16, in_rendering_feat_ch=56, anti_alias_pooling=True)
         tk = dict(n_samples_lod0=n_samples, n_importance_lod0=n_importance, n_samples_lod1=64, n_importance_lod1=64,
                   n_outside=0, perturb=perturb, alpha_type='div')
+        if num_lods > 1:
+            D1 = 2 * vol_dim
+            lod1 = {"sdf_network_lod1": SparseSdfNetwork(lod=1, ch_in=56, voxel_size=2.0 / (D1 - 1), vol_dims=[D1] * 3,
+                                                         hidden_dim=128, cost_type='variance_mean', d_pyramid_feature_compress=8,
+                                                         regnet_d_out=16, num_sdf_layers=4, multires=6),
+                    "variance_network_lod1": SingleVarianceNetwork(variance_init),
+                    "rendering_network_lod1": GeneralRenderingNetwork(in_geometry_feat_ch=16, in_rendering_feat_ch=56,
+                                                                      anti_alias_pooling=True)}
+    if num_lods > 1:
+        lod1["pyramid_feature_network_lod1"] = FeatureNet()
+        d0, d1 = sdf.vol_dims.tolist(), lod1["sdf_network_lod1"].vol_dims.tolist()
+        if d1 != [2 * d for d in d0]:
+            raise ValueError(f"the lod-1 vol_dims {d1} must be twice the lod-0 vol_dims {d0}")
     if states is not None:
         load = lambda m, sd: m.load_state_dict({k: torch.as_tensor(np.asarray(v)) for k, v in sd.items()}, strict=False)
         for m, key in ((fnet, "pyramid_feature_network"), (sdf, "sdf_network_lod0"), (rnet, "rendering_network_lod0"),
-                       (var, "variance_network_lod0")):
+                       (var, "variance_network_lod0"), *((m1, k1) for k1, m1 in lod1.items())):
+            if key not in states:
+                raise KeyError(f"no weights for {key!r} (num_lods = {num_lods})")
             res = load(m, states[key])
             assert not res.unexpected_keys, res.unexpected_keys
             assert all("num_batches_tracked" in k for k in res.missing_keys), res.missing_keys
-    for m in (fnet, sdf, var, rnet):
+    for m in (fnet, sdf, var, rnet, *lod1.values()):
         m.to(device)
         for p in m.parameters():
             p.requires_grad_(False)
     if conf is None:
-        conf = Conf({"general": Conf({"base_exp_dir": base_exp_dir}), "model": Conf({"num_lods": 1})})
-    trainer = GenericTrainer(None, fnet, None, sdf, None, var, None, rnet, None, tk["n_samples_lod0"], tk["n_importance_lod0"],
+        conf = Conf({"general": Conf({"base_exp_dir": base_exp_dir}), "model": Conf({"num_lods": num_lods})})
+    trainer = GenericTrainer(None, fnet, lod1.get("pyramid_feature_network_lod1"), sdf, lod1.get("sdf_network_lod1"), var,
+                             lod1.get("variance_network_lod1"), rnet, lod1.get("rendering_network_lod1"),
+                             tk["n_samples_lod0"], tk["n_importance_lod0"],
                              tk["n_samples_lod1"], tk["n_importance_lod1"], tk["n_outside"], tk["perturb"],
                              alpha_type=tk["alpha_type"], conf=conf, base_exp_dir=base_exp_dir)
     return trainer

@@ -160,6 +160,56 @@ class SparseNeuSRenderer(nn.Module):
             'mid_z_vals': mid,
         }
 
+    # ------------------------------------------------------------------ lod-0 pruning for the lod-1 level
+    @torch.no_grad()
+    def get_valid_sparse_coords_by_sdf(self, sdf_volume, coords_volume, mask_volume, feature_volume, threshold=0.02,
+                                       maximum_pts=110000):
+        """sdf_volume [1,X,Y,Z], coords_volume [3,X,Y,Z] (the lattice), mask_volume [1,X,Y,Z], feature_volume [C,X,Y,Z]
+        -> coords [N,4] (0, x, y, z) and features [N,C] of the surviving voxels in lattice order (reference :822-879).
+        coords_volume must be the lattice (coords_scale* of get_conditional_volume, interval 1): the kernels derive each
+        survivor's coordinates from its lattice index, so a volume of other coordinates is refused.
+
+        The reference prunes with avg_pool3d(|sdf| < t, 7, 1, 3) > 0 && mask and lowers t by 0.002 while more than
+        maximum_pts survive and t > 0.003.  Here one kernel pass counts the survivors of every rung of that ladder (built
+        with the same Python-double arithmetic; torch compares fp32 |sdf| with fp32(t)), and one copy brings the counts to
+        the host.  Above maximum_pts at the last rung, the same np.random.choice call as the reference's drops
+        survivors, so a caller who seeds numpy gets the reference's survivors."""
+        C, D = feature_volume.shape[0], feature_volume.shape[1]
+        if tuple(feature_volume.shape[1:]) != (D, D, D) or sdf_volume.numel() != D ** 3 or mask_volume.numel() != D ** 3:
+            raise ValueError("sdf_volume, mask_volume and feature_volume must describe the same D^3 lattice")
+        if tuple(coords_volume.shape) != (3, D, D, D) or not torch.equal(coords_volume, self._lattice(D, coords_volume.device)):
+            raise ValueError("coords_volume must be the [3, D, D, D] lattice of voxel indices (interval 1)")
+        ladder = [threshold]
+        t = threshold
+        while t > 0.003:
+            t = t - 0.002
+            ladder.append(t)
+        ladder32 = [float(np.float32(x)) for x in ladder]
+        minabs, counts = ops.prune_by_sdf(ops.cf32(sdf_volume).view(-1), ops.cf32(mask_volume).view(-1), D, ladder32)
+        r = 0
+        while counts[r] > maximum_pts and r + 1 < len(ladder):
+            r += 1
+        keep = ops.prune_select(minabs, ladder32[r])
+        rows, _, _ = ops.compact(keep)
+        n = counts[r]
+        if n > maximum_pts:
+            choice = np.random.choice(np.int64(n), n - maximum_pts, replace=False)
+            ops.clear_flags(keep, rows, torch.from_numpy(choice.astype(np.int32)).to(keep.device))
+            rows, _, _ = ops.compact(keep)
+            n = maximum_pts
+        self._last_prune = {"ladder": ladder32, "counts": counts, "rung": r, "keep": keep}
+        return ops.gather_rows(rows, n, D, ops.cf32(feature_volume).view(C, -1))
+
+    def _lattice(self, D, dev):
+        key = ("lattice", D, str(dev))
+        if key not in self._u:
+            r = torch.arange(D, dtype=torch.float32, device=dev)
+            self._u[key] = torch.stack(torch.meshgrid(r, r, r, indexing="ij"))
+        return self._u[key]
+
+    def get_valid_sparse_coords_by_sdf_depthfilter(self, *args, **kwargs):
+        raise NotImplementedError("prune_depth_filter (depth-map filtered pruning) is not on the accelerated path")
+
     # ------------------------------------------------------------------ B10
     @torch.no_grad()
     def extract_fields(self, bound_min, bound_max, resolution, query_func, device, **kwargs):

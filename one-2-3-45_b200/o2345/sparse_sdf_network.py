@@ -120,16 +120,19 @@ class SparseSdfNetwork(nn.Module):
                  cost_type='variance_mean', d_pyramid_feature_compress=16, regnet_d_out=8, num_sdf_layers=4,
                  multires=6):
         super().__init__()
-        if lod != 0:
-            raise NotImplementedError("only the lod-0 network is on the accelerated path (SURVEY.md 8(f) item 3)")
-        if d_pyramid_feature_compress != 16 or regnet_d_out != 16 or activation != 'softplus':
-            raise NotImplementedError("kernels are specialised for 16 compressed channels / 16 latent channels / softplus")
+        if lod not in (0, 1):
+            raise NotImplementedError("lod 0 and lod 1 (num_lods <= 2) are on the accelerated path")
+        if d_pyramid_feature_compress not in ((16,) if lod == 0 else (8, 16)) or regnet_d_out != 16 or activation != 'softplus':
+            raise NotImplementedError("kernels are specialised for 16 (lod 0) or 8 / 16 (lod 1) compressed channels, "
+                                      "16 latent channels and softplus")
         self.lod, self.ch_in, self.voxel_size = lod, ch_in, voxel_size
         self.vol_dims = torch.tensor(vol_dims)
         self.hidden_dim, self.cost_type = hidden_dim, cost_type
         self.d_pyramid_feature_compress, self.regnet_d_out, self.multires = d_pyramid_feature_compress, regnet_d_out, multires
         self.compress_layer = ConvBnReLU(ch_in, d_pyramid_feature_compress, 3, 1, 1)
-        self.sparse_costreg_net = SparseCostRegNet(d_in=2 * d_pyramid_feature_compress, d_out=regnet_d_out)
+        # lod > 0: the parent's 16 features join the variance / mean cost (reference :174-178)
+        d_in = 2 * d_pyramid_feature_compress + (16 if lod > 0 else 0)
+        self.sparse_costreg_net = SparseCostRegNet(d_in=d_in, d_out=regnet_d_out)
         self.sdf_layer = LatentSDFLayer(d_in=3, d_out=hidden_dim + 1, d_hidden=hidden_dim, n_layers=num_sdf_layers,
                                         multires=multires, d_conditional_feature=16)
         self._coords = None
@@ -139,32 +142,55 @@ class SparseSdfNetwork(nn.Module):
     def get_conditional_volume(self, feature_maps, partial_vol_origin, proj_mats, sizeH=None, sizeW=None, lod=0,
                                pre_coords=None, pre_feats=None):
         """feature_maps [1,V,C,H,W], partial_vol_origin [1,3], proj_mats [1,V,4,4] -> dict with
-        dense_volume_scale0 [1,16,D,D,D], valid_mask_volume_scale0 / visible_mask_scale0 [1,1,D,D,D],
-        coords_scale0 [1,3,D,D,D] (reference sparse_sdf_network.py:286-400)."""
+        dense_volume_scale{lod} [1,16,D,D,D], valid_mask_volume_scale{lod} / visible_mask_scale{lod} [1,1,D,D,D],
+        coords_scale{lod} [1,3,D,D,D] (reference sparse_sdf_network.py:286-400).  With lod 1 (the network's own lod,
+        as in the reference) the voxels are the 8 children of every row of pre_coords [N,4] (batch, x, y, z in this
+        lattice's units) seen by more than one view, and pre_feats [N,16] are their parents' features."""
         assert feature_maps.shape[0] == 1, "batch size 1 is assumed (as in the reference, :263)"
         dev = proj_mats.device
         D = int(self.vol_dims[0])
         V, _, H, W = feature_maps.shape[1:]
         sizeH = H if sizeH is None else int(sizeH)
         sizeW = W if sizeW is None else int(sizeW)
-        feats = torch.empty(V, H, W, 16, dtype=torch.float32, device=dev)
+        C = self.d_pyramid_feature_compress
+        feats = torch.empty(V, H, W, C, dtype=torch.float32, device=dev)
         self.compress_layer.run(feature_maps[0], out=feats, layout="nhwc")
         proj = ops.cf32(proj_mats[0])
         origin = ops.cf32(partial_vol_origin[0])
-        min_views = min(1, V - 1)
-        bits, keep = ops.frustum_mask(proj, origin, self.voxel_size, D, sizeH, sizeW, min_views)
-        rows, index, count = ops.compact(keep)
         n0 = D ** 3
-        cost = ops.costvol_gather(feats, proj, origin, self.voxel_size, D, sizeH, sizeW, rows, count, bits, n0)
-        level0 = ops.SparseLevel(D, rows, index, count, n0)
+        extra = {}
+        if self.lod == 0:
+            min_views = min(1, V - 1)
+            bits, keep = ops.frustum_mask(proj, origin, self.voxel_size, D, sizeH, sizeW, min_views)
+            rows, index, count = ops.compact(keep)
+            max_rows = n0
+            cost = ops.costvol_gather(feats, proj, origin, self.voxel_size, D, sizeH, sizeW, rows, count, bits, max_rows)
+        else:
+            if pre_coords is None or pre_feats is None:
+                raise ValueError("lod > 0 needs pre_coords and pre_feats (the pruned voxels of the previous lod)")
+            pre_coords, pre_feats = ops.cf32(pre_coords), ops.cf32(pre_feats)
+            if pre_coords.dim() != 2 or pre_coords.shape[1] != 4 or pre_feats.shape != (pre_coords.shape[0], 16):
+                raise ValueError(f"pre_coords must be [N,4] and pre_feats [N,16], got {tuple(pre_coords.shape)} / "
+                                 f"{tuple(pre_feats.shape)}")
+            if pre_coords.shape[0] == 0:
+                raise ValueError("no voxels survived the previous lod's pruning")
+            # `> 1` views, fixed (reference :355): the frustum test with min_views = 1 at this lattice
+            bits, fkeep = ops.frustum_mask(proj, origin, self.voxel_size, D, sizeH, sizeW, 1)
+            keep, parent = ops.lod_children(pre_coords, D, fkeep)
+            rows, index, count = ops.compact(keep)
+            max_rows = min(8 * pre_coords.shape[0], n0)
+            cost = ops.costvol_gather_lod(feats, proj, origin, self.voxel_size, D, sizeH, sizeW, rows, count, bits, max_rows,
+                                          parent, pre_feats)
+            extra = {"parent": parent, "frustum_keep": fkeep}
+        level0 = ops.SparseLevel(D, rows, index, count, max_rows)
         reg = self.sparse_costreg_net(cost, level0)
-        vol_cl, vol_cf, occ = ops.dense_scatter(reg, rows, count, D, n0)
+        vol_cl, vol_cf, occ = ops.dense_scatter(reg, rows, count, D, max_rows)
         vol_cf._o2345_cl = ((vol_cf.data_ptr(), vol_cf._version), vol_cl)
         if self._coords is None or self._coords.device != dev:
             r = torch.arange(D, dtype=torch.float32, device=dev)
             self._coords = torch.stack(torch.meshgrid(r, r, r, indexing="ij"))[None]
         self._last = {"mask_bits": bits, "keep": keep, "rows": rows, "index": index, "count": count, "cost": cost, "reg": reg,
-                      "feats_nhwc": feats}
+                      "feats_nhwc": feats, **extra}
         return {"dense_volume_scale%d" % self.lod: vol_cf, "valid_mask_volume_scale%d" % self.lod: occ,
                 "visible_mask_scale%d" % self.lod: occ, "coords_scale%d" % self.lod: self._coords}
 
@@ -185,5 +211,15 @@ class SparseSdfNetwork(nn.Module):
                             self.sdf_layer.packed(), want_grad=True)
         return out["grad"].unsqueeze(1)
 
-    def get_sdf_volume(self, *a, **k):
-        raise NotImplementedError("get_sdf_volume is only reached with num_lods > 1 (SURVEY.md 8(f) item 3)")
+    @inference_only
+    def get_sdf_volume(self, conditional_volume, mask_volume, coords_volume, partial_origin):
+        """[1,1,D,D,D]: the SDF MLP at every voxel with mask_volume > 0, at coords * voxel_size + partial_origin with
+        that voxel's own latent row, 1.0 elsewhere (reference :441-474).  coords_volume must be the lattice
+        (coords_scale* of get_conditional_volume): the kernel derives each voxel's coordinates from its index."""
+        vol_cl = channel_last_volume(conditional_volume)
+        D = vol_cl.shape[0]
+        if tuple(coords_volume.shape[-3:]) != (D, D, D) or mask_volume.numel() != D ** 3:
+            raise ValueError("conditional_volume, mask_volume and coords_volume must describe the same D^3 lattice")
+        sdf = ops.sdf_voxels(ops.cf32(mask_volume).view(-1), vol_cl, ops.cf32(partial_origin).view(-1), self.voxel_size,
+                             self.sdf_layer.packed())
+        return sdf.view(1, 1, D, D, D)

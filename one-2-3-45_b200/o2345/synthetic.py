@@ -48,14 +48,15 @@ def _bn(rng, c, prefix, sd, spread=0.15):
 
 
 def sdf_network_state(seed=0, ch_in=56, d_compress=16, regnet_d_out=16, hidden=128,
-                      multires=6, d_latent=16, perturb=0.05):
-    """Weights of SparseSdfNetwork (compress conv + sparse U-Net + weight-normed SDF MLP)."""
+                      multires=6, d_latent=16, perturb=0.05, parent_ch=0):
+    """Weights of SparseSdfNetwork (compress conv + sparse U-Net + weight-normed SDF MLP).  parent_ch = 16 for a lod > 0
+    network, whose U-Net input also carries the parent voxel's features."""
     rng = np.random.default_rng(seed)
     sd = {}
     fan = ch_in * 9
     sd["compress_layer.conv.weight"] = _uniform(rng, (d_compress, ch_in, 3, 3), 1.0 / math.sqrt(fan))
     _bn(rng, d_compress, "compress_layer.bn", sd)
-    for name, cin, cout in costreg_channels(2 * d_compress, regnet_d_out):
+    for name, cin, cout in costreg_channels(2 * d_compress + parent_ch, regnet_d_out):
         bound = 1.0 / math.sqrt((cout if name in ("conv7", "conv9", "conv11") else cin) * 27)
         sd[f"sparse_costreg_net.{name}.net.0.kernel"] = _uniform(rng, (27, cin, cout), bound)
         _bn(rng, cout, f"sparse_costreg_net.{name}.net.1", sd, spread=0.1)
@@ -152,6 +153,17 @@ def all_states(seed=0):
         "pyramid_feature_network": feature_net_state(seed + 1),
         "rendering_network_lod0": rendering_network_state(seed + 2),
         "variance_network_lod0": variance_network_state(),
+    }
+
+
+def lod1_states(seed=0):
+    """Weights of the four lod-1 networks of the demo conf (sdf_network_lod1: 8 compressed channels).  Separate from
+    all_states so that every lod-0 draw stays as it is."""
+    return {
+        "sdf_network_lod1": sdf_network_state(seed + 10, d_compress=8, parent_ch=16),
+        "pyramid_feature_network_lod1": feature_net_state(seed + 11),
+        "rendering_network_lod1": rendering_network_state(seed + 12),
+        "variance_network_lod1": variance_network_state(),
     }
 
 

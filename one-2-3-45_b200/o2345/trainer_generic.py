@@ -3,6 +3,10 @@
 Mirror of reference reconstruction/models/trainer_generic.py: constructor :18-125, forward dispatch
 :1052-1103, val_step :359-545, export_mesh_step :827-979, obtain_pyramid_feature_maps :1104-1125,
 validate_colored_mesh :1309-1380.  Training (`train_step`, losses) stays with the reference.
+
+With num_lods = 2 (the lod-1 refinement: a second, twice as fine volume built from the pruned lod-0 SDF) export_mesh
+writes and returns only the lod-1 coloured mesh.  The reference also builds the lod-0 coloured mesh first and writes it
+to the same <exp>/mesh.ply, which the lod-1 mesh then overwrites; that mesh is skipped here.
 """
 from __future__ import annotations
 
@@ -30,27 +34,44 @@ class GenericTrainer(nn.Module):
         self.conf, self.timestamp, self.base_exp_dir = conf, timestamp, base_exp_dir
         self.rendering_network_outside = rendering_network_outside
         self.pyramid_feature_network_geometry_lod0 = pyramid_feature_network_lod0
-        self.sdf_network_lod0 = sdf_network_lod0
-        self.variance_network_lod0 = variance_network_lod0
-        self.rendering_network_lod0 = rendering_network_lod0
+        self.pyramid_feature_network_geometry_lod1 = pyramid_feature_network_lod1
+        self.sdf_network_lod0, self.sdf_network_lod1 = sdf_network_lod0, sdf_network_lod1
+        self.variance_network_lod0, self.variance_network_lod1 = variance_network_lod0, variance_network_lod1
+        self.rendering_network_lod0, self.rendering_network_lod1 = rendering_network_lod0, rendering_network_lod1
         self.n_samples_lod0, self.n_importance_lod0 = n_samples_lod0, n_importance_lod0
+        self.n_samples_lod1, self.n_importance_lod1 = n_samples_lod1, n_importance_lod1
         self.n_outside, self.perturb, self.alpha_type = n_outside, perturb, alpha_type
-        self.num_lods = 1
-        if sdf_network_lod1 is not None:
-            raise NotImplementedError("num_lods > 1 is a 'next' row (SURVEY.md 8(f) item 3)")
+        self.num_lods = conf.get_int('model.num_lods')
+        if self.num_lods not in (1, 2):
+            raise NotImplementedError(f"num_lods={self.num_lods}: 1 or 2 levels are on the accelerated path")
+        self.prune_depth_filter = conf.get_bool('model.prune_depth_filter', default=False)
+        if self.prune_depth_filter:
+            raise NotImplementedError("model.prune_depth_filter (depth-map filtered pruning) is not on the accelerated path")
         self.sdf_renderer_lod0 = SparseNeuSRenderer(rendering_network_outside, sdf_network_lod0, variance_network_lod0,
                                                     rendering_network_lod0, n_samples_lod0, n_importance_lod0,
                                                     n_outside, perturb, alpha_type='div', conf=conf)
+        self.sdf_renderer_lod1 = None
+        if self.num_lods > 1:
+            missing = [n for n, m in (("pyramid_feature_network_lod1", pyramid_feature_network_lod1),
+                                      ("sdf_network_lod1", sdf_network_lod1), ("variance_network_lod1", variance_network_lod1),
+                                      ("rendering_network_lod1", rendering_network_lod1)) if m is None]
+            if missing:
+                raise ValueError(f"num_lods = 2 needs {', '.join(missing)}")
+            self.sdf_renderer_lod1 = SparseNeuSRenderer(rendering_network_outside, sdf_network_lod1, variance_network_lod1,
+                                                        rendering_network_lod1, n_samples_lod1, n_importance_lod1,
+                                                        n_outside, perturb, alpha_type='div', conf=conf)
         self.val_mesh_freq = 1
 
     def obtain_pyramid_feature_maps(self, imgs, lod=0):
-        return obtain_pyramid_feature_maps(self.pyramid_feature_network_geometry_lod0, imgs)
+        extractor = self.pyramid_feature_network_geometry_lod0 if lod == 0 else self.pyramid_feature_network_geometry_lod1
+        return obtain_pyramid_feature_maps(extractor, imgs)
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
                 alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
-                                 alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, iter_step=iter_step, save_vis=save_vis)
+                                 alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
+                                 iter_step=iter_step, save_vis=save_vis)
         if mode == 'export_mesh':
             return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution)
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
@@ -66,6 +87,21 @@ class GenericTrainer(nn.Module):
             proj_mats=sample['affine_mats'], sizeH=sizeH, sizeW=sizeW, lod=0)
         return imgs, fmaps, cond, sizeW, sizeH
 
+    @torch.no_grad()
+    def _lod1_volume(self, sample, imgs, cond, sizeW, sizeH):
+        """lod-0 SDF volume -> pruned lod-0 voxels -> lod-1 conditional volume (reference :897-932); also returns the
+        lod-1 feature maps."""
+        origin = sample['partial_vol_origin']
+        vol0, occ0, coords0 = cond['dense_volume_scale0'], cond['valid_mask_volume_scale0'], cond['coords_scale0']
+        sdf0 = self.sdf_network_lod0.get_sdf_volume(vol0, occ0, coords0, origin)
+        fmaps1 = self.obtain_pyramid_feature_maps(imgs, lod=1)
+        pre_coords, pre_feats = self.sdf_renderer_lod0.get_valid_sparse_coords_by_sdf(sdf0[0], coords0[0], occ0[0], vol0[0])
+        pre_coords[:, 1:] = pre_coords[:, 1:] * 2
+        cond1 = self.sdf_network_lod1.get_conditional_volume(
+            feature_maps=fmaps1[None], partial_vol_origin=origin, proj_mats=sample['affine_mats'], sizeH=sizeH, sizeW=sizeW,
+            pre_coords=pre_coords, pre_feats=pre_feats)
+        return fmaps1, cond1
+
     # ------------------------------------------------------------------ mode='val'
     @torch.no_grad()
     def val_step(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
@@ -74,29 +110,47 @@ class GenericTrainer(nn.Module):
         like the per-chunk host copies of the reference (:526-543) but with one copy at the end.
         `chunk_size` rays are marched per launch group (the reference uses 512; larger is faster)."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
-        vol, occ = cond['dense_volume_scale0'], cond['valid_mask_volume_scale0']
+        levels = [("", self.sdf_renderer_lod0, self.sdf_network_lod0, self.rendering_network_lod0, alpha_inter_ratio_lod0,
+                   cond['dense_volume_scale0'], cond['valid_mask_volume_scale0'], fmaps)]
+        if self.num_lods > 1:
+            fmaps1, cond1 = self._lod1_volume(sample, imgs, cond, sizeW, sizeH)
+            levels.append(("_lod1", self.sdf_renderer_lod1, self.sdf_network_lod1, self.rendering_network_lod1,
+                           alpha_inter_ratio_lod1, cond1['dense_volume_scale1'], cond1['valid_mask_volume_scale1'], fmaps1))
         near, far = sample['query_near_far'][0, :1], sample['query_near_far'][0, 1:]
         rays_o = sample['rays']['rays_o'][0].reshape(-1, 3)
         rays_d = sample['rays']['rays_v'][0].reshape(-1, 3)
-        colors, depths, normals = [], [], []
-        for ro, rd in zip(rays_o.split(chunk_size), rays_d.split(chunk_size)):
-            out = self.sdf_renderer_lod0.render(
-                ro, rd, near, far, self.sdf_network_lod0, self.rendering_network_lod0,
-                perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
-                alpha_inter_ratio=alpha_inter_ratio_lod0, lod=0, conditional_volume=vol,
-                conditional_valid_mask_volume=occ, feature_maps=fmaps, color_maps=imgs, w2cs=sample['w2cs'][0],
-                intrinsics=sample['intrinsics'][0], img_wh=[sizeW, sizeH], query_c2w=sample['query_c2w'],
-                if_render_with_grad=False)
-            colors.append(out['color_fine'])
-            depths.append(out['depth'])
-            normals.append((out['gradients'] * out['weights'][:, :, None] * out['inside_sphere'][..., None]).sum(dim=1))
-        return {"color": torch.cat(colors).cpu().numpy(), "depth": torch.cat(depths).cpu().numpy(),
-                "normal": torch.cat(normals).cpu().numpy()}
+        result = {}
+        # every chunk of lod 0, then every chunk of lod 1 (reference :503-589): the host generator's draws follow that order
+        for lod, (suffix, renderer, sdf_net, rnet, ratio, vol, occ, fm) in enumerate(levels):
+            colors, depths, normals = [], [], []
+            for ro, rd in zip(rays_o.split(chunk_size), rays_d.split(chunk_size)):
+                out = renderer.render(
+                    ro, rd, near, far, sdf_net, rnet, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
+                    alpha_inter_ratio=ratio, lod=lod, conditional_volume=vol, conditional_valid_mask_volume=occ,
+                    feature_maps=fm, color_maps=imgs, w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
+                    img_wh=[sizeW, sizeH], query_c2w=sample['query_c2w'], if_render_with_grad=False)
+                colors.append(out['color_fine'])
+                depths.append(out['depth'])
+                normals.append((out['gradients'] * out['weights'][:, :, None] * out['inside_sphere'][..., None]).sum(dim=1))
+            result.update({"color" + suffix: torch.cat(colors).cpu().numpy(), "depth" + suffix: torch.cat(depths).cpu().numpy(),
+                           "normal" + suffix: torch.cat(normals).cpu().numpy()})
+        return result
 
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False):
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
+        if self.num_lods > 1:
+            # the lod-1 mesh is coloured with the lod-0 feature maps, as in the reference (:959-978)
+            _, cond1 = self._lod1_volume(sample, imgs, cond, sizeW, sizeH)
+            return self.validate_colored_mesh(
+                density_or_sdf_network=self.sdf_network_lod1,
+                func_extract_geometry=self.sdf_renderer_lod1.extract_geometry, resolution=resolution,
+                conditional_volume=cond1['dense_volume_scale1'],
+                conditional_valid_mask_volume=cond1['valid_mask_volume_scale1'], feature_maps=fmaps, color_maps=imgs,
+                w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
+                rendering_network=self.rendering_network_lod1, lod=1, threshold=0, query_c2w=sample['query_c2w'],
+                scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH])
         return self.validate_colored_mesh(
             density_or_sdf_network=self.sdf_network_lod0,
             func_extract_geometry=self.sdf_renderer_lod0.extract_geometry, resolution=resolution,
@@ -119,8 +173,9 @@ class GenericTrainer(nn.Module):
             density_or_sdf_network, bmin, bmax, resolution=resolution, threshold=threshold,
             device=conditional_volume.device, conditional_volume=conditional_volume, lod=lod,
             occupancy_mask=occupancy_mask)
+        renderer = self.sdf_renderer_lod1 if lod == 1 else self.sdf_renderer_lod0
         vt = torch.tensor(vertices).to(conditional_volume)
-        rgb, _ = self.sdf_renderer_lod0.blend_points(vt, density_or_sdf_network, rendering_network, conditional_volume,
+        rgb, _ = renderer.blend_points(vt, density_or_sdf_network, rendering_network, conditional_volume,
                                                      conditional_valid_mask_volume, feature_maps, color_maps, w2cs,
                                                      intrinsics, img_wh)
         if scale_mat is not None:
@@ -135,7 +190,7 @@ class GenericTrainer(nn.Module):
         # before the export (reference :1374-1380).  Marching-cubes vertices can only coincide on lattice points: the renderer
         # listed the vertices that sit on one (on the device), and only those are compared.
         vertices, triangles, colors = merge_vertices(vertices, triangles, colors,
-                                                     candidates=getattr(self.sdf_renderer_lod0, "mc_lattice_candidates", None))
+                                                     candidates=getattr(renderer, "mc_lattice_candidates", None))
         if self.base_exp_dir is not None:
             os.makedirs(self.base_exp_dir, exist_ok=True)
             write_ply(os.path.join(self.base_exp_dir, 'mesh.ply'), vertices, triangles, colors)
