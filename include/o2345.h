@@ -32,9 +32,10 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 4   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 5   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
-                                 4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...) */
+                                 4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
+                                 5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone */
 
 typedef void* o2345_stream_t;
 
@@ -284,10 +285,9 @@ typedef struct o2345_views {
  * MLP -> rgb [n,3]; nvalid [n] = number of views whose mask is set (may be NULL).  dir_mode 0: target
  * direction = normalised (query_center - p) (Projector.compute); 1: dirs [n,3] given
  * (compute_view_independent, surface normals).  rnet_pack: O2345_RNET_PACK_FLOATS floats, every
- * matrix stored [in][out] in the order documented in csrc/render.cu. */
+ * matrix stored [in][out] in the order documented in csrc/blend_common.cuh. */
 #define O2345_BLEND_FP32 0     /* fp32 FMA mat-vecs in the reference's operation order (tight oracle parity)            */
 #define O2345_BLEND_TC_FP16 1  /* per-(sample, view) MLPs as mma.sync products: fp16 operands, fp32 accumulate / statistics */
-#define O2345_BLEND_TC5 2      /* the same MLPs as wgmma M = 128 tiles (4 samples x 32 views, a lane is a view) */
 int o2345_render_blend(const o2345_points* src, int64_t n, const uint8_t* active, const float* vol_cl,
                        const float* occ, int D, const o2345_views* views, int dir_mode, const float* query_center,
                        const float* dirs, const float* rnet_pack, int precision, float* rgb, int32_t* nvalid,

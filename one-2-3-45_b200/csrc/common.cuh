@@ -51,6 +51,26 @@ int sm_count();
 
 __device__ __forceinline__ float4 ldg4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 
+// Point gi of a point source (explicit list, lattice or ray samples).
+__device__ __forceinline__ void load_point(const o2345_points& src, int64_t gi, float& x, float& y, float& z) {
+  if (src.mode == O2345_PTS_EXPLICIT) {
+    x = __ldg(src.pts + 3 * gi), y = __ldg(src.pts + 3 * gi + 1), z = __ldg(src.pts + 3 * gi + 2);
+  } else if (src.mode == O2345_PTS_LATTICE) {
+    int R = src.R;
+    int64_t ix = gi / ((int64_t)R * R);
+    int iy = (int)((gi / R) % R), iz = (int)(gi % R);
+    x = __ldg(src.lin + ix), y = __ldg(src.lin + iy), z = __ldg(src.lin + iz);
+  } else {
+    int64_t r = gi / src.S;
+    int s = (int)(gi - r * src.S);
+    float t = __ldg(src.z + r * src.z_stride + s);
+    // o + d * t with separately rounded multiply and add (torch evaluates it that way)
+    x = __fadd_rn(__ldg(src.rays_o + 3 * r), __fmul_rn(__ldg(src.rays_d + 3 * r), t));
+    y = __fadd_rn(__ldg(src.rays_o + 3 * r + 1), __fmul_rn(__ldg(src.rays_d + 3 * r + 1), t));
+    z = __fadd_rn(__ldg(src.rays_o + 3 * r + 2), __fmul_rn(__ldg(src.rays_d + 3 * r + 2), t));
+  }
+}
+
 // Programmatic dependent launch (PDL).  The ~660 kernels of a UNet pass are launched with programmatic stream
 // serialization: kernel N+1 may be scheduled while kernel N drains, runs its prologue (barrier init, descriptor prefetch,
 // index math) and then blocks in pdl_wait() until kernel N has completed and flushed its writes.

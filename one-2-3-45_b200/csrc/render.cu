@@ -15,10 +15,12 @@
 //                         193-wide first layer is split into a per-sample part (geometry, mean,
 //                         variance) and a 59-wide per-view part.
 //   ray_composite_kernel  one thread per ray: NeuS alpha, transmittance, colour / depth.
+#include "blend_common.cuh"
 #include "common.cuh"
 
 namespace o2345 {
 namespace {
+using namespace rpack;
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
 // Blend-network activations: ex2.approx based (absolute error <= 3e-7 on values of O(1), far below the
@@ -146,38 +148,6 @@ __global__ void ray_mid_kernel(const float* __restrict__ rays_o, const float* __
 // B11/B12: projector + GeneralRenderingNetwork
 // ---------------------------------------------------------------------------------------
 constexpr int BW = 24;             // warps per CTA
-constexpr int CM = O2345_MAP_CH;   // 60 channels per pixel: rgb(3) + feat(56) + pad(1)
-constexpr int NF = 59;
-
-// packed weights (floats), all matrices stored [in][out]
-constexpr int P_D0W = 0;                    // [4][16]
-constexpr int P_D0B = P_D0W + 64;           // [16]
-constexpr int P_D1W = P_D0B + 16;           // [16][64]  (59 used)
-constexpr int P_D1B = P_D1W + 1024;         // [64]
-constexpr int P_B0W = P_D1B + 64;           // [193][64]: rows 0..15 geo, 16..74 mean, 75..133 var, 134..192 feat
-constexpr int P_B0B = P_B0W + 193 * 64;     // [64]
-constexpr int P_B1W = P_B0B + 64;           // [64][32]
-constexpr int P_B1B = P_B1W + 2048;         // [32]
-constexpr int P_V0W = P_B1B + 32;           // [32][32]
-constexpr int P_V0B = P_V0W + 1024;         // [32]
-constexpr int P_V1W = P_V0B + 32;           // [32][32]  residual outputs
-constexpr int P_V1B = P_V1W + 1024;         // [32]
-constexpr int P_V1V = P_V1B + 32;           // [32]      visibility output row
-constexpr int P_V1VB = P_V1V + 32;          // [4]       its bias (first element)
-constexpr int P_U0W = P_V1VB + 4;           // [32][32]
-constexpr int P_U0B = P_U0W + 1024;         // [32]
-constexpr int P_U1W = P_U0B + 32;           // [32]
-constexpr int P_U1B = P_U1W + 32;           // [4]
-constexpr int P_R0W = P_U1B + 4;            // [37][16]
-constexpr int P_R0B = P_R0W + 592;          // [16]
-constexpr int P_R1W = P_R0B + 16;           // [16][8]
-constexpr int P_R1B = P_R1W + 128;          // [8]
-constexpr int P_R2W = P_R1B + 8;            // [8]
-constexpr int P_R2B = P_R2W + 8;            // [4]
-constexpr int P_S = P_R2B + 4;              // [4]  |s|
-constexpr int P_TOTAL = P_S + 4;
-static_assert(P_TOTAL == O2345_RNET_PACK_FLOATS, "header and kernel disagree on the rendering-net pack");
-
 constexpr int WS_X = 512;                   // per-warp: two [64][4] activation buffers
 constexpr int WS_RGB = 32 * 4;              // per-warp: rgb of each view
 constexpr int WS_TOTAL = WS_X + WS_RGB;
@@ -220,12 +190,6 @@ __device__ __forceinline__ void matvec4(const float* __restrict__ W, const float
   }
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // bilinear (zeros padding, align_corners=True) of channels {lane, lane+32} at normalised (gx, gy)
 __device__ __forceinline__ void fetch_map(const float* __restrict__ map, int H, int W, float gx, float gy, int lane,
                                           float& f0, float& f1) {
@@ -245,30 +209,15 @@ __device__ __forceinline__ void fetch_map(const float* __restrict__ map, int H, 
   if (iny1 && inx1) { f0 = fmaf(__ldg(base + (int64_t)W * CM + CM + lane), wse, f0); if (c1) f1 = fmaf(__ldg(base + (int64_t)W * CM + CM + lane + 32), wse, f1); }
 }
 
-__device__ __forceinline__ void sample_point(const o2345_points& src, int64_t gi, float& x, float& y, float& z) {
-  if (src.mode == O2345_PTS_EXPLICIT) {
-    x = __ldg(src.pts + 3 * gi), y = __ldg(src.pts + 3 * gi + 1), z = __ldg(src.pts + 3 * gi + 2);
-  } else {
-    int64_t r = gi / src.S;
-    int s = (int)(gi - r * src.S);
-    float t = __ldg(src.z + r * src.z_stride + s);
-    x = __fadd_rn(__ldg(src.rays_o + 3 * r), __fmul_rn(__ldg(src.rays_d + 3 * r), t));
-    y = __fadd_rn(__ldg(src.rays_o + 3 * r + 1), __fmul_rn(__ldg(src.rays_d + 3 * r + 1), t));
-    z = __fadd_rn(__ldg(src.rays_o + 3 * r + 2), __fmul_rn(__ldg(src.rays_d + 3 * r + 2), t));
-  }
-}
-
 // Features of up to four valid views (slots g0..g0+3 of the `valid` mask): bilinear fetch of the 59 channels
 // (lanes own channels lane and lane+32) plus the direction feature ray_dir_fc(ray_diff) (reference
 // rendering_network.py:44-47,88-90).  Padded slots return zeros and weight 0.  If sRGB != nullptr the original
 // colours of the views are stored at sRGB[slot*4 + c].
-__device__ __forceinline__ void view_group_features(const o2345_views& views, unsigned valid, int g0, int nvalid, float wv,
-                                                    float gx, float gy, float rd0, float rd1, float rd2, float rd3,
-                                                    const float* __restrict__ sP, float* sA4, float* sB4, int lane,
+__device__ __forceinline__ void view_group_features(const o2345_views& views, const BlendSample& s, int g0, const float* __restrict__ sP, float* sA4, float* sB4, int lane,
                                                     int (&vid)[4], float (&wq)[4], float (&a0)[4], float (&a1)[4],
                                                     float* sRGB) {
   const int H = views.H, W = views.W;
-  unsigned m = valid;
+  unsigned m = s.valid;
   for (int k = 0; k < g0; ++k) m &= m - 1;
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
@@ -279,11 +228,11 @@ __device__ __forceinline__ void view_group_features(const o2345_views& views, un
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
     int vq = vid[q] >= 0 ? vid[q] : 0;
-    wq[q] = vid[q] >= 0 ? __shfl_sync(0xffffffffu, wv, vq) : 0.f;
-    float vgx = __shfl_sync(0xffffffffu, gx, vq), vgy = __shfl_sync(0xffffffffu, gy, vq);
+    wq[q] = vid[q] >= 0 ? __shfl_sync(0xffffffffu, s.wv, vq) : 0.f;
+    float vgx = __shfl_sync(0xffffffffu, s.gx, vq), vgy = __shfl_sync(0xffffffffu, s.gy, vq);
     fetch_map(views.maps + (int64_t)vq * H * W * CM, H, W, vgx, vgy, lane, f0[q], f1[q]);
-    float r0 = __shfl_sync(0xffffffffu, rd0, vq), r1 = __shfl_sync(0xffffffffu, rd1, vq);
-    float r2 = __shfl_sync(0xffffffffu, rd2, vq), r3 = __shfl_sync(0xffffffffu, rd3, vq);
+    float r0 = __shfl_sync(0xffffffffu, s.rd0, vq), r1 = __shfl_sync(0xffffffffu, s.rd1, vq);
+    float r2 = __shfl_sync(0xffffffffu, s.rd2, vq), r3 = __shfl_sync(0xffffffffu, s.rd3, vq);
     if (lane == 0) sA4[0 * 4 + q] = r0, sA4[1 * 4 + q] = r1, sA4[2 * 4 + q] = r2, sA4[3 * 4 + q] = r3;
   }
   __syncwarp();
@@ -297,7 +246,7 @@ __device__ __forceinline__ void view_group_features(const o2345_views& views, un
   matvec4<16, 64, 64>(sP + P_D1W, sB4, lane, sP[P_D1B + lane], sP[P_D1B + 32 + lane], d0, d1);
 #pragma unroll
   for (int q = 0; q < 4; ++q) {
-    bool on = g0 + q < nvalid;
+    bool on = g0 + q < s.nvalid;
     if (on && sRGB != nullptr && lane < 3) sRGB[(g0 + q) * 4 + lane] = f0[q];
     a0[q] = on ? f0[q] + eluf_(d0[q]) : 0.f;
     a1[q] = (on && lane + 32 < NF) ? f1[q] + eluf_(d1[q]) : 0.f;
@@ -321,86 +270,15 @@ render_blend_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ act
   const float abs_s = sP[P_S];
 
   for (int64_t gi = (int64_t)blockIdx.x * BW + warp; gi < n; gi += (int64_t)gridDim.x * BW) {
-    if (active && active[gi] == 0) {  // weight of this sample is exactly 0 in the compositing
-      if (lane < 3) rgb_out[3 * gi + lane] = 0.f;
-      if (lane == 0 && nvalid_out) nvalid_out[gi] = 0;
-      continue;
-    }
-    float px, py, pz;
-    sample_point(src, gi, px, py, pz);
-    // ---- geometry feature (ATen trilinear, zeros padding, align_corners=True) + occupancy
-    //      (reference render_utils.py:54-85, projector.py:168-183)
-    float geo = 0.f, occv = 0.f;
-    {
-      float p[3] = {px, py, pz};
-      float f[3], w1[3];
-      bool fin = true;
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        float t = ((p[a] + 1.f) / 2.f) * (float)(D - 1);
-        f[a] = floorf(t);
-        w1[a] = t - f[a];
-        fin = fin && (f[a] >= -1.f) && (f[a] <= (float)(D - 1));
-      }
-      if (fin) {
-#pragma unroll
-        for (int corner = 0; corner < 8; ++corner) {
-          int dx = corner >> 2, dy = (corner >> 1) & 1, dz = corner & 1;
-          int ix = (int)f[0] + dx, iy = (int)f[1] + dy, iz = (int)f[2] + dz;
-          if (ix < 0 || iy < 0 || iz < 0 || ix >= D || iy >= D || iz >= D) continue;
-          float w = (dx ? w1[0] : 1.f - w1[0]) * (dy ? w1[1] : 1.f - w1[1]) * (dz ? w1[2] : 1.f - w1[2]);
-          int64_t cell = ((int64_t)ix * D + iy) * D + iz;
-          if (lane < 16) geo = fmaf(__ldg(vol + cell * 16 + lane), w, geo);
-          occv = fmaf(__ldg(occ + cell), w, occv);
-        }
-      }
-    }
-    const bool gmask = (fabsf(px) < 1.f) && (fabsf(py) < 1.f) && (fabsf(pz) < 1.f) && (occv > 0.f);
-    // ---- lanes as views: projection, mask, ray difference, pooling weight
-    float gx = 2.f, gy = 2.f, rd0 = 0.f, rd1 = 0.f, rd2 = 0.f, rd3 = 0.f, ev = 3.4e38f;
-    bool vmask = false;
-    float tx, ty, tz;  // target direction (camera-to-point for rendering, normal for vertex colours)
-    if (dir_mode == 0) {
-      tx = query_center[0] - px, ty = query_center[1] - py, tz = query_center[2] - pz;
-      float nn = sqrtf(tx * tx + ty * ty + tz * tz) + 1e-6f;
-      tx /= nn, ty /= nn, tz /= nn;
-    } else {
-      tx = dirs[3 * gi], ty = dirs[3 * gi + 1], tz = dirs[3 * gi + 2];
-    }
-    if (lane < V) {
-      const float* P = views.proj + 12 * lane;
-      float X = P[0] * px + P[1] * py + P[2] * pz + P[3];
-      float Y = P[4] * px + P[5] * py + P[6] * pz + P[7];
-      float Z = fmaxf(P[8] * px + P[9] * py + P[10] * pz + P[11], 1e-3f);
-      gx = 2.f * (X / Z) / (views.sizeW - 1.f) - 1.f;
-      gy = 2.f * (Y / Z) / (views.sizeH - 1.f) - 1.f;
-      if (!(gx <= 1.f && gx >= -1.f)) gx = 2.f;
-      if (!(gy <= 1.f && gy >= -1.f)) gy = 2.f;
-      vmask = gmask && (fabsf(gx) < 1.f) && (fabsf(gy) < 1.f);
-      float cx = views.centers[3 * lane] - px, cy = views.centers[3 * lane + 1] - py, cz = views.centers[3 * lane + 2] - pz;
-      float nn = sqrtf(cx * cx + cy * cy + cz * cz) + 1e-6f;
-      cx /= nn, cy /= nn, cz /= nn;
-      float ddx = tx - cx, ddy = ty - cy, ddz = tz - cz;
-      float dn = fmaxf(sqrtf(ddx * ddx + ddy * ddy + ddz * ddz), 1e-6f);
-      rd0 = ddx / dn, rd1 = ddy / dn, rd2 = ddz / dn;
-      rd3 = tx * cx + ty * cy + tz * cz;
-      ev = expf(abs_s * (rd3 - 1.f));
-    }
-    float emin = ev;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) emin = fminf(emin, __shfl_xor_sync(0xffffffffu, emin, o));
-    float wv = vmask ? (ev - emin) : 0.f;
-    float wtot = warp_sum(wv);
-    wv = wv / (wtot + 1e-8f);
-    const unsigned valid = __ballot_sync(0xffffffffu, vmask);
-    const int nvalid = __popc(valid);
-    if (lane == 0 && nvalid_out) nvalid_out[gi] = nvalid;
+    if (skip_inactive(active, gi, lane, rgb_out, nvalid_out)) continue;
+    const BlendSample s = blend_front_end(src, gi, vol, occ, D, views, dir_mode, query_center, dirs, abs_s, lane);
+    if (lane == 0 && nvalid_out) nvalid_out[gi] = s.nvalid;
 
-    if (nvalid == 0) {
+    if (s.nvalid == 0) {
       // every logit is -1e9: softmax is uniform over ALL views (reference rendering_network.py:119-121)
       float r = 0.f, g = 0.f, b = 0.f;
       for (int v = 0; v < V; ++v) {
-        float vgx = __shfl_sync(0xffffffffu, gx, v), vgy = __shfl_sync(0xffffffffu, gy, v);
+        float vgx = __shfl_sync(0xffffffffu, s.gx, v), vgy = __shfl_sync(0xffffffffu, s.gy, v);
         float f0, f1;
         fetch_map(views.maps + (int64_t)v * H * W * CM, H, W, vgx, vgy, lane, f0, f1);
         r += __shfl_sync(0xffffffffu, f0, 0), g += __shfl_sync(0xffffffffu, f0, 1), b += __shfl_sync(0xffffffffu, f0, 2);
@@ -415,11 +293,10 @@ render_blend_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ act
     float mean0 = 0.f, mean1 = 0.f, sq0 = 0.f, sq1 = 0.f;
     float* sA4 = sX;            // [<=64][4] activations, view-interleaved
     float* sB4 = sX + 256;      // second buffer
-    for (int g0 = 0; g0 < nvalid; g0 += 4) {
+    for (int g0 = 0; g0 < s.nvalid; g0 += 4) {
       int vid[4];
       float wq[4], a0[4], a1[4];
-      view_group_features(views, valid, g0, nvalid, wv, gx, gy, rd0, rd1, rd2, rd3, sP, sA4, sB4, lane, vid, wq, a0, a1,
-                          sRGB);
+      view_group_features(views, s, g0, sP, sA4, sB4, lane, vid, wq, a0, a1, sRGB);
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
         mean0 = fmaf(wq[q], a0[q], mean0), mean1 = fmaf(wq[q], a1[q], mean1);
@@ -428,12 +305,12 @@ render_blend_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ act
     }
     // sum_v w (f - mean)^2 = sum_v w f^2 - mean^2 (2 - sum_v w): one pass instead of a second fetch of every view
     // (|error| ~ 1e-6 * f^2, two orders below the colour tolerance)
-    const float wsum1 = wtot / (wtot + 1e-8f);
+    const float wsum1 = s.wtot / (s.wtot + 1e-8f);
     float var0 = fmaxf(sq0 - mean0 * mean0 * (2.f - wsum1), 0.f);
     float var1 = fmaxf(sq1 - mean1 * mean1 * (2.f - wsum1), 0.f);
     // ---- per-sample part of base_fc[0]: [geo(16), mean(59), var(59)] -> 64
     __syncwarp();
-    if (lane < 16) sX[lane] = geo;
+    if (lane < 16) sX[lane] = s.geo;
     sX[16 + lane] = mean0;
     if (lane + 32 < NF) sX[16 + 32 + lane] = mean1;
     sX[75 + lane] = var0;
@@ -445,11 +322,10 @@ render_blend_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ act
 
     // ---- groups of four valid views share every weight load (4 independent FMA chains per output)
     float logit = -3.4e38f;  // lane v keeps the logit of view v
-    for (int g0 = 0; g0 < nvalid; g0 += 4) {
+    for (int g0 = 0; g0 < s.nvalid; g0 += 4) {
       int vid[4];
       float wq[4], a0[4], a1[4];
-      view_group_features(views, valid, g0, nvalid, wv, gx, gy, rd0, rd1, rd2, rd3, sP, sA4, sB4, lane, vid, wq, a0, a1,
-                          nullptr);
+      view_group_features(views, s, g0, sP, sA4, sB4, lane, vid, wq, a0, a1, nullptr);
       // base_fc[0], per-view part: x1 = elu(hs + Wf . f_v)
 #pragma unroll
       for (int q = 0; q < 4; ++q) sA4[lane * 4 + q] = a0[q], sA4[(lane + 32) * 4 + q] = a1[q];
@@ -490,8 +366,8 @@ render_blend_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ act
         // rgb_fc input [x(32), vis(1), ray_diff(4)]
         sB4[lane * 4 + q] = x3[q];
         int vq = vid[q] >= 0 ? vid[q] : 0;
-        float r0 = __shfl_sync(0xffffffffu, rd0, vq), r1 = __shfl_sync(0xffffffffu, rd1, vq);
-        float r2 = __shfl_sync(0xffffffffu, rd2, vq), r3 = __shfl_sync(0xffffffffu, rd3, vq);
+        float r0 = __shfl_sync(0xffffffffu, s.rd0, vq), r1 = __shfl_sync(0xffffffffu, s.rd1, vq);
+        float r2 = __shfl_sync(0xffffffffu, s.rd2, vq), r3 = __shfl_sync(0xffffffffu, s.rd3, vq);
         if (lane == 0) {
           sB4[32 * 4 + q] = vis2;
           sB4[33 * 4 + q] = r0, sB4[34 * 4 + q] = r1, sB4[35 * 4 + q] = r2, sB4[36 * 4 + q] = r3;
@@ -518,11 +394,11 @@ render_blend_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ act
     float lmax = logit;
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) lmax = fmaxf(lmax, __shfl_xor_sync(0xffffffffu, lmax, o));
-    float ex = vmask ? expf(logit - lmax) : 0.f;
+    float ex = s.vmask ? expf(logit - lmax) : 0.f;
     float den = warp_sum(ex);
     float r = 0.f, g = 0.f, b = 0.f;
     int slot = 0;
-    for (unsigned m = valid; m; m &= m - 1, ++slot) {
+    for (unsigned m = s.valid; m; m &= m - 1, ++slot) {
       int v = __ffs(m) - 1;
       float bw = __shfl_sync(0xffffffffu, ex, v) / den;
       r = fmaf(bw, sRGB[slot * 4], r), g = fmaf(bw, sRGB[slot * 4 + 1], g), b = fmaf(bw, sRGB[slot * 4 + 2], b);
@@ -619,9 +495,6 @@ namespace o2345 {
 int launch_render_blend_tc(const o2345_points* src, int64_t n, const uint8_t* active, const float* vol_cl, const float* occ, int D,
                            const o2345_views* views, int dir_mode, const float* query_center, const float* dirs,
                            const float* rnet_pack, float* rgb, int32_t* nvalid, cudaStream_t st);   // render_tc.cu
-int launch_render_blend_t5(const o2345_points* src, int64_t n, const uint8_t* active, const float* vol_cl, const float* occ, int D,
-                           const o2345_views* views, int dir_mode, const float* query_center, const float* dirs,
-                           const float* rnet_pack, float* rgb, int32_t* nvalid, cudaStream_t st);   // render_t5.cu
 }
 
 extern "C" int o2345_render_blend(const o2345_points* src, int64_t n, const uint8_t* active, const float* vol_cl,
@@ -632,11 +505,8 @@ extern "C" int o2345_render_blend(const o2345_points* src, int64_t n, const uint
   O2345_CHECK_ARG(src->mode == O2345_PTS_EXPLICIT || src->mode == O2345_PTS_RAYS, "explicit or ray points only");
   O2345_CHECK_ARG(views->V >= 1 && views->V <= 32 && views->maps && views->proj && views->centers, "1..32 views");
   O2345_CHECK_ARG((dir_mode == 0 && query_center) || (dir_mode == 1 && dirs), "direction source missing");
-  O2345_CHECK_ARG(precision == O2345_BLEND_FP32 || precision == O2345_BLEND_TC_FP16 || precision == O2345_BLEND_TC5, "unknown precision");
+  O2345_CHECK_ARG(precision == O2345_BLEND_FP32 || precision == O2345_BLEND_TC_FP16, "unknown precision");
   if (n == 0) return O2345_OK;
-  if (precision == O2345_BLEND_TC5)
-    return launch_render_blend_t5(src, n, active, vol_cl, occ, D, views, dir_mode, query_center, dirs, rnet_pack, rgb, nvalid,
-                                  (cudaStream_t)stream);
   if (precision == O2345_BLEND_TC_FP16)
     return launch_render_blend_tc(src, n, active, vol_cl, occ, D, views, dir_mode, query_center, dirs, rnet_pack, rgb, nvalid,
                                   (cudaStream_t)stream);

@@ -20,18 +20,19 @@
 // Numerics: features, statistics, softmax and the colour blend are fp32; only MMA operands are rounded to fp16
 // (|rel| 5e-4), which moves the blended colours by ~1e-3.  The fp32 kernel stays available (precision = 0) and is the
 // one the tight oracle parity tests use.
-#include <stdlib.h>
 #include <cuda_fp16.h>
 
+#include "blend_common.cuh"
 #include "common.cuh"
-#include "render_pack.cuh"
+#include "mma_sync.cuh"
 
 namespace o2345 {
 namespace {
 using namespace rpack;
 
-// warps per CTA = template parameter TW of the kernel: 10 (two CTAs per SM) or 20 (ONE CTA per SM: all 20 warps of the SM start
-// every sample together, see `lockstep`, and the 48 KB of fp16 weights are staged once per SM)
+// warps per CTA: ONE CTA of 20 warps per SM, so that all the warps of the SM start every sample together (see the sample loop)
+// and the 48 KB of fp16 weights are staged once per SM
+constexpr int TW = 20;
 
 // fp16 weights in shared memory: matrix [n][LD], LD = K + 8 halves (conflict-free 32-bit loads by (g, t))
 constexpr int LD16 = 24, LD32 = 40, LD48 = 56, LD64 = 72, LD144 = 152;
@@ -52,7 +53,7 @@ constexpr int F_D0B = 0, F_D1B = 16, F_B0B = 80, F_B1B = 144, F_V0B = 176, F_V1B
               F_R1B = 304, F_R2W = 312, F_R2B = 320, F_S = 321, F_TOTAL = 324;
 constexpr int REC = 12;                     // floats per view record
 constexpr int WARP_SMEM = 32 * REC * 4 + 2 * 16 * 32 * 4;
-constexpr int tc_smem(int tw) { return H_TOTAL * 2 + F_TOTAL * 4 + tw * WARP_SMEM; }
+constexpr int TC_SMEM = H_TOTAL * 2 + F_TOTAL * 4 + TW * WARP_SMEM;
 static_assert((H_TOTAL * 2) % 16 == 0, "bias block must stay 16-byte aligned");
 
 // Branch-free ELU: one MUFU.EX2 on min(x, 0) and a select (the ternary around __expf compiled to a divergent branch per
@@ -74,15 +75,6 @@ __device__ __forceinline__ uint32_t elu_h2(uint32_t v) {
   const __half2 e = h2exp2(__hmul2(__hmin2(x, zero), __float2half2_rn(1.4426950408889634f)));
   const __half2 r = __hadd2(__hmax2(x, zero), __hsub2(e, __float2half2_rn(1.f)));
   return *reinterpret_cast<const uint32_t*>(&r);
-}
-__device__ __forceinline__ uint32_t pack2(float x, float y) {
-  __half2 h = __floats2half2_rn(x, y);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 // c[16 x 8 NT] += a[16 x 16 KB] . W^T, W stored [n][LD] halves
 template <int KB, int NT>
@@ -126,11 +118,6 @@ __device__ __forceinline__ void elu_all(float (&c)[NT][4]) {
     for (int i = 0; i < 4; ++i) c[j][i] = elu_(c[j][i]);
 }
 
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
 // sum over the eight row groups (lanes with equal t)
 __device__ __forceinline__ float rows_sum(float v) {
   v += __shfl_xor_sync(0xffffffffu, v, 4);
@@ -143,19 +130,6 @@ __device__ __forceinline__ float rows_max(float v) {
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
   v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
   return v;
-}
-
-__device__ __forceinline__ void sample_point(const o2345_points& src, int64_t gi, float& x, float& y, float& z) {
-  if (src.mode == O2345_PTS_EXPLICIT) {
-    x = __ldg(src.pts + 3 * gi), y = __ldg(src.pts + 3 * gi + 1), z = __ldg(src.pts + 3 * gi + 2);
-  } else {
-    int64_t r = gi / src.S;
-    int s = (int)(gi - r * src.S);
-    float t = __ldg(src.z + r * src.z_stride + s);
-    x = __fadd_rn(__ldg(src.rays_o + 3 * r), __fmul_rn(__ldg(src.rays_d + 3 * r), t));
-    y = __fadd_rn(__ldg(src.rays_o + 3 * r + 1), __fmul_rn(__ldg(src.rays_d + 3 * r + 1), t));
-    z = __fadd_rn(__ldg(src.rays_o + 3 * r + 2), __fmul_rn(__ldg(src.rays_d + 3 * r + 2), t));
-  }
 }
 
 // Feature-channel order inside the MMA fragments.  A thread's four accumulator columns of one 16-column block are
@@ -176,12 +150,11 @@ __device__ void fill_w(__half* dst, int LD, int n_rows, int col0, int k_span, co
   }
 }
 
-template <int TW>
-__global__ void __launch_bounds__(TW * 32, 20 / TW)
+__global__ void __launch_bounds__(TW * 32, 1)
 render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ active, const float* __restrict__ vol,
                        const float* __restrict__ occ, int D, o2345_views views, int dir_mode,
                        const float* __restrict__ query_center, const float* __restrict__ dirs,
-                       const float* __restrict__ pack, float* __restrict__ rgb_out, int32_t* __restrict__ nvalid_out, int lockstep) {
+                       const float* __restrict__ pack, float* __restrict__ rgb_out, int32_t* __restrict__ nvalid_out) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   __half* sW = reinterpret_cast<__half*>(smem_raw);
   float* sB = reinterpret_cast<float*>(sW + H_TOTAL);
@@ -229,94 +202,24 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
   const float abs_s = sB[F_S];
 
   // The per-sample path is ~4 600 straight-line warp instructions (73 KB of SASS): ten warps at ten different places of it
-  // starve on instruction fetch (ncu: no_instruction = 4.5 stall cycles per issue).  lockstep: the warps of a CTA start every
-  // sample together (one barrier per ~4 600 instructions), so that they walk the code within a few cache lines of each other
-  // and share the fetches: 10.47 -> 8.74 ms per 8 192 rays with two CTAs of ten warps, 8.53 ms with ONE CTA of twenty warps per
-  // SM.  (Two more meeting points inside the sample -- before pass A and before pass B, early-leaving warps arriving without
-  // waiting -- gave nothing: 8.71 ms.)
+  // starve on instruction fetch (ncu: no_instruction = 4.5 stall cycles per issue).  So all the warps of the CTA start
+  // every sample together (one barrier per ~4 600 instructions): they walk the code within a few cache lines of each other
+  // and share the fetches.  Per 8 192 rays, two CTAs of ten warps took 10.47 ms without the barrier and 8.74 ms with it; ONE
+  // CTA of twenty warps per SM takes 8.53 ms.  (Two more meeting points inside the sample -- before pass A and before pass B,
+  // early-leaving warps arriving without waiting -- gave nothing: 8.71 ms.)
   for (int64_t g0 = (int64_t)blockIdx.x * TW; g0 < n; g0 += (int64_t)gridDim.x * TW) {
-    if (lockstep) __syncthreads();
+    __syncthreads();
     const int64_t gi = g0 + warp;
     if (gi >= n) continue;
-    if (active && active[gi] == 0) {  // weight of this sample is exactly 0 in the compositing
-      if (lane < 3) rgb_out[3 * gi + lane] = 0.f;
-      if (lane == 0 && nvalid_out) nvalid_out[gi] = 0;
-      continue;
-    }
-    float px, py, pz;
-    sample_point(src, gi, px, py, pz);
-    // ---- geometry feature (ATen trilinear, zeros padding, align_corners=True) + occupancy: as render_blend_kernel
-    float geo = 0.f, occv = 0.f;
-    {
-      float p[3] = {px, py, pz};
-      float f[3], w1[3];
-      bool fin = true;
-#pragma unroll
-      for (int a = 0; a < 3; ++a) {
-        float tt = ((p[a] + 1.f) / 2.f) * (float)(D - 1);
-        f[a] = floorf(tt);
-        w1[a] = tt - f[a];
-        fin = fin && (f[a] >= -1.f) && (f[a] <= (float)(D - 1));
-      }
-      if (fin) {
-#pragma unroll
-        for (int corner = 0; corner < 8; ++corner) {
-          int dx = corner >> 2, dy = (corner >> 1) & 1, dz = corner & 1;
-          int ix = (int)f[0] + dx, iy = (int)f[1] + dy, iz = (int)f[2] + dz;
-          if (ix < 0 || iy < 0 || iz < 0 || ix >= D || iy >= D || iz >= D) continue;
-          float w = (dx ? w1[0] : 1.f - w1[0]) * (dy ? w1[1] : 1.f - w1[1]) * (dz ? w1[2] : 1.f - w1[2]);
-          int64_t cell = ((int64_t)ix * D + iy) * D + iz;
-          if (lane < 16) geo = fmaf(__ldg(vol + cell * 16 + lane), w, geo);
-          occv = fmaf(__ldg(occ + cell), w, occv);
-        }
-      }
-    }
-    const bool gmask = (fabsf(px) < 1.f) && (fabsf(py) < 1.f) && (fabsf(pz) < 1.f) && (occv > 0.f);
-    // ---- lanes as views: projection, mask, ray difference, pooling weight
-    float gx = 2.f, gy = 2.f, rd0 = 0.f, rd1 = 0.f, rd2 = 0.f, rd3 = 0.f, ev = 3.4e38f;
-    bool vmask = false;
-    float tx, ty, tz;
-    if (dir_mode == 0) {
-      tx = query_center[0] - px, ty = query_center[1] - py, tz = query_center[2] - pz;
-      float nn = sqrtf(tx * tx + ty * ty + tz * tz) + 1e-6f;
-      tx /= nn, ty /= nn, tz /= nn;
-    } else {
-      tx = dirs[3 * gi], ty = dirs[3 * gi + 1], tz = dirs[3 * gi + 2];
-    }
-    if (lane < V) {
-      const float* P = views.proj + 12 * lane;
-      float X = P[0] * px + P[1] * py + P[2] * pz + P[3];
-      float Y = P[4] * px + P[5] * py + P[6] * pz + P[7];
-      float Z = fmaxf(P[8] * px + P[9] * py + P[10] * pz + P[11], 1e-3f);
-      gx = 2.f * (X / Z) / (views.sizeW - 1.f) - 1.f;
-      gy = 2.f * (Y / Z) / (views.sizeH - 1.f) - 1.f;
-      if (!(gx <= 1.f && gx >= -1.f)) gx = 2.f;
-      if (!(gy <= 1.f && gy >= -1.f)) gy = 2.f;
-      vmask = gmask && (fabsf(gx) < 1.f) && (fabsf(gy) < 1.f);
-      float cx = views.centers[3 * lane] - px, cy = views.centers[3 * lane + 1] - py, cz = views.centers[3 * lane + 2] - pz;
-      float nn = sqrtf(cx * cx + cy * cy + cz * cz) + 1e-6f;
-      cx /= nn, cy /= nn, cz /= nn;
-      float ddx = tx - cx, ddy = ty - cy, ddz = tz - cz;
-      float dn = fmaxf(sqrtf(ddx * ddx + ddy * ddy + ddz * ddz), 1e-6f);
-      rd0 = ddx / dn, rd1 = ddy / dn, rd2 = ddz / dn;
-      rd3 = tx * cx + ty * cy + tz * cz;
-      ev = expf(abs_s * (rd3 - 1.f));
-    }
-    float emin = ev;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) emin = fminf(emin, __shfl_xor_sync(0xffffffffu, emin, o));
-    float wv = vmask ? (ev - emin) : 0.f;
-    const float wtot = warp_sum(wv);
-    wv = wv / (wtot + 1e-8f);
-    const unsigned valid = __ballot_sync(0xffffffffu, vmask);
-    const int nvalid = __popc(valid);
-    if (lane == 0 && nvalid_out) nvalid_out[gi] = nvalid;
+    if (skip_inactive(active, gi, lane, rgb_out, nvalid_out)) continue;
+    const BlendSample s = blend_front_end(src, gi, vol, occ, D, views, dir_mode, query_center, dirs, abs_s, lane);
+    if (lane == 0 && nvalid_out) nvalid_out[gi] = s.nvalid;
 
-    if (nvalid == 0) {
+    if (s.nvalid == 0) {
       // every logit is -1e9: softmax is uniform over ALL views (reference rendering_network.py:119-121)
       float acc = 0.f;
       for (int v = 0; v < V; ++v) {
-        float vgx = __shfl_sync(0xffffffffu, gx, v), vgy = __shfl_sync(0xffffffffu, gy, v);
+        float vgx = __shfl_sync(0xffffffffu, s.gx, v), vgy = __shfl_sync(0xffffffffu, s.gy, v);
         float fx = ((vgx + 1.f) / 2.f) * (float)(W - 1), fy = ((vgy + 1.f) / 2.f) * (float)(H - 1);
         float x0 = floorf(fx), y0 = floorf(fy);
         if (!(x0 >= -1.f && x0 <= (float)(W - 1) && y0 >= -1.f && y0 <= (float)(H - 1)) || lane >= 3) continue;
@@ -336,9 +239,9 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
 
     // ---- per-view records, compacted by slot (= rank of the view among the valid ones)
     __syncwarp();
-    if (vmask) {
-      const int slot = __popc(valid & ((1u << lane) - 1u));
-      float fx = ((gx + 1.f) / 2.f) * (float)(W - 1), fy = ((gy + 1.f) / 2.f) * (float)(H - 1);
+    if (s.vmask) {
+      const int slot = __popc(s.valid & ((1u << lane) - 1u));
+      float fx = ((s.gx + 1.f) / 2.f) * (float)(W - 1), fy = ((s.gy + 1.f) / 2.f) * (float)(H - 1);
       float x0 = floorf(fx), y0 = floorf(fy);
       int ix = (int)x0, iy = (int)y0;
       float x1 = x0 + 1.f, y1 = y0 + 1.f;
@@ -349,11 +252,11 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
       r[2] = (iny1 && inx0) ? (x1 - fx) * (fy - y0) : 0.f;
       r[3] = (iny1 && inx1) ? (fx - x0) * (fy - y0) : 0.f;
       r[4] = __int_as_float(ix), r[5] = __int_as_float(iy), r[6] = __int_as_float(lane);
-      r[7] = rd0, r[8] = rd1, r[9] = rd2, r[10] = rd3, r[11] = wv;
+      r[7] = s.rd0, r[8] = s.rd1, r[9] = s.rd2, r[10] = s.rd3, r[11] = s.wv;
     }
     __syncwarp();
 
-    const int ntile = (nvalid + 15) >> 4;
+    const int ntile = (s.nvalid + 15) >> 4;
     float S[8][2], Q[8][2];
 #pragma unroll
     for (int j = 0; j < 8; ++j) S[j][0] = S[j][1] = Q[j][0] = Q[j][1] = 0.f;
@@ -366,7 +269,7 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
 #pragma unroll
       for (int rr = 0; rr < 2; ++rr) {
         const int slot = 16 * tile + g + 8 * rr;
-        const bool ok = slot < nvalid;
+        const bool ok = slot < s.nvalid;
         const float* r = sRec + (ok ? slot : 0) * REC;
         const float4 w4 = *reinterpret_cast<const float4*>(r);
         const float wq[4] = {ok ? w4.x : 0.f, ok ? w4.y : 0.f, ok ? w4.z : 0.f, ok ? w4.w : 0.f};
@@ -409,7 +312,7 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
         float c64[8][4];
         init_bias<8>(c64, sB + F_D1B, t);
         mm<1, 8>(c64, a16, sW + H_D1, LD16, g, t);
-        const bool ok0 = 16 * tile + g < nvalid, ok1 = 16 * tile + g + 8 < nvalid;
+        const bool ok0 = 16 * tile + g < s.nvalid, ok1 = 16 * tile + g + 8 < s.nvalid;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           F[j][0] = ok0 ? F[j][0] + elu_(c64[j][0]) : 0.f, F[j][1] = ok0 ? F[j][1] + elu_(c64[j][1]) : 0.f;
@@ -431,11 +334,11 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
     }
     // ---- weighted mean / variance over the views: sum over the eight row groups
     //      sum_v w (f - mean)^2 = sum_v w f^2 - mean^2 (2 - sum_v w)
-    const float wsum1 = wtot / (wtot + 1e-8f);
+    const float wsum1 = s.wtot / (s.wtot + 1e-8f);
     uint32_t aS[9][4];   // per-sample input [geo | mean | var] with all 16 rows equal
     {
-      float g0 = __shfl_sync(0xffffffffu, geo, 2 * t), g1 = __shfl_sync(0xffffffffu, geo, 2 * t + 1);
-      float g8 = __shfl_sync(0xffffffffu, geo, 2 * t + 8), g9 = __shfl_sync(0xffffffffu, geo, 2 * t + 9);
+      float g0 = __shfl_sync(0xffffffffu, s.geo, 2 * t), g1 = __shfl_sync(0xffffffffu, s.geo, 2 * t + 1);
+      float g8 = __shfl_sync(0xffffffffu, s.geo, 2 * t + 8), g9 = __shfl_sync(0xffffffffu, s.geo, 2 * t + 9);
       aS[0][0] = aS[0][1] = pack2(g0, g1), aS[0][2] = aS[0][3] = pack2(g8, g9);
     }
 #pragma unroll
@@ -454,7 +357,7 @@ render_blend_tc_kernel(o2345_points src, int64_t n, const uint8_t* __restrict__ 
     // ================= pass B: per-view MLPs, logits
     float lgA0 = -3.4e38f, lgA1 = -3.4e38f, lgB0 = -3.4e38f, lgB1 = -3.4e38f;   // logits of rows g, g + 8 in tile 0 / 1
     for (int tile = 0; tile < ntile; ++tile) {
-      const bool ok0 = 16 * tile + g < nvalid, ok1 = 16 * tile + g + 8 < nvalid;
+      const bool ok0 = 16 * tile + g < s.nvalid, ok1 = 16 * tile + g + 8 < s.nvalid;
       const float w0 = ok0 ? sRec[(16 * tile + g) * REC + 11] : 0.f, w1 = ok1 ? sRec[(16 * tile + g + 8) * REC + 11] : 0.f;
       uint32_t aF[4][4];
 #pragma unroll
@@ -556,27 +459,12 @@ int launch_render_blend_tc(const o2345_points* src, int64_t n, const uint8_t* ac
                            const float* rnet_pack, float* rgb, int32_t* nvalid, cudaStream_t st) {
   static PerDeviceOnce attr_done;
   if (attr_done.need()) {
-    O2345_CUDA(cudaFuncSetAttribute(render_blend_tc_kernel<10>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem(10)));
-    O2345_CUDA(cudaFuncSetAttribute(render_blend_tc_kernel<20>, cudaFuncAttributeMaxDynamicSharedMemorySize, tc_smem(20)));
+    O2345_CUDA(cudaFuncSetAttribute(render_blend_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, TC_SMEM));
   }
-  // tuning knobs (tools/time_render.py): O2345_BLEND_LOCKSTEP=0 lets the warps of a CTA drift apart, O2345_BLEND_WARPS=10 runs
-  // two CTAs of ten warps per SM (the round-1 configuration)
-  static int lockstep = -1, tw = 20;
-  if (lockstep < 0) {
-    const char* e = getenv("O2345_BLEND_LOCKSTEP");
-    lockstep = e ? atoi(e) : 1;
-    const char* w = getenv("O2345_BLEND_WARPS");
-    if (w && atoi(w) == 10) tw = 10;
-  }
-  const int64_t need = (n + tw - 1) / tw;
-  const int64_t cap = (int64_t)(20 / tw) * sm_count();
-  const int grid = (int)(need < cap ? need : cap);
-  if (tw == 20)
-    render_blend_tc_kernel<20><<<grid, 20 * 32, tc_smem(20), st>>>(*src, n, active, vol_cl, occ, D, *views, dir_mode, query_center, dirs,
-                                                                rnet_pack, rgb, nvalid, lockstep);
-  else
-    render_blend_tc_kernel<10><<<grid, 10 * 32, tc_smem(10), st>>>(*src, n, active, vol_cl, occ, D, *views, dir_mode, query_center, dirs,
-                                                                rnet_pack, rgb, nvalid, lockstep);
+  const int64_t need = (n + TW - 1) / TW;
+  const int grid = (int)(need < (int64_t)sm_count() ? need : (int64_t)sm_count());
+  render_blend_tc_kernel<<<grid, TW * 32, TC_SMEM, st>>>(*src, n, active, vol_cl, occ, D, *views, dir_mode, query_center, dirs,
+                                                         rnet_pack, rgb, nvalid);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

@@ -80,25 +80,6 @@ __device__ __forceinline__ Tri tri_setup(float px, float py, float pz, int D) {
   return t;
 }
 
-__device__ __forceinline__ void load_point(const o2345_points& src, int64_t gi, float& x, float& y, float& z) {
-  if (src.mode == O2345_PTS_EXPLICIT) {
-    x = __ldg(src.pts + 3 * gi), y = __ldg(src.pts + 3 * gi + 1), z = __ldg(src.pts + 3 * gi + 2);
-  } else if (src.mode == O2345_PTS_LATTICE) {
-    int R = src.R;
-    int64_t ix = gi / ((int64_t)R * R);
-    int iy = (int)((gi / R) % R), iz = (int)(gi % R);
-    x = __ldg(src.lin + ix), y = __ldg(src.lin + iy), z = __ldg(src.lin + iz);
-  } else {
-    int64_t r = gi / src.S;
-    int s = (int)(gi - r * src.S);
-    float t = __ldg(src.z + r * src.z_stride + s);
-    // o + d * t with separately rounded multiply and add (torch evaluates it that way)
-    x = __fadd_rn(__ldg(src.rays_o + 3 * r), __fmul_rn(__ldg(src.rays_d + 3 * r), t));
-    y = __fadd_rn(__ldg(src.rays_o + 3 * r + 1), __fmul_rn(__ldg(src.rays_d + 3 * r + 1), t));
-    z = __fadd_rn(__ldg(src.rays_o + 3 * r + 2), __fmul_rn(__ldg(src.rays_d + 3 * r + 2), t));
-  }
-}
-
 // Point and latent source of o2345_sdf_voxels (kernels instantiated with VOX = true): point i is lattice voxel
 // i = (x*D + y)*D + z at coord * vs + origin (one rounded multiply, one rounded add, as `coords * voxel_size + origin`
 // in fp32), its latent is row i of the channel-last volume as it is (no trilinear fetch), and it is evaluated iff

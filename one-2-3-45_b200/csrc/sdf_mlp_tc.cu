@@ -17,6 +17,7 @@
 #include <cuda_fp16.h>
 
 #include "common.cuh"
+#include "mma_sync.cuh"
 #include "sdf_common.cuh"
 
 namespace o2345 {
@@ -34,11 +35,6 @@ constexpr int K0PAD = 48;                      // layer-0 K (39) padded to three
 __device__ __forceinline__ void split(float x, __half& hi, __half& lo) {
   hi = __float2half_rn(x);
   lo = __float2half_rn(x - __half2float(hi));
-}
-__device__ __forceinline__ void mma16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 __device__ __forceinline__ void ldsm4t(uint32_t (&r)[4], const __half* p) {
   const uint32_t a = (uint32_t)__cvta_generic_to_shared(p);

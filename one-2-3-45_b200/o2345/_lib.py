@@ -36,7 +36,7 @@ class Epilogue(C.Structure):
 
 
 PTS_EXPLICIT, PTS_LATTICE, PTS_RAYS = 0, 1, 2
-BLEND_FP32, BLEND_TC_FP16, BLEND_TC5 = 0, 1, 2
+BLEND_FP32, BLEND_TC_FP16 = 0, 1
 SDF_FP32, SDF_TC_SPLIT = 0, 1
 SDF_PACK_FLOATS = 39 * 128 + 128 + 2 * (144 * 128 + 128) + 128 * 144 + 128 * 48
 RNET_PACK_FLOATS = 19664
@@ -129,7 +129,7 @@ _SIGS = {
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 4          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 5          # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 

@@ -378,7 +378,8 @@ class SourceViews:
 
 def render_blend(src: PointSource, active, vol_cl, occ, views: SourceViews, rnet_pack, query_center=None, dirs=None,
                  precision=L.BLEND_TC_FP16):
-    """precision: L.BLEND_TC_FP16 (tensor-core MLPs, fp16 operands / fp32 accumulate) or L.BLEND_FP32 (fp32 FMA)."""
+    """precision: L.BLEND_TC_FP16 (mma.sync MLPs, fp16 operands / fp32 accumulate; the default) or L.BLEND_FP32 (fp32 FMA, the
+    reference the parity tests compare against).  Any other value is refused."""
     n, dev = src.n, vol_cl.device
     rgb = torch.empty(n, 3, dtype=_f32, device=dev)
     nvalid = torch.empty(n, dtype=_i32, device=dev)

@@ -4,8 +4,9 @@ Mirror of reference reconstruction/models/rendering_network.py:26-129 (state-dic
 s, ray_dir_fc.{0,2}, base_fc.{0,2}, vis_fc.{0,2}, vis_fc2.{0,2}, rgb_fc.{0,2,4}) and
 reconstruction/models/fields.py:179-185.  The arithmetic of forward() lives in csrc/render_tc.cu
 (render_blend_tc_kernel: the per-(sample, view) MLPs as mma.sync chains, default) and csrc/render.cu
-(render_blend_kernel: fp32 FMA, O2345_BLEND_FP32), fused with the Projector's per-view feature fetch, so
-the [n_views, n_rays, n_samples, 59] tensors the reference materialises never exist.
+(render_blend_kernel: fp32 FMA, O2345_BLEND_FP32, the reference of the parity tests), fused with the Projector's
+per-view feature fetch, so the [n_views, n_rays, n_samples, 59] tensors the reference materialises never exist.  Both
+kernels share the per-sample front end and the weight-pack layout in csrc/blend_common.cuh.
 """
 from __future__ import annotations
 
@@ -33,7 +34,7 @@ class GeneralRenderingNetwork(nn.Module):
         self._pack, self._pack_key = None, None
 
     def packed(self):
-        """Weights in the [in][out] layout documented in csrc/render.cu (O2345_RNET_PACK_FLOATS floats)."""
+        """Weights in the [in][out] layout documented in csrc/blend_common.cuh (O2345_RNET_PACK_FLOATS floats)."""
         key = tuple((p.data_ptr(), p._version) for p in self.parameters())
         if self._pack is not None and key == self._pack_key:
             return self._pack

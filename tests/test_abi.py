@@ -79,6 +79,10 @@ def test_argument_checks_return_einval_without_touching_the_gpu():
         lambda: lib.o2345_render_blend(C.byref(_lib.Points(mode=0)), 4, None, fake, fake, 8,
                                        C.byref(_lib.Views(V=4, H=8, W=8, maps=0x1000, proj=0x1000, centers=0x1000)), 0, fake, None,
                                        fake, 9, fake, None, None),
+        # precision 2 (the wgmma kernel) was removed in ABI 5; _lib.load() refuses a library of another ABI version
+        lambda: lib.o2345_render_blend(C.byref(_lib.Points(mode=0)), 4, None, fake, fake, 8,
+                                       C.byref(_lib.Views(V=4, H=8, W=8, maps=0x1000, proj=0x1000, centers=0x1000)), 0, fake, None,
+                                       fake, 2, fake, None, None),
     ]
     for i, call in enumerate(cases):
         rc = call()

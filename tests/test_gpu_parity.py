@@ -173,10 +173,10 @@ def _render(tr, om, dev, vol, occ, fm):
 # blend kernels: 0 = fp32 FMA in the reference's operation order, 1 = tensor-core MLPs (fp16 operands, fp32 accumulate).
 # Colour tolerance of the tensor-core kernel: operands carry 2^-11 relative rounding through 11 small layers; the blend
 # weights are a softmax of O(1) logits and the colours are in [0, 1], and the measured drift against the fp32 kernel is 5e-5 max on the 32-view scene; 5e-4 is the stated bound.
-BLEND_TOL = {0: 2e-4, 1: 5e-4, 2: 5e-4}
+BLEND_TOL = {0: 2e-4, 1: 5e-4}
 
 
-@pytest.fixture(params=[0, 1, 2], ids=["blend_fp32", "blend_tc_fp16", "blend_tcgen05"])
+@pytest.fixture(params=[0, 1], ids=["blend_fp32", "blend_tc_fp16"])
 def precision(request, tr):
     old = tr.sdf_renderer_lod0.blend_precision
     tr.sdf_renderer_lod0.blend_precision = request.param
@@ -398,7 +398,7 @@ def test_full_size_render_properties(full, dev):
     assert torch.equal(a["color_fine"], c[:h])
 
 
-def test_full_size_blend_kernels_agree(full, dev):
+def test_full_size_tc_blend_agrees_with_fp32(full, dev):
     """Tensor-core blend kernel against the fp32 one on a 32-view, 256x256 scene (same samples, same maps)."""
     tr, sample, imgs, fmaps, cond = full
     ro = sample["rays"]["rays_o"][0][::29][:2048].contiguous()
@@ -407,7 +407,7 @@ def test_full_size_blend_kernels_agree(full, dev):
     outs = {}
     old = tr.sdf_renderer_lod0.blend_precision
     try:
-        for prec in (0, 1, 2):
+        for prec in (0, 1):
             tr.sdf_renderer_lod0.blend_precision = prec
             outs[prec] = tr.sdf_renderer_lod0.render(
                 ro, rd, near, far, tr.sdf_network_lod0, tr.rendering_network_lod0, perturb_overwrite=0, background_rgb=1.0,
@@ -416,12 +416,8 @@ def test_full_size_blend_kernels_agree(full, dev):
                 w2cs=sample["w2cs"][0], intrinsics=sample["intrinsics"][0], img_wh=[256, 256], query_c2w=sample["query_c2w"])
     finally:
         tr.sdf_renderer_lod0.blend_precision = old
-    for prec, name in ((1, "mma.sync"), (2, "wgmma")):
-        a, b = outs[0]["color_fine"], outs[prec]["color_fine"]
-        assert torch.equal(outs[0]["z_vals"], outs[prec]["z_vals"])                 # the sampler does not depend on the colours
-        assert torch.equal(outs[0]["color_fine_mask"], outs[prec]["color_fine_mask"])
-        d = (a - b).abs()
-        print("blend fp32 vs tensor-core (%s): max" % name, float(d.max()), "mean", float(d.mean()))
-        assert float(d.max()) < 5e-4 and float(d.mean()) < 5e-5
-    d = (outs[0]["color_fine"] - outs[2]["color_fine"]).abs()
+    assert torch.equal(outs[0]["z_vals"], outs[1]["z_vals"])                 # the sampler does not depend on the colours
+    assert torch.equal(outs[0]["color_fine_mask"], outs[1]["color_fine_mask"])
+    d = (outs[0]["color_fine"] - outs[1]["color_fine"]).abs()
+    print("blend fp32 vs tensor-core (mma.sync): max", float(d.max()), "mean", float(d.mean()))
     assert float(d.max()) < 5e-4 and float(d.mean()) < 5e-5

@@ -22,7 +22,7 @@ def spy(*a, **k):
         hist["h"] = torch.bincount(nv, minlength=33).tolist()
     return r
 ops.render_blend = spy
-for prec in [int(a) for a in os.environ.get("BLEND_PRECISIONS", "1,2").split(",")]:   # 1: mma.sync kernel (default), 2: wgmma kernel
+for prec in [int(a) for a in os.environ.get("BLEND_PRECISIONS", "1").split(",")]:   # 1: mma.sync kernel (default), 0: fp32 kernel
     tr.sdf_renderer_lod0.blend_precision = prec
     r = bench.render_throughput(tr, sample, imgs, fmaps, cond, sizeW, sizeH, dev, pk)
     print("precision", prec, json.dumps(r))
