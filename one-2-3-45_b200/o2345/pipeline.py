@@ -181,3 +181,49 @@ def image_to_mesh(zero123, trainer, input_u8, polar_angle=60, resolution=256, dd
     sample = sample_from_views(stage1, stage2, pose, dev)
     trainer.base_exp_dir = exp_dir
     return trainer(sample, mode="export_mesh", resolution=resolution)
+
+
+# --------------------------------------------------------------------------------------
+# many images -> many meshes: Zero123 calls of several images packed into one sampler batch
+# --------------------------------------------------------------------------------------
+# Images per pack: the sampler runs stage 1 at batch 16 K and stage 2 at batch 64 K.  Chosen from tools/throughput.py
+# (DESIGN.md section 5): the largest K measured (1, 2, 4, 8) whose UNet time per image still falls by more than the
+# run-to-run spread; K = 8 peaks at 14.7 GB allocated.
+MAX_PACK = 8
+
+
+def pack_slices(n, max_pack):
+    """Consecutive packs of at most max_pack of n images, in input order: [(start, stop), ...]."""
+    if max_pack < 1:
+        raise ValueError(f"max_pack must be >= 1, got {max_pack}")
+    return [(s, min(s + max_pack, n)) for s in range(0, n, max_pack)]
+
+
+@torch.no_grad()
+def images_to_meshes(zero123, trainer, inputs_u8, polar_angles, seed=0, resolution=256, exp_dirs=None, *, max_pack=None,
+                     indices=None, ddim_steps=75, stage2_steps=50, scale=3.0):
+    """image_to_mesh for a list of images: a generator of (index, mesh) in input order.  The images go through Zero123 in
+    packs of at most MAX_PACK (zero123.generate_views_multi: two sampler calls per pack), then each is reconstructed on its
+    own (sample_from_views + trainer(..., mode="export_mesh")).
+
+    polar_angles: one per image or one for all.  Image i's noise comes from seed + indices[i] (indices: the images'
+    positions in the caller's full list, default 0..n-1; a process that renders a share of a list passes the share's
+    positions), so a mesh does not depend on the pack size, the number of processes or which one renders it; `index` is
+    indices[i].  exp_dirs (one per image): stage1_8/, stage2_8/, pose.json and mesh.ply are written there.  max_pack
+    overrides MAX_PACK."""
+    from .zero123 import generate_views_multi
+    n = len(inputs_u8)
+    polars = list(polar_angles) if np.ndim(polar_angles) else [polar_angles] * n
+    indices = list(range(n)) if indices is None else list(indices)
+    if len(polars) != n or len(indices) != n or (exp_dirs is not None and len(exp_dirs) != n):
+        raise ValueError(f"{n} images need as many polar angles ({len(polars)}), indices ({len(indices)}) and exp_dirs")
+    dev = next(trainer.parameters()).device
+    for a, b in pack_slices(n, MAX_PACK if max_pack is None else max_pack):
+        dirs = None if exp_dirs is None else exp_dirs[a:b]
+        views = generate_views_multi(zero123, inputs_u8[a:b], polars[a:b], ddim_steps, stage2_steps, scale, seed=seed,
+                                     indices=indices[a:b], exp_dirs=dirs, device=dev, keep_on_device=dirs is None)
+        for i, (stage1, stage2, pose) in enumerate(views):
+            sample = sample_from_views(stage1, stage2, pose, dev)
+            trainer.base_exp_dir = None if dirs is None else dirs[i]
+            yield indices[a + i], trainer(sample, mode="export_mesh", resolution=resolution)
+        del views

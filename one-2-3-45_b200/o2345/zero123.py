@@ -225,19 +225,52 @@ def generate_views(model, input_u8, polar_angle=60, ddim_steps=75, stage2_steps=
         for i in ([1, 2, 3] + second):
             stage2_call([i])
     else:
-        n1 = ddim_iterations(ddim_steps, model.num_timesteps)
-        n2 = ddim_iterations(stage2_steps, model.num_timesteps)
-        draws = {}
-        for kind, key in [("s1", 0), ("s2", 0), ("s1", 1)] + [("s2", i) for i in [1, 2, 3] + second]:
-            # the reference's order of calls; inside a call: x_T, then one draw per iteration (ddim.py:137,223)
-            x_T = torch.randn(4, 4, 32, 32, device=dev)
-            draws[(kind, key)] = (x_T, [torch.randn(4, 4, 32, 32, device=dev) for _ in range(n1 if kind == "s1" else n2)])
-
-        def gather(keys, n):
-            return (torch.cat([draws[k][0] for k in keys]), [torch.cat([draws[k][1][i] for k in keys]) for i in range(n)])
-        stage1_call(first + second, *gather([("s1", 0), ("s1", 1)], n1))
+        draws = _draw_view_noise(second, ddim_iterations(ddim_steps, model.num_timesteps),
+                                 ddim_iterations(stage2_steps, model.num_timesteps), dev)
+        stage1_call(first + second, *_gather_noise([draws], [[("s1", 0), ("s1", 1)]]))
         anchors = first + second
-        stage2_call(anchors, *gather([("s2", i) for i in anchors], n2))
+        stage2_call(anchors, *_gather_noise([draws], [[("s2", i) for i in anchors]]))
+    return _finish_views(stage1, stage2, pose, exp_dir, keep_on_device)
+
+
+def _stage1_ids(polar_angle):
+    """The 8 stage-1 view ids of run.py's stage1_run: 0-3, then 4-7 (polar <= 75) or 8-11 (reference run.py:18-35)."""
+    return list(range(4)) + (list(range(4, 8)) if polar_angle <= 75 else list(range(8, 12)))
+
+
+def _draw_view_noise(second, n1, n2, dev):
+    """The noise of one image's ten reference sampler calls, drawn from the default generator of `dev` in the reference's order of
+    calls (stage 1 views 0-3, stage 2 of view 0, stage 1 of `second`, stage 2 of views 1-3 and `second`); inside a call x_T
+    first, then one draw per iteration (ddim.py:137,223).  -> {(kind, key): (x_T, [noise per iteration])}."""
+    draws = {}
+    for kind, key in [("s1", 0), ("s2", 0), ("s1", 1)] + [("s2", i) for i in [1, 2, 3] + second]:
+        x_T = torch.randn(4, 4, 32, 32, device=dev)
+        draws[(kind, key)] = (x_T, [torch.randn(4, 4, 32, 32, device=dev) for _ in range(n1 if kind == "s1" else n2)])
+    return draws
+
+
+def image_noise(seed, index, polar_angle, n1, n2, device):
+    """The noise contract of generate_views_multi for the image at position `index` of the caller's list: the generator of
+    `device` (the CUDA generator of that device; the CPU generator for a CPU device) seeded with seed + index, then the
+    draws of generate_views(batched=True) for n1 stage-1 and n2 stage-2 iterations."""
+    dev = torch.device(device)
+    if dev.type == "cuda":
+        with torch.cuda.device(dev):
+            torch.cuda.manual_seed(seed + index)
+    else:
+        torch.manual_seed(seed + index)
+    return _draw_view_noise(_stage1_ids(polar_angle)[4:], n1, n2, dev)
+
+
+def _gather_noise(draws, keys):
+    """x_T and the per-iteration noise of one batched sampler call: draws[i][k] for k in keys[i], image-major."""
+    parts = [d[k] for d, ks in zip(draws, keys) for k in ks]
+    return torch.cat([p[0] for p in parts]), [torch.cat([p[1][i] for p in parts]) for i in range(len(parts[0][1]))]
+
+
+def _finish_views(stage1, stage2, pose, exp_dir, keep_on_device):
+    """Host copies of the device-resident uint8 views (unless keep_on_device) and, with exp_dir, stage1_8/*.png,
+    stage2_8/*.png and pose.json as run.py writes them."""
     if not keep_on_device or exp_dir is not None:
         host1, host2 = torch.stack([stage1[i] for i in stage1]).cpu().numpy(), torch.stack([stage2[k] for k in stage2]).cpu().numpy()
         if not keep_on_device:
@@ -254,6 +287,53 @@ def generate_views(model, input_u8, polar_angle=60, ddim_steps=75, stage2_steps=
             Image.fromarray(im).save(os.path.join(exp_dir, "stage2_8", f"{k}.png"))
         json.dump(pose, open(os.path.join(exp_dir, "pose.json"), "w"), indent=4)
     return stage1, stage2, pose
+
+
+@torch.no_grad()
+def generate_views_multi(model, inputs_u8, polar_angles, ddim_steps=75, stage2_steps=50, scale=3.0, seed=0, indices=None,
+                         exp_dirs=None, device="cuda", keep_on_device=False):
+    """generate_views for K images in two sampler calls: stage 1 at batch 16 K (8 views x CFG per image) for the stage-1
+    iterations, then stage 2 at batch 64 K (32 views x CFG per image).  Every image gets the view ids, pose.json and
+    uint8 quantisation generate_views gives it; polar_angles (one per image, or one for all) may differ, so one call can
+    mix the two stage-1 id sets.
+
+    Noise: before image i's draws the CUDA generator of `device` is seeded with seed + indices[i] (indices: each image's
+    position in the caller's full list, default 0..K-1), then the image's noise is drawn exactly as
+    generate_views(batched=True) draws it.  An image's noise, and so its views up to the rounding of the GEMM shapes, does
+    not depend on K, on the other images or on which process renders it; with K = 1 the result is bit-identical to
+    `torch.cuda.manual_seed(seed + indices[0]); generate_views(...)`.
+
+    Returns a list of K (stage1, stage2, pose) triples as generate_views returns them; exp_dirs (one per image, or None)
+    receive the same files."""
+    dev = torch.device(device)
+    K = len(inputs_u8)
+    polars = [float(p) for p in polar_angles] if np.ndim(polar_angles) else [float(polar_angles)] * K
+    indices = list(range(K)) if indices is None else [int(i) for i in indices]
+    if K == 0 or len(polars) != K or len(indices) != K or (exp_dirs is not None and len(exp_dirs) != K):
+        raise ValueError(f"{K} images need as many polar angles ({len(polars)}), indices ({len(indices)}) and exp_dirs")
+    ids = [_stage1_ids(p) for p in polars]
+    n1, n2 = ddim_iterations(ddim_steps, model.num_timesteps), ddim_iterations(stage2_steps, model.num_timesteps)
+    draws = [image_noise(seed, indices[i], polars[i], n1, n2, dev) for i in range(K)]
+    inp = torch.cat([_as_input(u8, False) for u8 in inputs_u8]).to(dev)
+
+    x_T, noise = _gather_noise(draws, [[("s1", 0), ("s1", 1)]] * K)
+    sampler = DDIMSampler(model)
+    imgs = sample_model_batch(model, sampler, inp, [DELTA_X_1_8[j] for v in ids for j in v], [DELTA_Y_1_8[j] for v in ids for j in v],
+                              n_samples=8, ddim_steps=ddim_steps, scale=scale, x_T=x_T, step_noise=noise, to_host=False)
+    u8 = _to_uint8_device(imgs)
+    stage1 = [{j: u8[8 * i + k] for k, j in enumerate(v)} for i, v in enumerate(ids)]
+
+    x_T, noise = _gather_noise(draws, [[("s2", j) for j in v] for v in ids])
+    sampler = DDIMSampler(model)
+    ims = _as_input_device(torch.stack([stage1[i][j] for i, v in enumerate(ids) for j in v]), True)
+    imgs = sample_model_batch(model, sampler, ims, DELTA_X_2 * (8 * K), DELTA_Y_2 * (8 * K), n_samples=4, ddim_steps=stage2_steps,
+                              scale=scale, x_T=x_T, step_noise=noise, to_host=False)
+    u8 = _to_uint8_device(imgs)
+    out = []
+    for i, v in enumerate(ids):
+        stage2 = {f"{j}_{q}": u8[32 * i + 4 * a + q] for a, j in enumerate(v) for q in range(4)}
+        out.append(_finish_views(stage1[i], stage2, S.pose_json(polars[i]), None if exp_dirs is None else exp_dirs[i], keep_on_device))
+    return out
 
 
 def load_zero123_checkpoint(ckpt, device="cpu", use_ema=True, unet_config=None, first_stage_config=None, clip=True,

@@ -1,4 +1,5 @@
-"""`python run.py --img_path P [--gpu_idx N] [--half_precision] [--mesh_resolution R] [--output_format .ply]`
+"""`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
+[--mesh_resolution R] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -11,6 +12,12 @@ fetch the released ones).  With `--zero123_ckpt` the file is loaded the way the 
 the EMA shadow (`model_ema.*`, reference ldm/modules/ema.py:14-21 + ddpm.py:180-193), the CLIP ViT-L/14 image tower is
 attached and takes `cond_stage_model.*`; a file that lacks what the sampler needs is refused.  `--output_format .obj/.glb`
 follow reference utils/utils.py:31-45 (o2345/mesh_io.py).
+
+Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
+calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
+`--seed` (default 0) + i.  `--polar_angle` takes one value or one per image.  With one image and no `--seed` nothing is
+seeded, as in the reference.  Under torchrun (WORLD_SIZE > 1) each rank runs on cuda:LOCAL_RANK, renders the images
+o2345.sharding.assign_scenes gives it, and takes its weights from rank 0 (the only collective).
 """
 import argparse
 import os
@@ -33,58 +40,108 @@ def load_input(path):
     return np.asarray(im.convert("RGB").resize((256, 256), Image.LANCZOS), np.uint8)
 
 
-def main(argv=None):
-    ap = argparse.ArgumentParser(description="single image -> textured mesh on the o2345 (sm_90a) kernels")
-    ap.add_argument('--img_path', type=str, default="./demo/demo_examples/01_wild_hydrant.png", help='Path to the input image')
-    ap.add_argument('--gpu_idx', type=int, default=0, help='GPU index')
+def parse_args(argv=None):
+    ap = argparse.ArgumentParser(description="segmented image(s) -> textured mesh(es) on the o2345 (sm_90a) kernels")
+    ap.add_argument('--img_path', type=str, nargs='+', default=["./demo/demo_examples/01_wild_hydrant.png"],
+                    help='Path(s) to the input image(s)')
+    ap.add_argument('--gpu_idx', type=int, default=0, help='GPU index (under torchrun: LOCAL_RANK)')
     ap.add_argument('--half_precision', action='store_true', help='accepted for compatibility: the UNet / VAE kernels are fp16')
     ap.add_argument('--mesh_resolution', type=int, default=256, help='Mesh resolution')
     ap.add_argument('--output_format', type=str, default=".ply", help='Output format: .ply, .obj, .glb')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
-    ap.add_argument('--polar_angle', type=float, default=60.0, help='elevation of the input view in degrees (not estimated)')
+    ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
+                    help='elevation of the input view in degrees (not estimated): one value, or one per image')
+    ap.add_argument('--seed', type=int, default=None,
+                    help='base seed of the sampler noise: image i uses seed + i (default: unseeded for one image, 0 for several)')
     ap.add_argument('--zero123_ckpt', type=str, default=None, help='zero123-xl.ckpt (state_dict); default: seeded synthetic weights')
     ap.add_argument('--recon_ckpt', type=str, default=None, help='reconstruction checkpoint (ckpt_*.pth); default: seeded synthetic weights')
-    args = ap.parse_args(argv)
+    return ap.parse_args(argv)
+
+
+def plan_inputs(paths, polar_angles):
+    """-> (shape directories exp/<basename>, one polar angle per image).  Refuses, before any GPU work, two images whose
+    outputs would share a directory and a number of polar angles that is neither one nor one per image."""
+    ids = [os.path.basename(p).split('.')[0] for p in paths]
+    dup = sorted({i for i in ids if ids.count(i) > 1})
+    if dup:
+        raise SystemExit(f"several input images share the basename {dup[0]!r}: their outputs would both go to exp/{dup[0]}/")
+    if len(polar_angles) not in (1, len(paths)):
+        raise SystemExit(f"--polar_angle takes one value or one per image: {len(polar_angles)} values for {len(paths)} images")
+    polars = list(polar_angles) * len(paths) if len(polar_angles) == 1 else list(polar_angles)
+    return [os.path.join("exp", i) for i in ids], polars
+
+
+def _write_format(shape_dir, output_format):
+    mesh_path = os.path.join(shape_dir, "mesh.ply")
+    if output_format == ".ply":          # reference run.py:113-118
+        pass
+    elif output_format not in (".obj", ".glb"):
+        print("Invalid output format, must be one of .ply, .obj, .glb")
+    else:
+        from o2345.mesh_io import convert_mesh_format
+        mesh_path = convert_mesh_format(shape_dir, output_format)
+    return mesh_path
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    shape_dirs, polars = plan_inputs(args.img_path, args.polar_angle)
     if not torch.cuda.is_available():
         raise SystemExit("run.py needs a CUDA device: the o2345 path has no CPU fallback")
-    from o2345 import synthetic as S
-    from o2345.pipeline import build_networks, image_to_mesh
-    from o2345.zero123 import LatentDiffusion, build_zero123
-    dev = torch.device("cuda", args.gpu_idx)
+    from o2345 import sharding, synthetic as S
+    from o2345.pipeline import build_networks, image_to_mesh, images_to_meshes
+    from o2345.zero123 import build_zero123
+    rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
+    dev = torch.device("cuda", int(os.environ.get("LOCAL_RANK", 0)) if world > 1 else args.gpu_idx)
     torch.cuda.set_device(dev)
+    if world > 1:
+        import torch.distributed as dist
+        dist.init_process_group("nccl", device_id=dev)
 
-    if args.zero123_ckpt:
+    if args.zero123_ckpt and rank == 0:
         from o2345.zero123 import load_zero123_checkpoint
         model = load_zero123_checkpoint(args.zero123_ckpt, dev, use_ema=not args.no_ema,
                                         report=lambda m: print(m, file=sys.stderr))
     else:
-        print("no --zero123_ckpt: seeded synthetic Zero123 weights (the generated views are noise-like)", file=sys.stderr)
+        if rank == 0:
+            print("no --zero123_ckpt: seeded synthetic Zero123 weights (the generated views are noise-like)", file=sys.stderr)
         model = build_zero123(dev, seed=0, clip=True)
     model = model.half()
 
     states = S.all_states(0)
-    if args.recon_ckpt:
+    if args.recon_ckpt and rank == 0:
         from o2345.checkpoints import recon_states
         ck = torch.load(args.recon_ckpt, map_location="cpu")
         states.update(recon_states(ck, report=lambda m: print(m, file=sys.stderr)))
-    shape_id = os.path.basename(args.img_path).split('.')[0]
-    shape_dir = os.path.join("exp", shape_id)
-    os.makedirs(shape_dir, exist_ok=True)
-    trainer = build_networks(dev, vol_dim=96, states=states, perturb=0.0, base_exp_dir=shape_dir)
+    single = len(args.img_path) == 1 and world == 1
+    trainer = build_networks(dev, vol_dim=96, states=states, perturb=0.0, base_exp_dir=shape_dirs[0] if single else None)
+    sharding.broadcast_module_weights([model, trainer], src=0)       # rank 0's weights everywhere (no-op for one process)
 
-    mesh = image_to_mesh(model, trainer, load_input(args.img_path), polar_angle=args.polar_angle,
-                         resolution=args.mesh_resolution, exp_dir=shape_dir)
-    mesh_path = os.path.join(shape_dir, "mesh.ply")
-    if args.output_format == ".ply":          # reference run.py:113-118
-        pass
-    elif args.output_format not in (".obj", ".glb"):
-        print("Invalid output format, must be one of .ply, .obj, .glb")
-    else:
-        from o2345.mesh_io import convert_mesh_format
-        mesh_path = convert_mesh_format(shape_dir, args.output_format)
-    print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
-    print("Mesh saved to:", mesh_path)
-    return mesh_path
+    if single:                           # one image: exactly the single-image run
+        shape_dir = shape_dirs[0]
+        os.makedirs(shape_dir, exist_ok=True)
+        if args.seed is not None:
+            torch.cuda.manual_seed(args.seed)
+        mesh = image_to_mesh(model, trainer, load_input(args.img_path[0]), polar_angle=polars[0],
+                             resolution=args.mesh_resolution, exp_dir=shape_dir)
+        mesh_path = _write_format(shape_dir, args.output_format)
+        print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
+        print("Mesh saved to:", mesh_path)
+        return mesh_path
+
+    mine = sharding.assign_scenes(len(args.img_path), world, rank)
+    for i in mine:
+        os.makedirs(shape_dirs[i], exist_ok=True)
+    paths = []
+    for i, mesh in images_to_meshes(model, trainer, [load_input(args.img_path[i]) for i in mine], [polars[i] for i in mine],
+                                    seed=0 if args.seed is None else args.seed, resolution=args.mesh_resolution,
+                                    exp_dirs=[shape_dirs[i] for i in mine], indices=mine):
+        paths.append(_write_format(shape_dirs[i], args.output_format))
+        print(f"{args.img_path[i]}: {len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
+        print("Mesh saved to:", paths[-1])
+    if world > 1:
+        dist.destroy_process_group()
+    return paths
 
 
 if __name__ == "__main__":
