@@ -32,10 +32,11 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 5   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 6   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
-                                 5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone */
+                                 5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
+                                 6: rays of many cameras in one launch: render_blend dir_mode 2, o2345_ray_midpoints_per_ray */
 
 typedef void* o2345_stream_t;
 
@@ -269,6 +270,11 @@ int o2345_ray_merge(const float* z, const float* sdf, int S, const float* new_z,
 int o2345_ray_midpoints(const float* rays_o, const float* rays_d, int64_t R, const float* z, int S,
                         float sample_dist, const float* occ, int D, float* mid_z, float* dists, uint8_t* active,
                         o2345_stream_t stream);
+/* o2345_ray_midpoints with a last section of its own per ray: sample_dist [R] (device), so that one launch can hold
+ * rays of cameras with different near / far.  Same result per ray as o2345_ray_midpoints with that ray's value. */
+int o2345_ray_midpoints_per_ray(const float* rays_o, const float* rays_d, int64_t R, const float* z, int S,
+                                const float* sample_dist, const float* occ, int D, float* mid_z, float* dists,
+                                uint8_t* active, o2345_stream_t stream);
 
 #define O2345_MAP_CH 60 /* channel-last source maps: rgb(3) + pyramid features(56) + 1 pad */
 #define O2345_RNET_PACK_FLOATS 19664
@@ -284,7 +290,9 @@ typedef struct o2345_views {
 /* Per sample point: geometry feature, per-view colour+feature fetch, ray-difference, view-blending
  * MLP -> rgb [n,3]; nvalid [n] = number of views whose mask is set (may be NULL).  dir_mode 0: target
  * direction = normalised (query_center - p) (Projector.compute); 1: dirs [n,3] given
- * (compute_view_independent, surface normals).  rnet_pack: O2345_RNET_PACK_FLOATS floats, every
+ * (compute_view_independent, surface normals); 2: normalised (rays_o[ray] - p), the origin of the sample's own ray
+ * (O2345_PTS_RAYS only; the same bits as mode 0 with query_center = that origin: rays of many cameras in one
+ * launch; query_center and dirs are ignored).  rnet_pack: O2345_RNET_PACK_FLOATS floats, every
  * matrix stored [in][out] in the order documented in csrc/blend_common.cuh. */
 #define O2345_BLEND_FP32 0     /* fp32 FMA mat-vecs in the reference's operation order (tight oracle parity)            */
 #define O2345_BLEND_TC_FP16 1  /* per-(sample, view) MLPs as mma.sync products: fp16 operands, fp32 accumulate / statistics */

@@ -73,7 +73,8 @@ struct BlendSample {
 
 // Sample point gi, its geometry feature and occupancy (ATen trilinear, zeros padding, align_corners=True; reference
 // render_utils.py:54-85, projector.py:168-183), then the lanes as views: projection, view mask, ray difference and pooling
-// weight.  dir_mode 0: the target direction is camera-to-point (rendering); 1: dirs[gi] (the normals of vertex colours).
+// weight.  dir_mode 0: the target direction is camera-to-point (rendering); 1: dirs[gi] (the normals of vertex colours);
+// 2: ray-origin-to-point, the origin of sample gi's own ray (ray points only: cameras that differ from ray to ray).
 __device__ __forceinline__ BlendSample blend_front_end(const o2345_points& src, int64_t gi, const float* __restrict__ vol,
                                                        const float* __restrict__ occ, int D, const o2345_views& views, int dir_mode,
                                                        const float* __restrict__ query_center, const float* __restrict__ dirs,
@@ -114,8 +115,10 @@ __device__ __forceinline__ BlendSample blend_front_end(const o2345_points& src, 
   float ev = 3.4e38f;
   s.vmask = false;
   float tx, ty, tz;
-  if (dir_mode == 0) {
-    tx = query_center[0] - px, ty = query_center[1] - py, tz = query_center[2] - pz;
+  if (dir_mode != 1) {
+    // mode 2: every ray is its own camera centre (rays of several cameras in one launch), so c = rays_o[ray]
+    const float* c = dir_mode == 0 ? query_center : src.rays_o + 3 * (gi / src.S);
+    tx = c[0] - px, ty = c[1] - py, tz = c[2] - pz;
     float nn = sqrtf(tx * tx + ty * ty + tz * tz) + 1e-6f;
     tx /= nn, ty /= nn, tz /= nn;
   } else {

@@ -125,16 +125,14 @@ __global__ void ray_merge_kernel(const float* __restrict__ z, const float* __res
   }
 }
 
-// mid-point depths + section lengths + occupancy flag (reference sparse_neus_renderer.py:201-223)
-__global__ void ray_mid_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d, int64_t R,
-                               const float* __restrict__ z, int S, float sample_dist, const float* __restrict__ occ,
-                               int D, float* __restrict__ mid_z, float* __restrict__ dists, uint8_t* __restrict__ active) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= R * S) return;
-  int64_t r = i / S;
-  int s = (int)(i - r * S);
+// mid-point depths + section lengths + occupancy flag (reference sparse_neus_renderer.py:201-223) of sample i = r * S + s;
+// last: the length of ray r's last section
+__device__ __forceinline__ void ray_mid_sample(const float* __restrict__ rays_o, const float* __restrict__ rays_d, int64_t i,
+                                               int64_t r, int s, const float* __restrict__ z, int S, float last,
+                                               const float* __restrict__ occ, int D, float* __restrict__ mid_z,
+                                               float* __restrict__ dists, uint8_t* __restrict__ active) {
   float zi = z[i];
-  float d = (s + 1 < S) ? z[i + 1] - zi : sample_dist;
+  float d = (s + 1 < S) ? z[i + 1] - zi : last;
   float m = zi + d * 0.5f;
   mid_z[i] = m;
   dists[i] = d;
@@ -142,6 +140,26 @@ __global__ void ray_mid_kernel(const float* __restrict__ rays_o, const float* __
   float py = __fadd_rn(rays_o[3 * r + 1], __fmul_rn(rays_d[3 * r + 1], m));
   float pz = __fadd_rn(rays_o[3 * r + 2], __fmul_rn(rays_d[3 * r + 2], m));
   active[i] = (uint8_t)occ_lookup(occ, D, px, py, pz);
+}
+
+__global__ void ray_mid_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d, int64_t R,
+                               const float* __restrict__ z, int S, float sample_dist, const float* __restrict__ occ,
+                               int D, float* __restrict__ mid_z, float* __restrict__ dists, uint8_t* __restrict__ active) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R * S) return;
+  int64_t r = i / S;
+  ray_mid_sample(rays_o, rays_d, i, r, (int)(i - r * S), z, S, sample_dist, occ, D, mid_z, dists, active);
+}
+
+// the same with each ray's own last section (rays of cameras with different near / far in one launch)
+__global__ void ray_mid_per_ray_kernel(const float* __restrict__ rays_o, const float* __restrict__ rays_d, int64_t R,
+                                       const float* __restrict__ z, int S, const float* __restrict__ sample_dist,
+                                       const float* __restrict__ occ, int D, float* __restrict__ mid_z,
+                                       float* __restrict__ dists, uint8_t* __restrict__ active) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= R * S) return;
+  int64_t r = i / S;
+  ray_mid_sample(rays_o, rays_d, i, r, (int)(i - r * S), z, S, sample_dist[r], occ, D, mid_z, dists, active);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -491,6 +509,17 @@ extern "C" int o2345_ray_midpoints(const float* rays_o, const float* rays_d, int
   return O2345_OK;
 }
 
+extern "C" int o2345_ray_midpoints_per_ray(const float* rays_o, const float* rays_d, int64_t R, const float* z, int S,
+                                           const float* sample_dist, const float* occ, int D, float* mid_z, float* dists,
+                                           uint8_t* active, o2345_stream_t stream) {
+  O2345_CHECK_ARG(rays_o && rays_d && z && sample_dist && occ && mid_z && dists && active, "null pointer");
+  if (R == 0) return O2345_OK;
+  ray_mid_per_ray_kernel<<<cdiv(R * S, 256), 256, 0, (cudaStream_t)stream>>>(rays_o, rays_d, R, z, S, sample_dist, occ, D, mid_z,
+                                                                             dists, active);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
 namespace o2345 {
 int launch_render_blend_tc(const o2345_points* src, int64_t n, const uint8_t* active, const float* vol_cl, const float* occ, int D,
                            const o2345_views* views, int dir_mode, const float* query_center, const float* dirs,
@@ -504,7 +533,8 @@ extern "C" int o2345_render_blend(const o2345_points* src, int64_t n, const uint
   O2345_CHECK_ARG(src && vol_cl && occ && views && rnet_pack && rgb, "null pointer");
   O2345_CHECK_ARG(src->mode == O2345_PTS_EXPLICIT || src->mode == O2345_PTS_RAYS, "explicit or ray points only");
   O2345_CHECK_ARG(views->V >= 1 && views->V <= 32 && views->maps && views->proj && views->centers, "1..32 views");
-  O2345_CHECK_ARG((dir_mode == 0 && query_center) || (dir_mode == 1 && dirs), "direction source missing");
+  O2345_CHECK_ARG((dir_mode == 0 && query_center) || (dir_mode == 1 && dirs) || dir_mode == 2, "direction source missing");
+  O2345_CHECK_ARG(dir_mode != 2 || src->mode == O2345_PTS_RAYS, "dir_mode 2 (ray origins) needs ray points");
   O2345_CHECK_ARG(precision == O2345_BLEND_FP32 || precision == O2345_BLEND_TC_FP16, "unknown precision");
   if (n == 0) return O2345_OK;
   if (precision == O2345_BLEND_TC_FP16)

@@ -4,8 +4,11 @@ Command-line mirror of the reference's reconstruction/exp_runner_generic_blender
 modes of the demo configuration:
   export_mesh   <exp_dir>/{pose.json, stage1_8, stage2_8} -> <exp_dir>/mesh.ply   (what run.py's reconstruct() shells out to)
   val           volume-renders the query view -> <exp_dir>/val_color.png, val_depth.npy, val_normal.npy
+  turntable     volume-renders --n_frames views (default 36) on the circle of the input view, at its elevation and radius
+                -> <exp_dir>/turntable/000.png ... (RGBA), <exp_dir>/turntable.gif (on white), turntable_depth.npy [n,H,W]
 A conf with `model.num_lods = 2` adds the lod-1 level (`model.sdf_network_lod1`, `model.rendering_network_lod1`):
-export_mesh writes the lod-1 mesh, and val also writes val_color_lod1.png, val_depth_lod1.npy and val_normal_lod1.npy.
+export_mesh writes the lod-1 mesh, val also writes val_color_lod1.png, val_depth_lod1.npy and val_normal_lod1.npy, and
+turntable renders the lod-1 level.
 `--conf` is parsed (o2345/checkpoints.py: the HOCON subset the reference's confs use; pyhocon is not needed) and supplies
 `model.sdf_network_lod0` (voxel_size, vol_dims, ...), `model.variance_network`, `model.rendering_network`, `model.trainer`
 (samples, perturb) and `general.base_exp_dir`; if the file does not exist the constants of
@@ -24,7 +27,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
 
-def main(argv=None):
+MODES = ("export_mesh", "val", "turntable")
+
+
+def parse_args(argv=None):
     ap = argparse.ArgumentParser()
     ap.add_argument('--conf', type=str, default='./confs/one2345_lod0_val_demo.conf')
     ap.add_argument('--mode', type=str, default='export_mesh')
@@ -38,14 +44,23 @@ def main(argv=None):
     ap.add_argument('--specific_dataset_name', type=str, default='GSO')
     ap.add_argument('--resolution', type=int, default=360)
     ap.add_argument('--checkpoint_path', type=str, default=None, help='ckpt_*.pth of the reference (default: synthetic weights)')
+    ap.add_argument('--n_frames', type=int, default=36, help='turntable: number of views around the object')
     args = ap.parse_args(argv)
-    if args.mode not in ("export_mesh", "val"):
-        raise SystemExit(f"mode={args.mode!r}: only 'export_mesh' and 'val' run on the o2345 path (training stays with the reference)")
+    if args.mode not in MODES:
+        raise SystemExit(f"mode={args.mode!r}: only 'export_mesh' and 'val' of the reference's modes, plus 'turntable', run on the "
+                         "o2345 path (training stays with the reference)")
+    if args.n_frames < 1:
+        raise SystemExit(f"--n_frames must be at least 1, got {args.n_frames}")
+    return args
+
+
+def main(argv=None):
+    args = parse_args(argv)
     if not torch.cuda.is_available():
         raise SystemExit("needs a CUDA device: the o2345 path has no CPU fallback")
     from o2345 import synthetic as S
     from o2345.checkpoints import latest_checkpoint, load_conf, recon_states
-    from o2345.pipeline import build_networks, load_sample
+    from o2345.pipeline import build_networks, load_sample, render_turntable
     dev = torch.device("cuda", args.local_rank)
     torch.cuda.set_device(dev)
     exp_dir = args.specific_dataset_name
@@ -68,6 +83,10 @@ def main(argv=None):
         note("no checkpoint: seeded synthetic reconstruction weights")
     trainer = build_networks(dev, states=states, base_exp_dir=exp_dir, conf=conf,
                              **({} if conf is not None else {"vol_dim": 96, "perturb": 0.0}))
+    if args.mode == "turntable":
+        out = render_turntable(trainer, exp_dir, args.n_frames, out_dir=exp_dir)
+        print(f"{args.n_frames} turntable frames written to {os.path.join(exp_dir, 'turntable')}")
+        return out
     sample = load_sample(exp_dir, dev)
     if args.mode == "export_mesh":
         mesh = trainer(sample, mode="export_mesh", resolution=args.resolution)

@@ -85,6 +85,7 @@ _SIGS = {
     "o2345_ray_merge": (C.c_int, [c_fp, c_fp, C.c_int, c_fp, c_fp, C.c_int, c_i64, c_fp, c_fp, c_fp]),
     "o2345_ray_midpoints": (C.c_int, [c_fp, c_fp, c_i64, c_fp, C.c_int, C.c_float, c_fp, C.c_int, c_fp, c_fp,
                                       c_fp, c_fp]),
+    "o2345_ray_midpoints_per_ray": (C.c_int, [c_fp, c_fp, c_i64, c_fp, C.c_int, c_fp, c_fp, C.c_int, c_fp, c_fp, c_fp, c_fp]),
     "o2345_render_blend": (C.c_int, [C.POINTER(Points), c_i64, c_fp, c_fp, c_fp, C.c_int, C.POINTER(Views),
                                      C.c_int, c_fp, c_fp, c_fp, C.c_int, c_fp, c_fp, c_fp]),
     "o2345_gemm_f16": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, C.c_int, C.c_int, c_i64, c_i64, c_i64, C.c_int, C.c_int,
@@ -129,7 +130,7 @@ _SIGS = {
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 5          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 6          # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 

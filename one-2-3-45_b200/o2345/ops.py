@@ -356,12 +356,19 @@ def ray_merge(z, sdf, new_z, new_sdf):
 
 
 def ray_midpoints(rays_o, rays_d, z, sample_dist, occ):
+    """sample_dist: the last section length of every ray (a number), or a CUDA fp32 tensor [R] with one per ray."""
     R, S = z.shape
     mid = torch.empty_like(z)
     dists = torch.empty_like(z)
     active = torch.empty(R * S, dtype=_u8, device=z.device)
-    L.call("o2345_ray_midpoints", _f(rays_o), _f(rays_d), R, _f(z), S, float(sample_dist), _f(occ), occ.shape[-1],
-           _f(mid), _f(dists), _p(active, _u8), _stream())
+    if torch.is_tensor(sample_dist):
+        if sample_dist.numel() != R:
+            raise L.O2345Error(f"per-ray sample_dist has {sample_dist.numel()} values for {R} rays")
+        L.call("o2345_ray_midpoints_per_ray", _f(rays_o), _f(rays_d), R, _f(z), S, _f(sample_dist), _f(occ), occ.shape[-1],
+               _f(mid), _f(dists), _p(active, _u8), _stream())
+    else:
+        L.call("o2345_ray_midpoints", _f(rays_o), _f(rays_d), R, _f(z), S, float(sample_dist), _f(occ), occ.shape[-1],
+               _f(mid), _f(dists), _p(active, _u8), _stream())
     return mid, dists, active
 
 
@@ -377,13 +384,15 @@ class SourceViews:
 
 
 def render_blend(src: PointSource, active, vol_cl, occ, views: SourceViews, rnet_pack, query_center=None, dirs=None,
-                 precision=L.BLEND_TC_FP16):
-    """precision: L.BLEND_TC_FP16 (mma.sync MLPs, fp16 operands / fp32 accumulate; the default) or L.BLEND_FP32 (fp32 FMA, the
+                 precision=L.BLEND_TC_FP16, ray_origins=False):
+    """Target direction: towards query_center, along dirs, or (ray_origins=True, ray points only) towards each sample's own
+    ray origin, for rays of several cameras in one call.
+    precision: L.BLEND_TC_FP16 (mma.sync MLPs, fp16 operands / fp32 accumulate; the default) or L.BLEND_FP32 (fp32 FMA, the
     reference the parity tests compare against).  Any other value is refused."""
     n, dev = src.n, vol_cl.device
     rgb = torch.empty(n, 3, dtype=_f32, device=dev)
     nvalid = torch.empty(n, dtype=_i32, device=dev)
-    mode = 0 if dirs is None else 1
+    mode = 2 if ray_origins else 0 if dirs is None else 1
     L.call("o2345_render_blend", C.byref(src.struct), n, _p(active, _u8), _f(vol_cl), _f(occ), vol_cl.shape[0],
            C.byref(views.struct), mode, _f(query_center), _f(dirs), _f(rnet_pack), int(precision), _f(rgb), _p(nvalid, _i32),
            _stream())

@@ -152,6 +152,56 @@ def load_sample(folder, device):
 
 
 # --------------------------------------------------------------------------------------
+# turntable: the reconstruction rendered from a circle of cameras around the object
+# --------------------------------------------------------------------------------------
+@torch.no_grad()
+def render_turntable(trainer, sample_or_dir, n_frames=36, out_dir=None, chunk_size=65536):
+    """Volume-renders n_frames views on the circle of the input view (synthetic.orbit_cameras: its elevation and radius,
+    azimuths 0, 360 / n, ...) through trainer.render_cameras, with alpha_inter_ratio 1.0 as `--mode val` renders.
+
+    sample_or_dir: an experiment folder (pose.json, stage1_8/, stage2_8/: read like load_sample) or a sample dict (its
+    trans_mat / scale_mat give the frame).  With out_dir, writes out_dir/turntable/NNN.png (RGBA: colour over opacity,
+    opacity = weights_sum), out_dir/turntable.gif (on white) and out_dir/turntable_depth.npy [n,H,W].
+    Returns render_cameras' dict (device tensors) plus the cameras: c2ws [n,4,4], intrinsics [n,3,3], near_far [n,2]."""
+    dev = next(trainer.parameters()).device
+    if isinstance(sample_or_dir, (str, os.PathLike)):
+        meta = json.load(open(os.path.join(sample_or_dir, "pose.json")))
+        sample = load_sample(sample_or_dir, dev)
+        W, H = (int(v) for v in sample['img_wh'][0])
+        scene = S.scene_cameras(meta, n_src=32, img_wh=(W, H))
+        K = scene["query_intrinsic"]
+    else:
+        sample = sample_or_dir
+        trans_mat = sample['trans_mat'][0].cpu().numpy().astype(np.float64)
+        scene = {"trans_mat": trans_mat, "scale_mat": sample['scale_mat'][0].cpu().numpy()}
+        meta = {"c2ws": {"0": trans_mat @ np.diag([1.0, -1.0, -1.0, 1.0])}}     # view 0 back in pose.json's convention
+        K = sample['intrinsics'][0][0].cpu().numpy()
+    c2ws, intr, near_far = S.normalise_cameras(scene, S.orbit_cameras(meta, n_frames), K)
+    out = trainer.render_cameras(sample, c2ws, intr, near_far, chunk_size=chunk_size, alpha_inter_ratio=1.0)
+    out.update(c2ws=c2ws, intrinsics=intr, near_far=near_far)
+    if out_dir is not None:
+        write_turntable(out, out_dir)
+    return out
+
+
+def write_turntable(frames, out_dir):
+    """out_dir/turntable/NNN.png, turntable.gif and turntable_depth.npy from render_cameras' dict."""
+    from PIL import Image
+    alpha = frames["weights_sum"].clamp(0, 1)[..., None]
+    # the composited colour is premultiplied by the opacity (no background): PNG wants it straight
+    rgba = torch.cat([(frames["color"] / alpha.clamp_min(1e-6)).clamp(0, 1) * (alpha > 0), alpha], -1)
+    on_white = (frames["color"] + (1 - alpha)).clamp(0, 1)
+    to_u8 = lambda x: (x * 255).round().to(torch.uint8).cpu().numpy()
+    rgba, on_white = to_u8(rgba), to_u8(on_white)
+    os.makedirs(os.path.join(out_dir, "turntable"), exist_ok=True)
+    for i, f in enumerate(rgba):
+        Image.fromarray(f, "RGBA").save(os.path.join(out_dir, "turntable", f"{i:03d}.png"))
+    gif = [Image.fromarray(f, "RGB") for f in on_white]
+    gif[0].save(os.path.join(out_dir, "turntable.gif"), save_all=True, append_images=gif[1:], duration=80, loop=0)
+    np.save(os.path.join(out_dir, "turntable_depth.npy"), frames["depth"].cpu().numpy())
+
+
+# --------------------------------------------------------------------------------------
 # run.py end to end (reference run.py:79-119): image -> 8 + 32 generated views -> mesh
 # --------------------------------------------------------------------------------------
 def sample_from_views(stage1, stage2, pose, device, pin=False):

@@ -81,7 +81,7 @@ class SparseNeuSRenderer(nn.Module):
         dev = rays_o.device
         rays_o, rays_d = ops.cf32(rays_o), ops.cf32(rays_d)
         R = rays_o.shape[0]
-        n_s, n_i = self.n_samples, self.n_importance
+        n_s = self.n_samples
         near_t = near if torch.is_tensor(near) else torch.tensor([near], device=dev)
         far_t = far if torch.is_tensor(far) else torch.tensor([far], device=dev)
         near_t, far_t = near_t.to(dev).float(), far_t.to(dev).float()
@@ -97,32 +97,13 @@ class SparseNeuSRenderer(nn.Module):
             z = lower + (upper - lower) * torch.rand(z.shape).to(dev)
         z = z.contiguous()
         vol_cl = channel_last_volume(conditional_volume)
-        occ = ops.cf32(conditional_valid_mask_volume)
         pack = sdf_network.sdf_layer.packed()
-
-        if n_i > 0:
-            sdf = ops.sdf_query(ops.PointSource.rays(rays_o, rays_d, z), vol_cl, pack)["sdf"].view(R, n_s)
-            n_steps = 4
-            u = self._u_table(n_i // n_steps, dev)
-            for i in range(n_steps):
-                new_z = ops.ray_upsample(rays_o, rays_d, z, sdf, 64 * 2 ** i, occ, u)
-                src = ops.PointSource.rays(rays_o, rays_d, new_z)
-                act = ops.occ_nearest(src, occ)
-                new_sdf = ops.sdf_query(src, vol_cl, pack, active=act, inactive_sdf=100.0)["sdf"].view(R, -1)
-                z, sdf = ops.ray_merge(z, sdf, new_z, new_sdf)
-        S = z.shape[1]
-
-        mid, dists, active = ops.ray_midpoints(rays_o, rays_d, z, sample_dist, occ)
-        src = ops.PointSource.rays(rays_o, rays_d, mid)
-        q = ops.sdf_query(src, vol_cl, pack, active=active, inactive_sdf=100.0, want_grad=True)
         views = self._source_views(feature_maps, color_maps, w2cs, intrinsics, img_wh)
         qc = ops.cf32(query_c2w.reshape(-1, 4, 4)[0, :3, 3])
-        color_pts, nvalid = ops.render_blend(src, active, vol_cl, occ, views, rendering_network.packed(), query_center=qc,
-                                             precision=self.blend_precision)
         inv_s = self.variance_network.inv_s()
-        bg = None if background_rgb is None else float(background_rgb)
-        comp = ops.ray_composite(rays_d, mid, dists, q["sdf"], q["grad"], color_pts, active, nvalid, inv_s,
-                                 float(alpha_inter_ratio), bg)
+        z, mid, active, q, comp = self._march(rays_o, rays_d, z, sample_dist, vol_cl, pack, conditional_valid_mask_volume,
+                                              views, rendering_network, qc, inv_s, alpha_inter_ratio, background_rgb)
+        S = z.shape[1]
 
         weights, depth = comp["weights"], comp["depth"]
         pts_mask = active.view(R, S).float()
@@ -159,6 +140,59 @@ class SparseNeuSRenderer(nn.Module):
             'z_vals': z,
             'mid_z_vals': mid,
         }
+
+    def _march(self, rays_o, rays_d, z, sample_dist, vol_cl, pack, conditional_valid_mask_volume, views, rendering_network,
+               query_center, inv_s, alpha_inter_ratio, background_rgb):
+        """Coarse depths z [R, n_samples] -> four importance rounds, SDF and gradient at the section mid-points, view
+        blending and NeuS compositing.  sample_dist: the last section length, one number or a per-ray tensor [R];
+        query_center None: each ray's origin is its camera centre (rays of several cameras).
+        -> (z [R,S], mid [R,S], active [R*S], sdf query dict, ray_composite dict)."""
+        R, n_s = z.shape
+        n_i = self.n_importance
+        occ = ops.cf32(conditional_valid_mask_volume)
+        if n_i > 0:
+            sdf = ops.sdf_query(ops.PointSource.rays(rays_o, rays_d, z), vol_cl, pack)["sdf"].view(R, n_s)
+            n_steps = 4
+            u = self._u_table(n_i // n_steps, z.device)
+            for i in range(n_steps):
+                new_z = ops.ray_upsample(rays_o, rays_d, z, sdf, 64 * 2 ** i, occ, u)
+                src = ops.PointSource.rays(rays_o, rays_d, new_z)
+                act = ops.occ_nearest(src, occ)
+                new_sdf = ops.sdf_query(src, vol_cl, pack, active=act, inactive_sdf=100.0)["sdf"].view(R, -1)
+                z, sdf = ops.ray_merge(z, sdf, new_z, new_sdf)
+
+        mid, dists, active = ops.ray_midpoints(rays_o, rays_d, z, sample_dist, occ)
+        src = ops.PointSource.rays(rays_o, rays_d, mid)
+        q = ops.sdf_query(src, vol_cl, pack, active=active, inactive_sdf=100.0, want_grad=True)
+        color_pts, nvalid = ops.render_blend(src, active, vol_cl, occ, views, rendering_network.packed(), query_center=query_center,
+                                             precision=self.blend_precision, ray_origins=query_center is None)
+        bg = None if background_rgb is None else float(background_rgb)
+        comp = ops.ray_composite(rays_d, mid, dists, q["sdf"], q["grad"], color_pts, active, nvalid, inv_s, float(alpha_inter_ratio),
+                                 bg)
+        return z, mid, active, q, comp
+
+    @inference_only
+    def render_views(self, rays_o, rays_d, near, far, sdf_network, rendering_network, conditional_volume,
+                     conditional_valid_mask_volume, feature_maps, color_maps, w2cs, intrinsics, img_wh, background_rgb=None,
+                     alpha_inter_ratio=0.0):
+        """render() at perturb 0 for rays of many cameras in one call: near / far [R] or [R,1] per ray, the blending
+        direction from each ray's own origin (its camera centre).  Every ray gets the bits render() gives it with its
+        camera's query_c2w and scalar near / far; nothing is drawn from the host generator (no jitter, no sdf_random).
+        -> dict(color [R,3], depth [R,1], weights_sum [R,1], weights [R,S], gradients [R,S,3], inside_sphere [R,S])."""
+        rays_o, rays_d = ops.cf32(rays_o), ops.cf32(rays_d)
+        R, n_s, dev = rays_o.shape[0], self.n_samples, rays_o.device
+        near, far = near.to(dev).float().view(R, 1), far.to(dev).float().view(R, 1)
+        # the same elementwise arithmetic as render()'s scalar near / far, one row per ray
+        z = (near + (far - near) * torch.linspace(0.0, 1.0, n_s).to(dev)[None, :]).contiguous()
+        sample_dist = ((far - near) / n_s).view(R).contiguous()
+        views = self._source_views(feature_maps, color_maps, w2cs, intrinsics, img_wh)
+        z, mid, active, q, comp = self._march(rays_o, rays_d, z, sample_dist, channel_last_volume(conditional_volume),
+                                              sdf_network.sdf_layer.packed(), conditional_valid_mask_volume, views,
+                                              rendering_network, None, self.variance_network.inv_s(), alpha_inter_ratio,
+                                              background_rgb)
+        S = z.shape[1]
+        return {"color": comp["color"], "depth": comp["depth"], "weights_sum": comp["weights_sum"], "weights": comp["weights"],
+                "gradients": q["grad"].view(R, S, 3), "inside_sphere": active.view(R, S).float()}
 
     # ------------------------------------------------------------------ lod-0 pruning for the lod-1 level
     @torch.no_grad()

@@ -256,19 +256,7 @@ def scene_cameras(meta=None, n_src=32, img_wh=(256, 256), factor=1.1):
     scale_mat = np.diag([radius, radius, radius, 1.0]).astype(np.float32)
     scale_mat[:3, 3] = center
 
-    w2cs, c2ws, affine, near_fars = [], [], [], []
-    for e in ext:
-        R = e[:3, :3]
-        cam_center = -R.T @ e[:3, 3]
-        c2w = np.eye(4, dtype=np.float32)
-        c2w[:3, :3] = R.T
-        c2w[:3, 3] = (cam_center - scale_mat[:3, 3].astype(np.float64)) / float(radius)
-        w2c = np.linalg.inv(c2w)
-        a = np.eye(4)
-        a[:3, :4] = K4[:3, :3] @ w2c[:3, :4]
-        dist = math.sqrt(float(np.sum(c2w[:3, 3].astype(np.float64) ** 2)))
-        w2cs.append(w2c), c2ws.append(c2w), affine.append(a)
-        near_fars.append([0.95 * (dist - 1), 1.05 * (dist + 1)])
+    w2cs, c2ws, affine, near_fars = zip(*[_normalised_camera(e, K4[:3, :3], scale_mat) for e in ext])
     f32 = lambda x: np.asarray(x, np.float32)
     w2cs, c2ws, affine, near_fars = f32(w2cs), f32(c2ws), f32(affine), f32(near_fars)
     intr = np.tile(K[None], (len(ids), 1, 1))
@@ -278,7 +266,60 @@ def scene_cameras(meta=None, n_src=32, img_wh=(256, 256), factor=1.1):
         "query_intrinsic": intr[0], "query_near_far": near_fars[0],
         "scale_mat": scale_mat, "trans_mat": f32(ref_inv), "scale_factor": np.float32(1.0 / radius),
         "partial_vol_origin": np.array([-1.0, -1.0, -1.0], np.float32), "img_wh": np.array([W, H]),
+        "ref_inv": ref_inv,   # float64 trans_mat: normalise_cameras reproduces the scene's own cameras bit for bit with it
     }
+
+
+def _normalised_camera(ext, K, scale_mat):
+    """One camera of BlenderPerView.__getitem__'s loop (reference :256-274): ext is its view-0-relative w2c (float64),
+    K [3,3] its intrinsics.  -> (w2c float64, c2w float32, affine K w2c float64, [near, far])."""
+    R = ext[:3, :3]
+    cam_center = -R.T @ ext[:3, 3]
+    c2w = np.eye(4, dtype=np.float32)
+    c2w[:3, :3] = R.T
+    c2w[:3, 3] = (cam_center - scale_mat[:3, 3].astype(np.float64)) / float(scale_mat[0, 0])
+    w2c = np.linalg.inv(c2w)
+    a = np.eye(4)
+    a[:3, :4] = np.asarray(K, np.float64) @ w2c[:3, :4]
+    dist = math.sqrt(float(np.sum(c2w[:3, 3].astype(np.float64) ** 2)))
+    return w2c, c2w, a, [0.95 * (dist - 1), 1.05 * (dist + 1)]
+
+
+_BLENDER2OPENCV = np.diag([1.0, -1.0, -1.0, 1.0])
+
+
+def normalise_cameras(scene, c2ws_blender, intrinsics):
+    """Cameras given in pose.json's frame (Blender c2w [n,4,4] or [4,4]) -> the normalised frame the scene's volume
+    lives in, with the dataset's arithmetic: blender2opencv, then relative to view 0 (w2c @ w2c_ref_inv), then
+    K w2c scale_mat decomposed, near / far from the camera distance (reference BlenderPerView.__getitem__ :172-274).
+
+    scene: scene_cameras' dict (its float64 "ref_inv" reproduces the scene's own cameras bit for bit; a sample's float32
+    "trans_mat" is used when there is none).  intrinsics [3,3] or [n,3,3].
+    Returns float32 (c2w [n,4,4] OpenCV, intrinsics [n,3,3], near_far [n,2])."""
+    poses = np.asarray(c2ws_blender, np.float64).reshape(-1, 4, 4)
+    n = len(poses)
+    K = np.broadcast_to(np.asarray(intrinsics, np.float64).reshape(-1, 3, 3), (n, 3, 3))
+    ref_inv = np.asarray(scene.get("ref_inv", scene["trans_mat"]), np.float64).reshape(4, 4)
+    scale_mat = np.asarray(scene["scale_mat"], np.float32).reshape(4, 4)
+    c2ws, near_fars = [], []
+    for pose, k in zip(poses, K):
+        _, c2w, _, nf = _normalised_camera(np.linalg.inv(pose @ _BLENDER2OPENCV) @ ref_inv, k, scale_mat)
+        c2ws.append(c2w), near_fars.append(nf)
+    return np.asarray(c2ws, np.float32), K.astype(np.float32), np.asarray(near_fars, np.float32)
+
+
+def orbit_cameras(meta, n_frames):
+    """n_frames Blender c2w [n,4,4] on the circle of the input view (view 0 of pose.json): its elevation and radius, at
+    azimuths 0, 360 / n, ... degrees from it, looking at the origin (reference utils/utils.py:80-145, _look_at_poses)."""
+    c = np.asarray(next(iter(meta["c2ws"].values())), np.float64)[:3, 3]
+    radius = float(np.linalg.norm(c))
+    polar = math.acos(max(-1.0, min(1.0, c[2] / radius)))
+    azim0 = math.atan2(c[0], -c[1])
+    azim = azim0 + 2 * math.pi * np.arange(n_frames) / n_frames
+    poses = _look_at_poses(np.full(n_frames, polar), azim, radius)
+    out = np.tile(np.eye(4, dtype=np.float32), (n_frames, 1, 1))
+    out[:, :3, :] = poses
+    return out
 
 
 def query_rays(intrinsic, c2w, H=256, W=256):

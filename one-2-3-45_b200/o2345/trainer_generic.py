@@ -136,6 +136,64 @@ class GenericTrainer(nn.Module):
                            "normal" + suffix: torch.cat(normals).cpu().numpy()})
         return result
 
+    # ------------------------------------------------------------------ any camera
+    @torch.no_grad()
+    def render_cameras(self, sample, c2ws, intrinsics, near_far, img_wh=None, chunk_size=65536, background_rgb=None,
+                       alpha_inter_ratio=0.0):
+        """Volume-renders the scene of `sample` from C cameras of its normalised frame (synthetic.normalise_cameras):
+        c2ws [C,4,4] OpenCV c2w, intrinsics [C,3,3] (or one [3,3]), near_far [C,2].  The feature maps and the conditional
+        volume are built once; the rays of every camera (pixel centres as the query view's, row-major) are concatenated
+        and marched in launch groups of `chunk_size` rays that may mix cameras.  With num_lods = 2 the lod-1 level (the
+        one export_mesh meshes) is rendered.  No jitter and no draws from the host generator: camera c gets the bits of
+        val_step(perturb_overwrite=0) for a sample whose query camera is c.
+        Returns device tensors: color [C,H,W,3], depth [C,H,W], normal [C,H,W,3] (val_step's formula) and weights_sum
+        [C,H,W] (the opacity, for RGBA frames)."""
+        from .synthetic import query_rays
+        as_np = lambda x: (x.detach().cpu().numpy() if torch.is_tensor(x) else np.asarray(x)).astype(np.float32)
+        c2ws = as_np(c2ws).reshape(-1, 4, 4)
+        n_cam = len(c2ws)
+        if chunk_size < 1 or n_cam == 0:
+            raise ValueError(f"chunk_size must be >= 1 and at least one camera is needed (got {chunk_size}, {n_cam})")
+        intrinsics = np.broadcast_to(as_np(intrinsics).reshape(-1, 3, 3), (n_cam, 3, 3))
+        near_far = as_np(near_far).reshape(n_cam, 2)
+        imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
+        renderer, sdf_net, rnet, vol, occ, fm = (self.sdf_renderer_lod0, self.sdf_network_lod0, self.rendering_network_lod0,
+                                                 cond['dense_volume_scale0'], cond['valid_mask_volume_scale0'], fmaps)
+        if self.num_lods > 1:
+            fmaps1, cond1 = self._lod1_volume(sample, imgs, cond, sizeW, sizeH)
+            renderer, sdf_net, rnet, vol, occ, fm = (self.sdf_renderer_lod1, self.sdf_network_lod1, self.rendering_network_lod1,
+                                                     cond1['dense_volume_scale1'], cond1['valid_mask_volume_scale1'], fmaps1)
+        W, H = (sizeW, sizeH) if img_wh is None else (int(img_wh[0]), int(img_wh[1]))
+        dev = vol.device
+        HW = H * W
+        rays = [query_rays(k, c, H, W) for k, c in zip(intrinsics, c2ws)]
+        rays_o = torch.from_numpy(np.concatenate([o for o, _ in rays])).to(dev)
+        rays_d = torch.from_numpy(np.concatenate([v for _, v in rays])).to(dev)
+        nf = torch.from_numpy(np.repeat(near_far, HW, axis=0)).to(dev)
+        # val_step marches 512-ray chunks and sums the normals per chunk; torch's reduction order depends on the tensor
+        # shape, so the normals are summed over the same per-camera 512-ray units.  A launch group is whole units.
+        unit = min(512, chunk_size)
+        units = [(c * HW + a, c * HW + min(a + unit, HW)) for c in range(n_cam) for a in range(0, HW, unit)]
+        groups, start = [], 0
+        for i in range(1, len(units) + 1):
+            if i == len(units) or units[i][1] - units[start][0] > max(chunk_size, unit):
+                groups.append(units[start:i])
+                start = i
+        color = torch.empty(n_cam * HW, 3, device=dev)
+        depth, opacity = torch.empty(n_cam * HW, 1, device=dev), torch.empty(n_cam * HW, 1, device=dev)
+        normal = torch.empty(n_cam * HW, 3, device=dev)
+        for g in groups:
+            a, b = g[0][0], g[-1][1]
+            out = renderer.render_views(rays_o[a:b], rays_d[a:b], nf[a:b, 0], nf[a:b, 1], sdf_net, rnet, vol, occ, fm, imgs,
+                                        sample['w2cs'][0], sample['intrinsics'][0], [sizeW, sizeH],
+                                        background_rgb=background_rgb, alpha_inter_ratio=alpha_inter_ratio)
+            color[a:b], depth[a:b], opacity[a:b] = out["color"], out["depth"], out["weights_sum"]
+            terms = out['gradients'] * out['weights'][:, :, None] * out['inside_sphere'][..., None]    # elementwise: any shape
+            for u0, u1 in g:
+                torch.sum(terms[u0 - a:u1 - a], dim=1, out=normal[u0:u1])
+        return {"color": color.view(n_cam, H, W, 3), "depth": depth.view(n_cam, H, W), "normal": normal.view(n_cam, H, W, 3),
+                "weights_sum": opacity.view(n_cam, H, W)}
+
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False):
