@@ -649,19 +649,47 @@ constexpr int smem_bytes(int bn, int stages) {
   return stages * (BM * BK * 2 + bn * BK * 2) + epi_slab_bytes(bn) + 2 * stages * 8 + 16 + epi_smem_bytes(bn) + 1024;
 }
 
-// One stage of the TMA producer: the 128 rows of A and the BN rows of B for k-block kb of the tile at (m0, n0).
+// Where the producer's next k-block comes from.  The producer is one thread that waits for a free stage and then issues its
+// loads, so every instruction between the two adds to the latency of refilling the ring.  Integer divisions by runtime sizes
+// cost ~100 cycles of dependent instructions each.  So the tile's pixel origin and batch indices are computed once per
+// tile, and the conv's (tap, channel block) is stepped along with kb instead of divided out of it.
+struct ProducerPos {
+  int x, y, b;       // conv: tile origin in the activation (x, y, image); batched: (head, batch) in (y, b)
+  int tap, tx, ty;   // conv: tap of the next k-block and its column / row in the tap grid
+  int cb;            // conv: channel block of the next k-block
+};
+__device__ __forceinline__ ProducerPos producer_start(const GemmParams& p, int m0, int bz, int kb0) {
+  ProducerPos q;
+  q.x = q.y = q.b = q.tap = q.tx = q.ty = q.cb = 0;
+  if (p.conv) {
+    const int r = m0 / p.cW;
+    q.x = m0 - r * p.cW, q.y = r % p.cH, q.b = r / p.cH;
+    q.tap = kb0 / p.cblocks, q.cb = kb0 - q.tap * p.cblocks;
+    q.ty = q.tap / p.ctx, q.tx = q.tap - q.ty * p.ctx;
+  } else if (p.batched) {
+    q.y = bz % p.nh, q.b = bz / p.nh;
+  }
+  return q;
+}
+__device__ __forceinline__ void producer_step(const GemmParams& p, ProducerPos& q) {
+  if (p.conv && ++q.cb == p.cblocks) {
+    q.cb = 0, ++q.tap;
+    if (++q.tx == p.ctx) q.tx = 0, ++q.ty;
+  }
+}
+
+// One stage of the TMA producer: the 128 rows of A and the BN rows of B for k-block kb of the tile at (m0, n0); q is kb's position.
 template <int BN>
 __device__ __forceinline__ void produce_stage(const GemmParams& p, const CUtensorMap* tmA, const CUtensorMap* tmB, uint8_t* a_dst,
-                                              uint8_t* b_dst, uint64_t* full_bar, int kb, int m0, int n0, int bz) {
+                                              uint8_t* b_dst, uint64_t* full_bar, int kb, int m0, int n0, const ProducerPos& q) {
   mbar_expect_tx(full_bar, BM * BK * 2 + BN * BK * 2);
   if (p.conv) {
-    const int tap = kb / p.cblocks, c0 = (kb - tap * p.cblocks) * BK;
-    const int x0 = m0 % p.cW, y0 = (m0 / p.cW) % p.cH, b0 = m0 / (p.cW * p.cH);
-    tma_load_4d(a_dst, tmA, full_bar, c0, x0 + tap % p.ctx + p.cox, y0 + tap / p.ctx + p.coy, b0);
-    tma_load_2d(b_dst, tmB, full_bar, tap * p.cC + c0, n0);
+    const int c0 = q.cb * BK;
+    tma_load_4d(a_dst, tmA, full_bar, c0, q.x + q.tx + p.cox, q.y + q.ty + p.coy, q.b);
+    tma_load_2d(b_dst, tmB, full_bar, q.tap * p.cC + c0, n0);
   } else if (p.batched) {
-    tma_load_4d(a_dst, tmA, full_bar, kb * BK, m0, bz % p.nh, bz / p.nh);
-    tma_load_4d(b_dst, tmB, full_bar, kb * BK, n0, bz % p.nh, bz / p.nh);
+    tma_load_4d(a_dst, tmA, full_bar, kb * BK, m0, q.y, q.b);
+    tma_load_4d(b_dst, tmB, full_bar, kb * BK, n0, q.y, q.b);
   } else {
     tma_load_2d(a_dst, tmA, full_bar, kb * BK, m0);
     tma_load_2d(b_dst, tmB, full_bar, kb * BK, n0);
@@ -735,12 +763,14 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (warp < 4) {
     if (threadIdx.x == 0) {  // ---------------- TMA producer
       asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the epilogue's generic accesses to the ring come first
+      ProducerPos q = producer_start(p, m0, bz, kb0);
       for (int kb = kb0; kb < kb1; ++kb) {
         const uint32_t c = cnt + (kb - kb0);
         const int s = c % STAGES;
         const uint32_t ph = (c / STAGES) & 1;
         mbar_wait(empty + s, ph ^ 1, p, WAIT_EMPTY, s);
-        produce_stage<BN>(p, &tmA, &tmB, sA + s * A_BYTES, sB + s * B_BYTES, full + s, kb, m0, n0, bz);
+        produce_stage<BN>(p, &tmA, &tmB, sA + s * A_BYTES, sB + s * B_BYTES, full + s, kb, m0, n0, q);
+        producer_step(p, q);
         if (kb == kb0) stamp(p, 2);
       }
       stamp(p, 3);
