@@ -32,11 +32,13 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 6   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 7   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
-                                 6: rays of many cameras in one launch: render_blend dir_mode 2, o2345_ray_midpoints_per_ray */
+                                 6: rays of many cameras in one launch: render_blend dir_mode 2, o2345_ray_midpoints_per_ray
+                                 7: the GEMM epilogue's GroupNorm column statistics are gone: o2345_epilogue lost its last two fields,
+                                    and the norm + patch gather entry point that read the tables went with them */
 
 typedef void* o2345_stream_t;
 
@@ -332,11 +334,6 @@ typedef struct {
                             32 = 16 values followed by their 16 gates, C gets N/2 columns value * gelu(gate) */
   float alpha;           /* scale on the accumulator */
   int out_f32;           /* C is fp32 instead of fp16 */
-  float* colstats;       /* optional fp32 [M / stats_rows_per_group, 2, N], zero on entry: the kernel ADDS, per row group (image)
-                            and column, the sum and the sum of squares of the fp16 values it writes -- the statistics the next
-                            GroupNorm needs (openaimodel.py:256-276), so that no kernel has to re-read the tensor for them.
-                            fp16 output, act 0, N and ldc multiples of 8; stats_rows_per_group 64 or a multiple of 128 */
-  int stats_rows_per_group;
 } o2345_epilogue;
 
 int o2345_gemm_f16(const void* A, const void* B, void* C, int M, int N, int K, int64_t lda, int64_t ldb,
@@ -413,13 +410,6 @@ void o2345_debug_groupnorm_cluster(int cl);
  * pad_lo on the low side (pad_lo < 0: k/2; pad_lo = 0 reproduces the VAE encoder's F.pad(x, (0,1,0,1))). */
 int o2345_norm_act_im2col(const void* x, int B, int H, int W, int C, int ksize, int stride, int upsample, int pad_lo,
                           const float* scale, const float* shift, int act, void* out, o2345_stream_t stream);
-/* The same gather with GroupNorm(x) (+SiLU if act) computed from RAW statistics: stats_a [B, 2, Ca] (sum, then sum of squares,
- * per image and channel, over the H*W pixels of x) for channels [0, Ca) and stats_b [B, 2, C - Ca] for the rest (NULL when
- * Ca == C) -- the tables the producing GEMMs accumulated through o2345_epilogue.colstats (two tables: x is a channel
- * concat).  G groups, eps, gamma / beta [C] (may be NULL).  Replaces o2345_groupnorm_stats + o2345_norm_act_im2col. */
-int o2345_norm_act_im2col_stats(const void* x, int B, int H, int W, int C, int ksize, int stride, int upsample, int pad_lo,
-                                const float* stats_a, int Ca, const float* stats_b, int G, float eps, const float* gamma,
-                                const float* beta, int act, void* out, o2345_stream_t stream);
 int o2345_layernorm_rows(const void* x, int64_t M, int C, float eps, const float* gamma, const float* beta, void* y,
                          o2345_stream_t stream);
 int o2345_softmax_rows(const void* s, int64_t rows, int n, void* p, o2345_stream_t stream);

@@ -141,10 +141,6 @@ struct GemmParams {
   int splits;
   float* ws;
   int persist;                 // 1: a grid of at most one CTA per SM walks the tiles (staged epilogues only)
-  // GroupNorm statistics of the OUTPUT: colstats[(g * 2 + 0) * N + col] += x and colstats[(g * 2 + 1) * N + col] += x^2 over the
-  // final fp16 values of row group g = row / stats_rpg (the consumer turns them into mean / rstd); nullptr: off
-  float* colstats;
-  int stats_rpg, stats_groups;
   long long* trace;            // diagnostic: CTA (0,0,0) stores clock64() stamps of its phases (o2345_debug_gemm_trace), else nullptr
   TrapRecord* diag;            // host-mapped record written before a bounded wait traps (may be nullptr)
   int bn, mode;                // for the trap record
@@ -301,17 +297,9 @@ __device__ __forceinline__ void splitk_partial(const GemmParams& p, const uint32
 // (row, 8 columns) when N and ldc allow 16-byte accesses, else one per element.  The planes were written by other SMs: reads
 // bypass L1.  Row-bias / residual loads are issued before the plane sums so that one round trip covers them all.
 template <int BN>
-__device__ __forceinline__ void splitk_finalize(const GemmParams& p, int m0, int n0, int z, int te, float* sstat) {
+__device__ __forceinline__ void splitk_finalize(const GemmParams& p, int m0, int n0, int z, int te) {
   const bool vec = (p.N % 8) == 0 && (p.ldc % 8) == 0 && (!p.rowbias || (p.rowbias_ld % 8) == 0);
   const int64_t plane = (int64_t)p.M * p.N;
-  // GroupNorm statistics (fp16 output only; the host refuses other combinations): this split's rows fall into at most
-  // two row groups (stats_rpg is a multiple of 128, or 64): shared-memory accumulators [2 groups][2 moments][BN], then one
-  // red.add per column, moment and group for the whole share.
-  const bool stats = p.colstats != nullptr && vec && !p.out_f32;
-  if (stats) {
-    for (int i = te; i < 4 * BN; i += EPI_THREADS) sstat[i] = 0.f;
-    epi_bar();
-  }
   if (vec) {
     constexpr int PPR = BN / 8;
     constexpr int NP = BM * PPR;
@@ -371,24 +359,6 @@ __device__ __forceinline__ void splitk_finalize(const GemmParams& p, int m0, int
         for (int e = 0; e < 8; ++e) v[e] += __half2float(h[e]);
       }
       store8(p, o, v);
-      if (stats) {
-        float* acc = sstat + (row / p.stats_rpg - m0 / p.stats_rpg) * 2 * BN + (col - n0);
-#pragma unroll
-        for (int e = 0; e < 8; ++e) {
-          const float x = __half2float(__float2half_rn(v[e]));       // the value the consumer will read back
-          atomicAdd(acc + e, x), atomicAdd(acc + BN + e, x * x);
-        }
-      }
-    }
-    if (stats) {
-      epi_bar();
-      const int g0 = m0 / p.stats_rpg;
-      const int last_row = m0 + BM - 1 < p.M ? m0 + BM - 1 : p.M - 1;
-      const int ng = last_row / p.stats_rpg - g0 + 1;                 // 1 or 2
-      for (int i = te; i < ng * 2 * BN; i += EPI_THREADS) {
-        const int gi = i / (2 * BN), rem = i - gi * 2 * BN, mom = rem / BN, c = rem - mom * BN;
-        if (n0 + c < p.N && sstat[i] != 0.f) atomicAdd(p.colstats + ((int64_t)(g0 + gi) * 2 + mom) * p.N + n0 + c, sstat[i]);
-      }
     }
     return;
   }
@@ -574,10 +544,7 @@ __device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpO
       const int grow = row0 + rl, col = g.ocol0 + ci * 8;
       if (grow < p.M && col < g.nout) {
         uint4 v = *reinterpret_cast<const uint4*>(slab + rl * g.stride + ci * 16);
-        if (p.residual) {
-          v = add_h8(v, resq[u]);
-          if (p.colstats) *reinterpret_cast<uint4*>(slab + rl * g.stride + ci * 16) = v;   // the statistics see the final value
-        }
+        if (p.residual) v = add_h8(v, resq[u]);
         *reinterpret_cast<uint4*>(C + out_row(p, grow) * p.ldc + col) = v;
       }
     }
@@ -602,44 +569,8 @@ __device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpO
 #pragma unroll
     for (int u = 0; u < UN; ++u) {
       if (!ok[u]) continue;
-      if (p.residual) {
-        v[u] = add_h8(v[u], q[u]);
-        if (p.colstats) {
-          const int pp = base + 32 * u;
-          const int rl = pp / g.ppr, ci = pp - rl * g.ppr;
-          *reinterpret_cast<uint4*>(slab + rl * g.stride + ci * 16) = v[u];
-        }
-      }
+      if (p.residual) v[u] = add_h8(v[u], q[u]);
       *reinterpret_cast<uint4*>(C + o[u]) = v[u];
-    }
-  }
-  // GroupNorm statistics of the tensor just written (the consumer's GroupNorm needs sum and sum of squares per image and
-  // channel group): column sums over this warp's 32 rows -- all in one image, stats_rpg is a multiple of 32 -- read back
-  // from the slab (lanes walk columns, conflict-free), one red.add per column and moment.
-  if (MODE == 0 && p.colstats) {
-    __syncwarp();
-    const int nrows = p.M - row0 < 32 ? p.M - row0 : 32;
-    if (nrows > 0) {
-      float* ssum = p.colstats + (int64_t)(row0 / p.stats_rpg) * 2 * g.nout;
-      for (int cp = lane; 2 * cp < g.outc; cp += 32) {
-        const int col = g.ocol0 + 2 * cp;
-        if (col >= g.nout) break;
-        float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-        if (nrows == 32) {
-#pragma unroll 8
-          for (int r = 0; r < 32; ++r) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(slab + r * g.stride + cp * 4));
-            s0 += f.x, s1 += f.y, q0 = fmaf(f.x, f.x, q0), q1 = fmaf(f.y, f.y, q1);
-          }
-        } else {
-          for (int r = 0; r < nrows; ++r) {
-            const float2 f = __half22float2(*reinterpret_cast<const __half2*>(slab + r * g.stride + cp * 4));
-            s0 += f.x, s1 += f.y, q0 = fmaf(f.x, f.x, q0), q1 = fmaf(f.y, f.y, q1);
-          }
-        }
-        atomicAdd(ssum + col, s0), atomicAdd(ssum + col + 1, s1);
-        atomicAdd(ssum + g.nout + col, q0), atomicAdd(ssum + g.nout + col + 1, q1);
-      }
     }
   }
 }
@@ -847,7 +778,7 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     cluster_sync_all();
     if (warp >= 4) {   // every split finalizes its share of the 128 x BN block: sum of the planes + epilogue
       if (threadIdx.x == 128) stamp_ns(p, 21, true);
-      splitk_finalize<BN>(p, blockIdx.x * BM, blockIdx.y * BN, bz, threadIdx.x - 128, reinterpret_cast<float*>(smem));
+      splitk_finalize<BN>(p, blockIdx.x * BM, blockIdx.y * BN, bz, threadIdx.x - 128);
       if (threadIdx.x == 128) stamp_ns(p, 22, true);
     }
   }
@@ -1039,20 +970,15 @@ int launch_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const Gemm
 
 // ring depth per tile width: as many stages as fit next to the epilogue slabs in 227 KB (one CTA per SM)
 int dispatch(const Config& c, int mode, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, int batch, cudaStream_t st) {
-  if (p.colstats && mode == 3 && c.splits <= 1) {
-    set_error("o2345_gemm_f16: column statistics need the staged fp16 epilogue (16-byte aligned C / residual) or split-K");
-    return O2345_EUNSUPPORTED;
-  }
   if (c.bn == 64) return launch_mode<64, 6>(mode, a, b, p, batch, c.persist, st);
   if (c.bn == 128) return launch_mode<128, 5>(mode, a, b, p, batch, c.persist, st);
   if (c.bn == 160) return launch_mode<160, 4>(mode, a, b, p, batch, c.persist, st);
   return launch_mode<256, 3>(mode, a, b, p, batch, c.persist, st);
 }
 
-int fill_epilogue(GemmParams& p, const o2345_epilogue* ep, int M, int N, int64_t ldc) {
+int fill_epilogue(GemmParams& p, const o2345_epilogue* ep, int N, int64_t ldc) {
   p.bias = nullptr, p.rowbias = nullptr, p.rowbias_ld = 0, p.rows_per_group = 1, p.residual = nullptr;
   p.out_f32 = 0, p.act = 0, p.alpha = 1.f, p.trace = g_trace;
-  p.colstats = nullptr, p.stats_rpg = 1, p.stats_groups = 0;
   p.diag = nullptr, p.bn = p.mode = 0;
   if (!ep) return O2345_OK;
   O2345_CHECK_ARG(ep->act >= 0 && ep->act <= 4, "unknown activation");
@@ -1063,13 +989,6 @@ int fill_epilogue(GemmParams& p, const o2345_epilogue* ep, int M, int N, int64_t
   p.bias = ep->bias, p.rowbias = reinterpret_cast<const __half*>(ep->rowbias), p.rowbias_ld = ep->rowbias_ld;
   p.rows_per_group = ep->rowbias ? ep->rows_per_group : 1;
   p.residual = reinterpret_cast<const __half*>(ep->residual), p.out_f32 = ep->out_f32, p.act = ep->act, p.alpha = ep->alpha;
-  if (ep->colstats) {
-    O2345_CHECK_ARG(ep->act == 0 && !ep->out_f32 && (N % 8) == 0 && (ldc % 8) == 0,
-                    "column statistics: fp16 output without activation, N and ldc multiples of 8");
-    O2345_CHECK_ARG(ep->stats_rows_per_group > 0 && ((ep->stats_rows_per_group % 128) == 0 || ep->stats_rows_per_group == 64),
-                    "column statistics: rows per group must be 64 or a multiple of 128");
-    p.colstats = ep->colstats, p.stats_rpg = ep->stats_rows_per_group, p.stats_groups = cdiv(M, ep->stats_rows_per_group);
-  }
   return O2345_OK;
 }
 
@@ -1133,7 +1052,7 @@ int conv_launch(const void* x, int B, int H, int W, int C, const void* weight, i
   }
   GemmParams p;
   p.M = B * H * W, p.N = N, p.K = taps * C, p.ldc = ldc, p.nh = 1, p.stride_c_h = 0, p.stride_c_b = 0, p.C = out;
-  int rc = fill_epilogue(p, ep, p.M, N, ldc);
+  int rc = fill_epilogue(p, ep, N, ldc);
   if (rc) return rc;
   p.batched = 0, p.conv = 1, p.cC = C, p.cH = H, p.cW = W, p.cblocks = (C + BK - 1) / BK;
   p.ctaps = taps, p.ctx = tx, p.cox = ox, p.coy = oy, p.up = up, p.upa = upa, p.upb = upb;
@@ -1172,8 +1091,8 @@ extern "C" int o2345_conv_up2x_f16(const void* x, int B, int H, int W, int C, co
   O2345_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && (C % 8) == 0 && N > 0, "bad sizes (C must be a multiple of 8)");
   O2345_CHECK_ARG(conv_tiles(H, W), "up-sampling conv: the LOW-resolution image must tile into 128-pixel boxes (see o2345_conv3x3_f16)");
   O2345_CHECK_ARG(((uintptr_t)x % 16) == 0 && ((uintptr_t)weight4 % 16) == 0, "operands must be 16-byte aligned");
-  O2345_CHECK_ARG(!ep || (!ep->residual && !ep->colstats && !ep->rowbias && ep->act != 3),
-                  "up-sampling conv: bias / activation epilogues only (no residual, row bias, statistics, GEGLU)");
+  O2345_CHECK_ARG(!ep || (!ep->residual && !ep->rowbias && ep->act != 3),
+                  "up-sampling conv: bias / activation epilogues only (no residual, row bias, GEGLU)");
   O2345_CHECK_ARG((int64_t)B * 4 * H * W < (1ll << 31), "output rows must fit 31 bits");
   const __half* w = reinterpret_cast<const __half*>(weight4);
   for (int ph = 0; ph < 4; ++ph) {   // phase (a, b) = (row parity, column parity) of the output pixel
@@ -1197,7 +1116,7 @@ extern "C" int o2345_gemm_f16(const void* A, const void* B, void* C, int M, int 
                   "batch strides must be multiples of 8 fp16");
   GemmParams p;
   p.M = M, p.N = N, p.K = K, p.ldc = ldc, p.nh = nh > 0 ? nh : 1, p.stride_c_h = stride_c_h, p.stride_c_b = stride_c_b, p.C = C;
-  int rc = fill_epilogue(p, ep, M, N, ldc);
+  int rc = fill_epilogue(p, ep, N, ldc);
   if (rc) return rc;
   O2345_CHECK_ARG(nh == 0 || (!p.rowbias && p.act != 3), "row bias / GEGLU are not available in batched mode");
   p.batched = nh > 0 ? 1 : 0;

@@ -199,73 +199,6 @@ __global__ void norm_act_apply_kernel(const __half* __restrict__ x, int HW, int 
   }
 }
 
-// The same gather with the GroupNorm finished IN the consumer: instead of a scale / shift table it receives the raw per-(image,
-// channel) sums and sums of squares that the PRODUCING GEMM accumulated in its epilogue (o2345_epilogue.colstats) -- for a
-// channel concat, one table per part -- and turns them into mean / rstd per group in its prologue: no kernel re-reads the
-// activation for statistics (round 1: 77 groupnorm_stats launches per UNet iteration).
-// grid (chunks, B); blockDim is a multiple of C / 8, so a thread's 8-channel slot (and its scale / shift) never changes.
-__global__ void norm_act_im2col_stats_kernel(const __half* __restrict__ x, int H, int W, int C, int KS, int stride, int up,
-                                             const float* __restrict__ stats_a, int Ca, const float* __restrict__ stats_b, int G,
-                                             float eps, const float* __restrict__ gamma, const float* __restrict__ beta, int act,
-                                             __half* __restrict__ out, int Ho, int Wo, int pad, int items) {
-  pdl_wait();
-  pdl_trigger();
-  extern __shared__ float gs[];            // [G] sum -> mean, [G] sum of squares -> rstd
-  const int b = blockIdx.y, cg = C / G, c8 = C >> 3, Cb = C - Ca;
-  // every thread fetches the two moments of a few channels (ONE L2 round trip for the whole CTA) and folds them into the
-  // group sums in shared memory; a serial per-group loop would cost cg dependent round trips in every CTA
-  for (int g = threadIdx.x; g < 2 * G; g += blockDim.x) gs[g] = 0.f;
-  __syncthreads();
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const float* t = c < Ca ? stats_a + (int64_t)b * 2 * Ca + c : stats_b + (int64_t)b * 2 * Cb + (c - Ca);
-    const int ld = c < Ca ? Ca : Cb;
-    atomicAdd(gs + c / cg, __ldcg(t));
-    atomicAdd(gs + G + c / cg, __ldcg(t + ld));
-  }
-  __syncthreads();
-  if (threadIdx.x < G) {
-    const int g = threadIdx.x;
-    const float n = (float)H * (float)W * (float)cg, m = gs[g] / n, q = gs[G + g] / n;
-    gs[g] = m, gs[G + g] = rsqrtf(fmaxf(q - m * m, 0.f) + eps);
-  }
-  __syncthreads();
-  const int slot = threadIdx.x % c8;
-  float sv[8], tv[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const int c = slot * 8 + e, g = c / cg;
-    const float ga = gamma ? gamma[c] : 1.f, be = beta ? beta[c] : 0.f, r = gs[G + g];
-    sv[e] = r * ga, tv[e] = be - gs[g] * r * ga;
-  }
-  const int64_t per_image = (int64_t)Ho * Wo * KS * KS * c8;
-  const int Hin = up ? 2 * H : H, Win = up ? 2 * W : W;
-  for (int k = 0; k < items; ++k) {
-    const int64_t idx = ((int64_t)blockIdx.x * items + k) * blockDim.x + threadIdx.x;   // idx % c8 == slot
-    if (idx >= per_image) return;
-    const int kk = (int)((idx / c8) % (KS * KS));
-    const int64_t pix = idx / ((int64_t)c8 * KS * KS);
-    const int ox = (int)(pix % Wo), oy = (int)(pix / Wo);
-    const int ky = kk / KS, kx = kk % KS;
-    const int iy = oy * stride + ky - pad, ix = ox * stride + kx - pad;
-    uint4 o = make_uint4(0, 0, 0, 0);
-    if (iy >= 0 && iy < Hin && ix >= 0 && ix < Win) {
-      const int sy = up ? iy >> 1 : iy, sx = up ? ix >> 1 : ix;
-      const uint4 v = *reinterpret_cast<const uint4*>(x + (((int64_t)b * H + sy) * W + sx) * C + slot * 8);
-      const __half2* h = reinterpret_cast<const __half2*>(&v);
-      __half2 r[4];
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        float2 f = __half22float2(h[e]);
-        f.x = fmaf(f.x, sv[2 * e], tv[2 * e]), f.y = fmaf(f.y, sv[2 * e + 1], tv[2 * e + 1]);
-        if (act) f.x = silu(f.x), f.y = silu(f.y);
-        r[e] = __floats2half2_rn(f.x, f.y);
-      }
-      o = *reinterpret_cast<uint4*>(r);
-    }
-    *reinterpret_cast<uint4*>(out + (((int64_t)b * Ho * Wo + pix) * KS * KS + kk) * C + slot * 8) = o;
-  }
-}
-
 // GroupNorm (+SiLU) of a whole activation in ONE kernel (ksize 1: the implicit-conv and transformer inputs, 55 of the 61 GroupNorms
 // of a UNet pass): an image is handled by one thread-block CLUSTER of CL CTAs.  Pass 1: every CTA reads its slab of pixels
 // ONCE (16-byte loads, four in flight per thread, a thread keeps its 8-channel slot), parks it in shared memory (KEEP) and sums
@@ -739,27 +672,6 @@ extern "C" int o2345_norm_act_im2col(const void* x, int B, int H, int W, int C, 
   int64_t total = (int64_t)B * Ho * Wo * ksize * ksize * (C / 8);
   O2345_CUDA(launch_pdl(norm_act_im2col_kernel, dim3(cdiv(total, 256)), dim3(256), (size_t)(0), ST, (const __half*)x, B, H, W, C, ksize, stride, upsample, scale, shift,
                                                            act, (__half*)out, Ho, Wo, pad));
-  O2345_LAUNCH_CHECK();
-  return O2345_OK;
-}
-
-extern "C" int o2345_norm_act_im2col_stats(const void* x, int B, int H, int W, int C, int ksize, int stride, int upsample, int pad_lo,
-                                           const float* stats_a, int Ca, const float* stats_b, int G, float eps, const float* gamma,
-                                           const float* beta, int act, void* out, o2345_stream_t stream) {
-  O2345_CHECK_ARG(x && out && stats_a && (C % 8) == 0 && C / 8 <= 512 && (ksize == 1 || ksize == 3) && (stride == 1 || stride == 2),
-                  "bad arguments");
-  O2345_CHECK_ARG(G > 0 && G <= 256 && (C % G) == 0 && Ca > 0 && Ca <= C && (Ca == C) == (stats_b == nullptr),
-                  "groups must divide C; stats_b covers the channels past Ca (NULL when Ca == C)");
-  int Hin = upsample ? 2 * H : H, Win = upsample ? 2 * W : W;
-  int pad_hi = ksize / 2, pad = pad_lo < 0 ? ksize / 2 : pad_lo;
-  int Ho = (Hin + pad + pad_hi - ksize) / stride + 1, Wo = (Win + pad + pad_hi - ksize) / stride + 1;
-  const int c8 = C / 8;
-  const int threads = (512 / c8) * c8;                 // a multiple of the channel slots: a thread keeps its slot
-  const int items = 4;
-  const int64_t per_image = (int64_t)Ho * Wo * ksize * ksize * c8;
-  O2345_CUDA(launch_pdl(norm_act_im2col_stats_kernel, dim3(cdiv(per_image, (int64_t)threads * items), B), dim3(threads),
-                        (size_t)(2 * G * sizeof(float)), ST, (const __half*)x, H, W, C, ksize, stride, upsample, stats_a, Ca, stats_b, G,
-                        eps, gamma, beta, act, (__half*)out, Ho, Wo, pad, items));
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

@@ -32,7 +32,7 @@ class Views(C.Structure):
 
 class Epilogue(C.Structure):
     _fields_ = [("bias", c_fp), ("residual", c_fp), ("rowbias", c_fp), ("rowbias_ld", c_i64), ("rows_per_group", C.c_int),
-                ("act", C.c_int), ("alpha", C.c_float), ("out_f32", C.c_int), ("colstats", c_fp), ("stats_rows_per_group", C.c_int)]
+                ("act", C.c_int), ("alpha", C.c_float), ("out_f32", C.c_int)]
 
 
 PTS_EXPLICIT, PTS_LATTICE, PTS_RAYS = 0, 1, 2
@@ -106,8 +106,6 @@ _SIGS = {
     "o2345_groupnorm_apply": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_float, c_fp, c_fp, C.c_int, c_fp, c_fp]),
     "o2345_norm_act_im2col": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, c_fp,
                                         C.c_int, c_fp, c_fp]),
-    "o2345_norm_act_im2col_stats": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, C.c_int,
-                                              c_fp, C.c_int, C.c_float, c_fp, c_fp, C.c_int, c_fp, c_fp]),
     "o2345_layernorm_rows": (C.c_int, [c_fp, c_i64, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp]),
     "o2345_softmax_rows": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp]),
     "o2345_attention_f16": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, c_fp, C.c_int,
@@ -130,7 +128,7 @@ _SIGS = {
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 6          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 7          # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 

@@ -39,30 +39,20 @@ def _splitk_ws(dev):
     return _WS[k]
 
 
-def _epilogue(bias=None, residual=None, rowbias=None, rows_per_group=1, act=0, alpha=1.0, out_f32=False, colstats=None):
-    """o2345_epilogue; the tensors must stay alive until the call returns (they are arguments of the caller).
-    colstats = (fp32 [groups, 2, N] zeroed table, rows per group): the GEMM adds the GroupNorm statistics of its output."""
+def _epilogue(bias=None, residual=None, rowbias=None, rows_per_group=1, act=0, alpha=1.0, out_f32=False):
+    """o2345_epilogue; the tensors must stay alive until the call returns (they are arguments of the caller)."""
     if rowbias is not None:
         assert rowbias.dtype == _f16 and rowbias.stride(-1) == 1
-    if colstats is not None:
-        assert colstats[0].dtype == _f32 and colstats[0].is_contiguous()
     return L.Epilogue(bias=_p(bias, _f32), residual=None if residual is None else residual.data_ptr(),
                       rowbias=None if rowbias is None else rowbias.data_ptr(),
                       rowbias_ld=0 if rowbias is None else rowbias.stride(0), rows_per_group=int(rows_per_group),
-                      act=int(act), alpha=float(alpha), out_f32=int(out_f32),
-                      colstats=None if colstats is None else colstats[0].data_ptr(),
-                      stats_rows_per_group=0 if colstats is None else int(colstats[1]))
-
-
-def stats_fusable(HW):
-    """Row groups (images of HW pixels) the GEMM epilogues can keep GroupNorm statistics for."""
-    return HW == 64 or HW % 128 == 0
+                      act=int(act), alpha=float(alpha), out_f32=int(out_f32))
 
 
 ACT_NONE, ACT_SILU, ACT_GELU, ACT_GEGLU, ACT_QUICKGELU = 0, 1, 2, 3, 4
 
 
-def gemm(a, b, bias=None, residual=None, act=0, alpha=1.0, out_dtype=_f16, out=None, rowbias=None, rows_per_group=1, colstats=None):
+def gemm(a, b, bias=None, residual=None, act=0, alpha=1.0, out_dtype=_f16, out=None, rowbias=None, rows_per_group=1):
     """out[M,N] = act(alpha * a[M,K] @ b[N,K]^T + bias + rowbias[row // rows_per_group]) + residual.  a, b fp16 with
     contiguous K; rows may be strided.  act = ACT_GEGLU: b's rows are interleaved 16 values / 16 gates (geglu_pack) and
     out has N/2 columns."""
@@ -75,7 +65,7 @@ def gemm(a, b, bias=None, residual=None, act=0, alpha=1.0, out_dtype=_f16, out=N
     assert out.stride(-1) == 1
     if residual is not None:
         assert residual.dtype == _f16 and residual.stride(0) == out.stride(0) and residual.stride(-1) == 1
-    ep = _epilogue(bias, residual, rowbias, rows_per_group, act, alpha, out.dtype == _f32, colstats)
+    ep = _epilogue(bias, residual, rowbias, rows_per_group, act, alpha, out.dtype == _f32)
     L.call("o2345_gemm_f16", _v(a), _v(b), _v(out), M, N, K, a.stride(0), b.stride(0), out.stride(0), 0, 0, 0, 0, 0, 0, 0, 0,
            C.byref(ep), _v(_splitk_ws(a.device)), WS_FLOATS, _stream())
     return out
@@ -137,21 +127,6 @@ def norm_act_im2col(x, B, H, W, C, ksize=3, stride=1, upsample=False, gn=None, a
     scale, shift = gn if gn is not None else (None, None)
     L.call("o2345_norm_act_im2col", _v(x), B, H, W, C, ksize, stride, int(upsample), int(pad_lo), _v(scale), _v(shift),
            int(act), _v(out), _stream())
-    return out, Ho, Wo
-
-
-def norm_act_im2col_stats(x, B, H, W, C, ksize, stride, upsample, stats_a, stats_b, G, eps, gamma, beta, act, pad_lo=-1):
-    """GroupNorm (+SiLU) + patch gather with the statistics taken from the producers' epilogue tables: stats_a [B, 2, Ca],
-    stats_b [B, 2, C - Ca] or None.  Returns ([B*Ho*Wo, k*k*C] fp16, Ho, Wo)."""
-    Hin, Win = (2 * H, 2 * W) if upsample else (H, W)
-    pad_hi = ksize // 2
-    pad = pad_hi if pad_lo < 0 else pad_lo
-    Ho, Wo = (Hin + pad + pad_hi - ksize) // stride + 1, (Win + pad + pad_hi - ksize) // stride + 1
-    out = torch.empty(B * Ho * Wo, ksize * ksize * C, dtype=_f16, device=x.device)
-    Ca = stats_a.shape[-1]
-    assert stats_a.shape == (B, 2, Ca) and (stats_b is None) == (Ca == C) and (stats_b is None or stats_b.shape == (B, 2, C - Ca))
-    L.call("o2345_norm_act_im2col_stats", _v(x), B, H, W, C, ksize, stride, int(upsample), int(pad_lo), _p(stats_a, _f32), Ca,
-           _p(stats_b, _f32), int(G), float(eps), _p(gamma, _f32), _p(beta, _f32), int(act), _v(out), _stream())
     return out, Ho, Wo
 
 
@@ -248,18 +223,18 @@ def conv_up2x(x, B, H, W, C, weight4, bias=None, act=0):
     N = weight4.shape[1]
     assert weight4.shape == (4, N, 4 * C) and weight4.dtype == _f16 and weight4.is_contiguous()
     out = torch.empty(B * 4 * H * W, N, dtype=_f16, device=x.device)
-    ep = _epilogue(bias, None, None, 1, act, 1.0, False, None)
+    ep = _epilogue(bias, None, None, 1, act, 1.0, False)
     L.call("o2345_conv_up2x_f16", _v(x), B, H, W, C, _v(weight4), N, _v(out), N, C_.byref(ep), _v(_splitk_ws(x.device)), WS_FLOATS, _stream())
     return out
 
 
-def conv3x3(x, B, H, W, C, weight, bias=None, residual=None, act=0, out_dtype=_f16, rowbias=None, colstats=None):
+def conv3x3(x, B, H, W, C, weight, bias=None, residual=None, act=0, out_dtype=_f16, rowbias=None):
     """Implicit-GEMM 3x3 convolution (stride 1, pad 1) of a channel-last activation x [B*H*W, C]; weight [N, 9*C] in
     (ky, kx, c) order.  No im2col buffer: TMA fetches the nine shifted windows, zero-filling outside the image.
     rowbias [B, >=N] fp16: per-image channel bias (the ResBlock's timestep embedding)."""
     N = weight.shape[0]
     out = torch.empty(B * H * W, N, dtype=out_dtype, device=x.device)
-    ep = _epilogue(bias, residual, rowbias, H * W, act, 1.0, out_dtype == _f32, colstats)
+    ep = _epilogue(bias, residual, rowbias, H * W, act, 1.0, out_dtype == _f32)
     L.call("o2345_conv3x3_f16", _v(x), B, H, W, C, _v(weight), N, _v(out), out.stride(0), C_.byref(ep),
            _v(_splitk_ws(x.device)), WS_FLOATS, _stream())
     return out

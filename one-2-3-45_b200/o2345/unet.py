@@ -9,10 +9,10 @@ signature and returns the epsilon prediction [N,4,H,W] in fp32 (values rounded t
 autocast would round them).
 
 Execution: activations are channel-last fp16 [N*H*W, C].  Every Linear / 1x1 conv is one wgmma GEMM and every
-3x3 stride-1 conv an implicit GEMM whose nine shifted windows are fetched by TMA (csrc/gemm_tc.cu: CTA-pair
-`cta_group::2` tiles, split-K for small grids); the strided / up-sampling convs gather patches first
-(csrc/unet_ops.cu).  GroupNorm is a per-(image, channel) affine computed by one statistics kernel and applied together
-with SiLU; the ResBlock's `h + emb`, the attention / feed-forward residuals, the GEGLU gate and the single-token
+3x3 stride-1 conv an implicit GEMM whose nine shifted windows are fetched by TMA (csrc/gemm_tc.cu: 128 x BN wgmma
+tiles, operand tiles multicast over a 2 x 2 CTA cluster, split-K for small grids); the strided / up-sampling convs
+gather patches first (csrc/unet_ops.cu).  GroupNorm (+SiLU) is one cluster kernel, or statistics kernel + apply for the
+large maps; the ResBlock's `h + emb`, the attention / feed-forward residuals, the GEGLU gate and the single-token
 cross-attention term ride in GEMM epilogues.  Self-attention is the fused mma.sync kernel (csrc/attention.cu; scores
 never leave the SM); the batched-GEMM -> softmax -> batched-GEMM route remains for other head sizes.
 Cross-attention: Zero123 conditions on ONE token, so softmax over a single key is exactly 1 and
@@ -212,13 +212,7 @@ class UNetModel(nn.Module):
         self.use_cuda_graph = True
         self._graphs = {}
         self._ctx_ref, self._ctx_ver, self._ctx_pk, self._cross_out = None, None, None, {}
-        # GroupNorm statistics tables filled by the producing GEMMs' epilogues (one arena, zeroed once per pass).  OFF by
-        # default: the epilogues' red.add.f32 hit each (image, channel) address from 32 row slabs, and the L2 atomic units
-        # serialise same-address updates, which can cost more than the 46 statistics kernels it removes (not measured on H100).
-        # Kept as a tested option (tests/test_gpu_gemm.py::test_epilogue_groupnorm_statistics_feed_the_next_norm).
-        self.fuse_gn_stats = False
         self.gn_one_kernel = True    # GroupNorm statistics + apply in one cluster kernel (o2345_groupnorm_apply)
-        self._arena, self._arena_off, self._arena_need = None, 0, 0
 
     # ------------------------------------------------------------------ executor
     def _pk(self):
@@ -227,66 +221,31 @@ class UNetModel(nn.Module):
             self._packed = _Packed(self)
         return self._packed
 
-    def _stats_table(self, B, N, HW, dev):
-        """A zeroed [B, 2, N] fp32 table (sum, sum of squares per image and channel) out of the per-pass arena, or None when the
-        producer cannot keep statistics for this shape / the arena is not sized yet (first pass: the consumers then compute
-        their statistics the round-1 way, from the tensor)."""
-        if not (self.fuse_gn_stats and A.stats_fusable(HW)):
-            return None
-        n, off = B * 2 * N, self._arena_off
-        self._arena_off += n
-        self._arena_need = max(self._arena_need, self._arena_off)
-        if self._arena is None or self._arena.device != dev or off + n > self._arena.numel():
-            return None
-        return self._arena[off:off + n].view(B, 2, N)
-
-    def _size_arena(self, dev):
-        """(Re)allocates the statistics arena for the largest pass seen so far.  Never called inside a stream capture;
-        arenas that captured graphs still point into are kept alive."""
-        if self.fuse_gn_stats and self._arena_need and (self._arena is None or self._arena.device != dev or
-                                                         self._arena.numel() < self._arena_need):
-            if self._arena is not None:
-                self._old_arenas = getattr(self, "_old_arenas", []) + [self._arena]
-            self._arena = torch.zeros(self._arena_need, dtype=_f32, device=dev)
-
-    def _begin_pass(self, dev):
-        if not torch.cuda.is_current_stream_capturing():
-            self._size_arena(dev)
-        self._arena_off = 0
-        if self._arena is not None and self.fuse_gn_stats:
-            self._arena.zero_()
-
-    def _norm(self, pk, x, B, H, W, C, gn, act, xs, ksize=1, stride=1, up=False):
-        """GroupNorm(x) (+SiLU) as the K-major A operand of the following GEMM: from the producers' statistics tables `xs` =
-        (table of the first Ca channels, table of the rest or None) when there are any, else statistics kernel + apply."""
-        if xs is not None:
-            ga, be = pk.norm(gn)
-            return A.norm_act_im2col_stats(x, B, H, W, C, ksize, stride, up, xs[0], xs[1], 32, gn.eps, ga, be, act)
+    def _norm(self, pk, x, B, H, W, C, gn, act, ksize=1, stride=1, up=False):
+        """GroupNorm(x) (+SiLU) as the K-major A operand of the following GEMM: one cluster kernel, or statistics kernel +
+        apply / patch gather."""
         if ksize == 1 and stride == 1 and not up and self.gn_one_kernel and A.groupnorm_apply_pays(B, H * W, C):
             return A.groupnorm_apply(x, B, H * W, C, 32, gn.eps, *pk.norm(gn), act), H, W
         g = A.groupnorm_stats(x, B, H * W, C, 32, gn.eps, *pk.norm(gn))
         return A.norm_act_im2col(x, B, H, W, C, ksize, stride, up, g, act)
 
-    def _conv3(self, pk, x, B, H, W, C, conv, gn=None, act=False, stride=1, up=False, residual=None, rowbias=None, xs=None,
-               want_stats=True):
-        """3x3 conv (optionally behind GroupNorm + SiLU).  -> (out, Ho, Wo, statistics table of `out` or None)."""
+    def _conv3(self, pk, x, B, H, W, C, conv, gn=None, act=False, stride=1, up=False, residual=None, rowbias=None):
+        """3x3 conv (optionally behind GroupNorm + SiLU).  -> (out, Ho, Wo)."""
         w, b = pk.conv(conv)
         Ho, Wo = ((2 * H, 2 * W) if up else ((H + 2 - 3) // stride + 1, (W + 2 - 3) // stride + 1))
-        cs = self._stats_table(B, w.shape[0], Ho * Wo, x.device) if want_stats else None
-        colstats = None if cs is None else (cs, Ho * Wo)
         if stride == 1 and not up and A.conv3x3_supported(H, W, C):
             # implicit GEMM: normalise once ([M, C], not 9x) and let TMA fetch the nine shifted windows
-            a = x if gn is None else self._norm(pk, x, B, H, W, C, gn, act, xs)[0]
-            return A.conv3x3(a, B, H, W, C, w, bias=b, residual=residual, rowbias=rowbias, colstats=colstats), H, W, cs
-        if A.USE_CONV_UP2X and up and stride == 1 and gn is None and cs is None and residual is None and rowbias is None and A.conv3x3_supported(H, W, C):
+            a = x if gn is None else self._norm(pk, x, B, H, W, C, gn, act)[0]
+            return A.conv3x3(a, B, H, W, C, w, bias=b, residual=residual, rowbias=rowbias), H, W
+        if A.USE_CONV_UP2X and up and stride == 1 and gn is None and residual is None and rowbias is None and A.conv3x3_supported(H, W, C):
             # nearest 2x + 3x3 conv = four 2x2 convs of the low-resolution map (no [M, 9C] gather, 4C instead of 9C per output)
             w4, b4 = pk.conv_up(conv)
-            return A.conv_up2x(x, B, H, W, C, w4, bias=b4), Ho, Wo, None
+            return A.conv_up2x(x, B, H, W, C, w4, bias=b4), Ho, Wo
         if gn is None:
             a, Ho, Wo = A.norm_act_im2col(x, B, H, W, C, 3, stride, up, None, act)
         else:
-            a, Ho, Wo = self._norm(pk, x, B, H, W, C, gn, act, xs, 3, stride, up)
-        return A.gemm(a, w, bias=b, residual=residual, rowbias=rowbias, rows_per_group=Ho * Wo, colstats=colstats), Ho, Wo, cs
+            a, Ho, Wo = self._norm(pk, x, B, H, W, C, gn, act, 3, stride, up)
+        return A.gemm(a, w, bias=b, residual=residual, rowbias=rowbias, rows_per_group=Ho * Wo), Ho, Wo
 
     def _emb_pack(self, pk):
         """All 22 ResBlock `emb_layers` Linears as ONE [sum Cout, 1280] GEMM per iteration (they share the input)."""
@@ -301,20 +260,18 @@ class UNetModel(nn.Module):
             pk.w["emb_all"] = (torch.cat(ws, 0).contiguous(), torch.cat(bs, 0).contiguous(), off)
         return pk.w["emb_all"]
 
-    def _resblock(self, pk, blk, x, B, H, W, emb_all, xs):
+    def _resblock(self, pk, blk, x, B, H, W, emb_all):
         C, Co = blk.channels, blk.out_channels
         off = self._emb_pack(pk)[2][id(blk)]
         # h + emb_out[..., None, None] (openaimodel.py:271) rides in the conv epilogue as a per-image channel bias
-        h, _, _, hs = self._conv3(pk, x, B, H, W, C, blk.in_layers[2], gn=blk.in_layers[0], act=True,
-                                  rowbias=emb_all[:, off:off + Co], xs=xs)
+        h, _, _ = self._conv3(pk, x, B, H, W, C, blk.in_layers[2], gn=blk.in_layers[0], act=True, rowbias=emb_all[:, off:off + Co])
         if isinstance(blk.skip_connection, nn.Identity):
             skip = x
         else:
             ws, bs = pk.conv(blk.skip_connection)
             skip = A.gemm(x, ws, bias=bs)
-        out, _, _, os_ = self._conv3(pk, h, B, H, W, Co, blk.out_layers[3], gn=blk.out_layers[0], act=True, residual=skip,
-                                     xs=None if hs is None else (hs, None))
-        return out, Co, os_
+        out, _, _ = self._conv3(pk, h, B, H, W, Co, blk.out_layers[3], gn=blk.out_layers[0], act=True, residual=skip)
+        return out, Co
 
     def _attention(self, pk, attn, xn, B, N, C, residual, rowbias=None):
         """Self-attention on layer-normed tokens xn [B*N, C]; returns to_out(...) + residual (+ rowbias[image])."""
@@ -377,9 +334,9 @@ class UNetModel(nn.Module):
         A.bgemm(pp, vt, o, H, B, (N * Tp, H * N * Tp), (d * Tp, C * Tp), (d, N * C), N, d, Tp, Tp, Tp, C)
         return A.gemm(o, wo, bias=bo, residual=h)
 
-    def _transformer(self, pk, st, x, B, H, W, C, ctx16, xs):
+    def _transformer(self, pk, st, x, B, H, W, C, ctx16):
         N = H * W
-        a, _, _ = self._norm(pk, x, B, H, W, C, st.norm, False, xs)
+        a, _, _ = self._norm(pk, x, B, H, W, C, st.norm, False)
         wi, bi = pk.conv(st.proj_in)
         h = A.gemm(a, wi, bias=bi)
         blk = st.transformer_blocks[0]
@@ -396,28 +353,24 @@ class UNetModel(nn.Module):
         gg = A.gemm(A.layernorm(h, *pk.norm(blk.norm3), eps=blk.norm3.eps), w1, bias=b1, act=A.ACT_GEGLU)
         h = A.gemm(gg, w2, bias=b2, residual=h)
         wo, bo = pk.conv(st.proj_out)
-        cs = self._stats_table(B, wo.shape[0], N, x.device)
-        return A.gemm(h, wo, bias=bo, residual=x, colstats=None if cs is None else (cs, N)), cs
+        return A.gemm(h, wo, bias=bo, residual=x)
 
-    def _run_block(self, pk, seq, x, B, H, W, C, emb_act, ctx16, xs):
-        """xs: statistics tables of x (see _norm) or None.  -> (x, H, W, C, statistics table of x or None)."""
-        st = None
+    def _run_block(self, pk, seq, x, B, H, W, C, emb_act, ctx16):
         for layer in seq:
             if isinstance(layer, ResBlock):
-                x, C, st = self._resblock(pk, layer, x, B, H, W, emb_act, xs)
+                x, C = self._resblock(pk, layer, x, B, H, W, emb_act)
             elif isinstance(layer, SpatialTransformer):
-                x, st = self._transformer(pk, layer, x, B, H, W, C, ctx16, xs)
+                x = self._transformer(pk, layer, x, B, H, W, C, ctx16)
             elif isinstance(layer, Downsample):
-                x, H, W, st = self._conv3(pk, x, B, H, W, C, layer.op, stride=2)
+                x, H, W = self._conv3(pk, x, B, H, W, C, layer.op, stride=2)
             elif isinstance(layer, Upsample):
-                x, H, W, st = self._conv3(pk, x, B, H, W, C, layer.conv, up=True)
+                x, H, W = self._conv3(pk, x, B, H, W, C, layer.conv, up=True)
             elif isinstance(layer, nn.Conv2d):
-                x, H, W, st = self._conv3(pk, x, B, H, W, C, layer)
+                x, H, W = self._conv3(pk, x, B, H, W, C, layer)
                 C = layer.out_channels
             else:
                 raise TypeError(type(layer))
-            xs = None if st is None else (st, None)
-        return x, H, W, C, st
+        return x, H, W, C
 
     @inference_only
     def forward(self, x, timesteps=None, context=None, y=None, **kwargs):
@@ -433,8 +386,7 @@ class UNetModel(nn.Module):
         g = self._graphs.get(key)
         if g is None:
             sx, st, sc = x.detach().float().clone(), timesteps.detach().clone(), context.detach().float().clone()
-            self._forward_impl(sx, st, sc)                       # warm-up: packs weights, sets kernel attributes, sizes the statistics arena
-            self._size_arena(x.device)
+            self._forward_impl(sx, st, sc)                       # warm-up: packs weights, sets kernel attributes
             torch.cuda.synchronize()
             graph = torch.cuda.CUDAGraph()
             n0 = _lib.launches()
@@ -452,7 +404,6 @@ class UNetModel(nn.Module):
     @torch.no_grad()
     def _forward_impl(self, x, timesteps, context):
         pk = self._pk()
-        self._begin_pass(x.device)
         B, Cin, H, W = x.shape
         C = (Cin + 7) // 8 * 8
         h = A.nchw_to_cl(x, torch.zeros(B * H * W, C, dtype=_f16, device=x.device))
@@ -463,18 +414,16 @@ class UNetModel(nn.Module):
         wa, ba, _ = self._emb_pack(pk)
         emb_act = A.gemm(A.silu(emb), wa, bias=ba)                          # [B, sum Cout]: emb_layers of every ResBlock
         ctx16 = context.reshape(-1, context.shape[-1]).to(_f16).contiguous()
-        hs, st = [], None
+        hs = []
         for seq in self.input_blocks:
-            h, H, W, C, st = self._run_block(pk, seq, h, B, H, W, C, emb_act, ctx16, None if st is None else (st, None))
-            hs.append((h, C, st))
-        h, H, W, C, st = self._run_block(pk, self.middle_block, h, B, H, W, C, emb_act, ctx16, None if st is None else (st, None))
+            h, H, W, C = self._run_block(pk, seq, h, B, H, W, C, emb_act, ctx16)
+            hs.append((h, C))
+        h, H, W, C = self._run_block(pk, self.middle_block, h, B, H, W, C, emb_act, ctx16)
         for seq in self.output_blocks:
-            skip, Cs, sst = hs.pop()
+            skip, Cs = hs.pop()
             cat = torch.empty(B * H * W, C + Cs, dtype=_f16, device=h.device)
             A.copy_channels(h, cat, 0)
             A.copy_channels(skip, cat, C)
-            xs = None if (st is None or sst is None) else (st, sst)        # GroupNorm over the concat: one table per part
-            h, H, W, C, st = self._run_block(pk, seq, cat, B, H, W, C + Cs, emb_act, ctx16, xs)
-        out, _, _, _ = self._conv3(pk, h, B, H, W, C, self.out[2], gn=self.out[0], act=True, xs=None if st is None else (st, None),
-                                   want_stats=False)
+            h, H, W, C = self._run_block(pk, seq, cat, B, H, W, C + Cs, emb_act, ctx16)
+        out, _, _ = self._conv3(pk, h, B, H, W, C, self.out[2], gn=self.out[0], act=True)
         return A.cl_to_nchw(out, B, self.out_channels, H, W)

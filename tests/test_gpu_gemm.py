@@ -161,50 +161,6 @@ def test_groupnorm_affine_matches_torch(B, HW, C):
         assert (y1.float() - y.float()).abs().max().item() < 4e-3      # fp16 rounding of values up to ~8: one ulp either way
 
 
-@pytest.mark.parametrize("B,H,W,C,N,split", [(8, 32, 32, 320, 320, 0), (8, 16, 16, 640, 640, 0), (8, 8, 8, 1280, 1280, 0), (4, 16, 16, 640, 320, 3),
-                                             (8, 8, 8, 1280, 1280, 6), (2, 16, 16, 64, 96, 0)])
-def test_epilogue_groupnorm_statistics_feed_the_next_norm(B, H, W, C, N, split):
-    """The GEMM / conv epilogue adds per-(image, channel) sum and sum of squares of the fp16 tensor it writes (staged epilogue and
-    split-K finalize); norm_act_im2col_stats turns the tables -- two of them for a channel concat -- into GroupNorm + SiLU.
-    Against torch.group_norm on the same fp16 tensors."""
-    import ctypes as C_
-    from o2345 import _lib as L, ops_a
-    g = torch.Generator(device="cuda").manual_seed(B * 100 + C + split)
-    HW = H * W
-    x = (torch.randn(B, H, W, C, device="cuda", generator=g) * 0.5).half()
-    w = (torch.randn(N, C, 3, 3, device="cuda", generator=g) * (2.0 / (9 * C)) ** 0.5).half()
-    wk = w.permute(0, 2, 3, 1).reshape(N, 9 * C).contiguous()
-    bias = torch.randn(N, device="cuda", generator=g)
-    res = torch.randn(B * HW, N, device="cuda", generator=g).half()
-    stats = torch.zeros(B, 2, N, device="cuda")
-    lib = L.load()
-    lib.o2345_debug_gemm_force(0, 0, split)
-    try:
-        y = ops_a.conv3x3(x.view(-1, C), B, H, W, C, wk, bias=bias, residual=res, colstats=(stats, HW))
-    finally:
-        lib.o2345_debug_gemm_force(0, 0, 0)
-    yf = y.float().view(B, HW, N)
-    assert float((stats[:, 0] - yf.sum(1)).abs().max()) < 2e-3 * HW ** 0.5 + 1e-3 * float(yf.sum(1).abs().max())
-    assert float((stats[:, 1] - (yf * yf).sum(1)).abs().max()) < 1e-3 * float((yf * yf).sum(1).abs().max())
-    # consumer: GroupNorm(32) + SiLU of cat[y, z] with one table per part (z's table from a plain GEMM epilogue)
-    Cz = 2 * N if N % 64 == 0 else N
-    az = (torch.randn(B * HW, 64, device="cuda", generator=g) * 0.5).half()
-    wz = (torch.randn(Cz, 64, device="cuda", generator=g) * 0.2).half()
-    stats_z = torch.zeros(B, 2, Cz, device="cuda")
-    z = ops_a.gemm(az, wz, colstats=(stats_z, HW))
-    cat = torch.cat([y, z], 1).contiguous()
-    Ct = N + Cz
-    gamma, beta = torch.randn(Ct, device="cuda", generator=g), torch.randn(Ct, device="cuda", generator=g)
-    got, _, _ = ops_a.norm_act_im2col_stats(cat, B, H, W, Ct, 1, 1, False, stats, stats_z, 32, 1e-5, gamma, beta, True)
-    want = torch.nn.functional.silu(torch.nn.functional.group_norm(cat.float().view(B, HW, Ct).permute(0, 2, 1), 32, gamma, beta, 1e-5))
-    assert float((got.float().view(B, HW, Ct) - want.permute(0, 2, 1)).abs().max()) < 2e-2
-    # single table, 3x3 stride-2 gather (the Downsample path)
-    got3, Ho, Wo = ops_a.norm_act_im2col_stats(y, B, H, W, N, 3, 2, False, stats, None, 32, 1e-5, gamma[:N], beta[:N], True)
-    sc, sh = ops_a.groupnorm_stats(y, B, HW, N, 32, 1e-5, gamma[:N], beta[:N])
-    want3, _, _ = ops_a.norm_act_im2col(y, B, H, W, N, 3, 2, False, (sc, sh), True)
-    assert (Ho, Wo) == (H // 2, W // 2) and float((got3.float() - want3.float()).abs().max()) < 2e-2
-
-
 @pytest.fixture
 def persistent_everywhere():
     """Forces the persistent launch of the GEMM kernel wherever it is available (staged fp16 epilogue, no split-K), whatever

@@ -13,7 +13,6 @@ from o2345.unet import UNetModel
 lib = L.load()
 net = UNetModel().cuda().requires_grad_(False)
 net.use_cuda_graph = False
-net.fuse_gn_stats = False
 BATCH = int(os.environ.get("UNET_BATCH", "8"))
 x = torch.randn(BATCH, 8, 32, 32, device="cuda"); t = torch.full((BATCH,), 501, device="cuda"); ctx = torch.randn(BATCH, 1, 768, device="cuda")
 net(x, t, ctx); torch.cuda.synchronize()
