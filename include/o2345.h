@@ -32,13 +32,14 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 7   /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 8  /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
                                  6: rays of many cameras in one launch: render_blend dir_mode 2, o2345_ray_midpoints_per_ray
                                  7: the GEMM epilogue's GroupNorm column statistics are gone: o2345_epilogue lost its last two fields,
-                                    and the norm + patch gather entry point that read the tables went with them */
+                                    and the norm + patch gather entry point that read the tables went with them
+                                 8: the mesh rasterizer: o2345_raster, o2345_raster_scratch_bytes, o2345_debug_raster_split */
 
 typedef void* o2345_stream_t;
 
@@ -443,6 +444,51 @@ int o2345_clip_patches(const float* x, int B, int H, int W, int res, int patch, 
                        void* out, o2345_stream_t stream);
 /* tok [B*N, d] fp16: row 0 of every image := class_embedding + pos[0]; rows n >= 1 += pos[n] (cls, pos fp32 on the device) */
 int o2345_clip_add_positions(void* tok, const float* cls, const float* pos, int B, int N, int d, o2345_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Mesh rasterizer (render_eval.py): V views of one triangle mesh, one sample at every pixel centre, bit-reproducible.
+ * Stands in for the reference's Blender / BlenderProc evaluation renderer (render/single_render_eval.py) for geometry,
+ * silhouette and depth; colour is the defined model below, not Cycles.  oracle/raster_oracle.py restates every rule.
+ *   vertices   camera space c = R p + t (OpenCV: x right, y down, z forward), pixel x = fx * c.x / c.z + cx (y alike),
+ *              snapped to fixed point with 8 subpixel bits (round to nearest even); every float op rounded to nearest in
+ *              the order of csrc/raster.cu, without FMA contraction;
+ *   triangles  int64 edge functions, top-left fill rule, pixel (i, j) sampled at (i + 0.5, j + 0.5); no back-face culling.
+ *              Dropped: zero screen area, any vertex at camera z <= near, any vertex projecting 2^21 pixels or more
+ *              from the image origin;
+ *   depth      perspective-correct camera z; per pixel the smallest (z bits << 32 | triangle id) wins, so equal depths go
+ *              to the lower id and the result does not depend on execution order.
+ * ------------------------------------------------------------------------------------------ */
+typedef struct o2345_raster_mesh {
+  const float* verts;      /* [nv,3] world positions                                                               */
+  const float* colors;     /* [nv,3] base colour per vertex, or NULL (white)                                       */
+  const float* uvs;        /* [nv,2] texture coordinates (glTF: origin at the image's top-left), or NULL           */
+  const int32_t* faces;    /* [nf,3] vertex indices; a face with an index outside [0, nv) is dropped               */
+  const int32_t* face_tex; /* [nf] texture of each face (-1 or >= n_tex: none), or NULL                            */
+  const uint8_t* texels;   /* RGBA8 texels of every texture, row-major, packed one after another                    */
+  const int32_t* tex_info; /* [n_tex,5]: first texel, width, height, wrap s, wrap t (O2345_WRAP_*)                  */
+  int64_t nv, nf;
+  int n_tex;
+} o2345_raster_mesh;
+
+#define O2345_WRAP_REPEAT 0
+#define O2345_WRAP_CLAMP 1
+#define O2345_WRAP_MIRROR 2
+#define O2345_SHADE_UNLIT 0    /* colour = base colour as stored                                                     */
+#define O2345_SHADE_LAMBERT 1  /* colour = base colour * (0.4 + 0.6 * max(n.z, 0)), n the camera-facing world normal */
+
+/* Bytes of scratch o2345_raster needs (-1 for negative sizes). */
+int64_t o2345_raster_scratch_bytes(int64_t nv, int64_t nf, int V, int W, int H);
+/* w2c [V,3,4] (row-major [R | t]), intr [V,4] = (fx, fy, cx, cy).  Outputs (any may be NULL), pixel (v, j, i) at
+ * index (v * H + j) * W + i: color [.,3] (perspective-correct vertex colour times the bilinear texture sample of the
+ * face's texture, then the shading term), alpha (1 covered, 0 background), depth (camera z, 0 background), normal [.,3]
+ * (unit world-space face normal turned toward the camera centre), tri (face index, -1 background).  Background pixels
+ * are all zero. */
+int o2345_raster(const o2345_raster_mesh* mesh, int V, const float* w2c, const float* intr, int W, int H, float near,
+                 int shading, void* scratch, int64_t scratch_bytes, float* color, float* alpha, float* depth,
+                 float* normal, int32_t* tri, o2345_stream_t stream);
+/* Tuning hook (tools/time_raster.py): triangles whose clipped bounding box holds more than `pixels` pixel centres are
+ * walked by a warp instead of one thread; 0 restores the default (64). */
+void o2345_debug_raster_split(int pixels);
 
 #ifdef __cplusplus
 }

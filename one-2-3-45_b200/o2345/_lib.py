@@ -35,12 +35,19 @@ class Epilogue(C.Structure):
                 ("act", C.c_int), ("alpha", C.c_float), ("out_f32", C.c_int)]
 
 
+class RasterMesh(C.Structure):
+    _fields_ = [("verts", c_fp), ("colors", c_fp), ("uvs", c_fp), ("faces", c_fp), ("face_tex", c_fp), ("texels", c_fp),
+                ("tex_info", c_fp), ("nv", c_i64), ("nf", c_i64), ("n_tex", C.c_int)]
+
+
 PTS_EXPLICIT, PTS_LATTICE, PTS_RAYS = 0, 1, 2
 BLEND_FP32, BLEND_TC_FP16 = 0, 1
 SDF_FP32, SDF_TC_SPLIT = 0, 1
 SDF_PACK_FLOATS = 39 * 128 + 128 + 2 * (144 * 128 + 128) + 128 * 144 + 128 * 48
 RNET_PACK_FLOATS = 19664
 MAP_CH = 60
+SHADE_UNLIT, SHADE_LAMBERT = 0, 1
+WRAP_REPEAT, WRAP_CLAMP, WRAP_MIRROR = 0, 1, 2
 
 _SIGS = {
     "o2345_abi_version": (C.c_int, []),
@@ -123,12 +130,16 @@ _SIGS = {
     "o2345_clip_patches": (C.c_int, [c_fp, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_float), C.POINTER(C.c_float),
                                      C.c_int, c_fp, c_fp]),
     "o2345_clip_add_positions": (C.c_int, [c_fp, c_fp, c_fp, C.c_int, C.c_int, C.c_int, c_fp]),
+    "o2345_raster_scratch_bytes": (c_i64, [c_i64, c_i64, C.c_int, C.c_int, C.c_int]),
+    "o2345_raster": (C.c_int, [C.POINTER(RasterMesh), C.c_int, c_fp, c_fp, C.c_int, C.c_int, C.c_float, C.c_int, c_fp, c_i64,
+                               c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
+    "o2345_debug_raster_split": (None, [C.c_int]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 7          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 8          # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 
@@ -167,7 +178,7 @@ def last_error() -> str:
 
 
 # kernels launched per successful entry-point call (memsets are not counted)
-_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4}
+_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4}
 _launches = 0
 
 

@@ -162,3 +162,176 @@ def convert_mesh_format(exp_dir, output_format=".obj"):
     else:
         write_glb(out, v2, f2, c)
     return out
+
+
+# ----------------------------------------------------------------------------- readers of the evaluation renderer
+# (o2345/mesh_raster.py).  Each returns the file's own axes; the Blender import conventions live in mesh_raster.
+
+def read_obj(path):
+    """Wavefront OBJ: `v x y z [r g b]` vertices (trimesh's and write_obj's vertex colours) and `f` polygons (`a`, `a/b`,
+    `a/b/c`, `a//c`, negative indices), fan-triangulated.  -> (vertices float64 [n,3], triangles int64 [m,3], colors float64
+    [n,3] in [0, 1] or None when no vertex carries a colour).  Texture coordinates and materials are ignored."""
+    verts, cols, faces = [], [], []
+    with open(path, "r", errors="replace") as fh:
+        for line in fh:
+            if line.startswith("v "):
+                q = line.split()
+                verts.append([float(x) for x in q[1:4]])
+                cols.append([float(x) for x in q[4:7]] if len(q) >= 7 else None)
+            elif line.startswith("f "):
+                idx = []
+                for tok in line.split()[1:]:
+                    i = int(tok.split("/")[0])
+                    idx.append(i - 1 if i > 0 else len(verts) + i)
+                faces.extend([idx[0], idx[k], idx[k + 1]] for k in range(1, len(idx) - 1))
+    v = np.asarray(verts, np.float64).reshape(-1, 3)
+    f = np.asarray(faces, np.int64).reshape(-1, 3)
+    if len(f) and (f.min() < 0 or f.max() >= len(v)):
+        raise ValueError(f"{path}: a face refers to a vertex that does not exist")
+    has = [c is not None for c in cols]
+    c = None
+    if any(has):
+        c = np.ones((len(v), 3), np.float64)
+        for i, ci in enumerate(cols):
+            if ci is not None:
+                c[i] = ci
+    return v, f, c
+
+
+_GLTF_TYPES = {5120: np.int8, 5121: np.uint8, 5122: np.int16, 5123: np.uint16, 5125: np.uint32, 5126: np.float32}
+_GLTF_WIDTH = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4, "MAT4": 16}
+
+
+def _glb_accessor(doc, binary, i):
+    a = doc["accessors"][i]
+    if "sparse" in a or "bufferView" not in a:
+        raise ValueError("glTF: sparse accessors and accessors without a bufferView are not supported")
+    bv = doc["bufferViews"][a["bufferView"]]
+    if bv.get("buffer", 0) != 0:
+        raise ValueError("glTF: only the GLB's own binary chunk is supported as a buffer")
+    dt = np.dtype(_GLTF_TYPES[a["componentType"]]).newbyteorder("<")
+    width, count = _GLTF_WIDTH[a["type"]], a["count"]
+    start = bv.get("byteOffset", 0) + a.get("byteOffset", 0)
+    stride = bv.get("byteStride") or width * dt.itemsize
+    rows = np.ndarray((count, width), dt, buffer=binary, offset=start, strides=(stride, dt.itemsize))
+    out = rows.astype(np.float64) if dt.kind == "f" else rows.astype(np.int64)
+    if a.get("normalized"):
+        info = np.iinfo(dt)
+        out = np.maximum(out / info.max, -1.0)
+    return out
+
+
+def _gltf_node_matrix(n):
+    if "matrix" in n:
+        return np.asarray(n["matrix"], np.float64).reshape(4, 4).T     # column-major
+    x, y, z, w = n.get("rotation", [0.0, 0.0, 0.0, 1.0])
+    R = np.array([[1 - 2 * (y * y + z * z), 2 * (x * y - z * w), 2 * (x * z + y * w)],
+                  [2 * (x * y + z * w), 1 - 2 * (x * x + z * z), 2 * (y * z - x * w)],
+                  [2 * (x * z - y * w), 2 * (y * z + x * w), 1 - 2 * (x * x + y * y)]], np.float64)
+    M = np.eye(4)
+    M[:3, :3] = R * np.asarray(n.get("scale", [1.0, 1.0, 1.0]), np.float64)[None, :]
+    M[:3, 3] = n.get("translation", [0.0, 0.0, 0.0])
+    return M
+
+
+_GLTF_WRAP = {10497: 0, 33071: 1, 33648: 2}     # REPEAT, CLAMP_TO_EDGE, MIRRORED_REPEAT -> O2345_WRAP_*
+
+
+def read_glb(path):
+    """Binary glTF 2.0 -> dict:
+      roots     [4x4] world matrix of every root node of the default scene that has a mesh below it;
+      meshes    one entry per node with a mesh: verts [n,3], faces [m,3] (every indexed or non-indexed triangle primitive of
+                the mesh, joined), colors [n,3] (COLOR_0 times the material's baseColorFactor, white without either), uvs
+                [n,2] (TEXCOORD_0, or None), face_tex [m] (texture of the material's baseColorTexture, -1 without), root
+                (index into roots), local_to_root [4x4] (product of the node matrices below the root's own);
+      textures  [(RGBA uint8 [h,w,4], wrap s, wrap t)] decoded with PIL.
+    All in glTF's own (Y-up) axes.  Primitives that are not triangle lists, alpha modes, normal / occlusion /
+    metallic-roughness textures and texture transforms are ignored; a texture is sampled at TEXCOORD_0."""
+    import io
+    raw = open(path, "rb").read()
+    magic, version, _ = struct.unpack_from("<III", raw, 0)
+    if magic != 0x46546C67 or version != 2:
+        raise ValueError(f"{path}: not a binary glTF 2.0 file")
+    jlen, jtype = struct.unpack_from("<II", raw, 12)
+    if jtype != 0x4E4F534A:
+        raise ValueError(f"{path}: the first GLB chunk is not JSON")
+    doc = json.loads(raw[20:20 + jlen].decode("utf-8"))
+    binary = b""
+    off = 20 + jlen
+    if off + 8 <= len(raw):
+        blen, btype = struct.unpack_from("<II", raw, off)
+        if btype == 0x004E4942:
+            binary = raw[off + 8:off + 8 + blen]
+
+    textures, tex_of_image = [], {}
+
+    def texture(ti):
+        t = doc["textures"][ti]
+        src = t.get("source")
+        if src is None:
+            return -1
+        samp = doc.get("samplers", [{}])[t["sampler"]] if "sampler" in t else {}
+        key = (src, samp.get("wrapS", 10497), samp.get("wrapT", 10497))
+        if key not in tex_of_image:
+            from PIL import Image
+            img = doc["images"][src]
+            if "bufferView" not in img:
+                raise ValueError(f"{path}: image {src} is not embedded in the GLB")
+            bv = doc["bufferViews"][img["bufferView"]]
+            data = binary[bv.get("byteOffset", 0):bv.get("byteOffset", 0) + bv["byteLength"]]
+            rgba = np.asarray(Image.open(io.BytesIO(data)).convert("RGBA"), np.uint8)
+            tex_of_image[key] = len(textures)
+            textures.append((rgba, _GLTF_WRAP.get(key[1], 0), _GLTF_WRAP.get(key[2], 0)))
+        return tex_of_image[key]
+
+    def mesh(mi):
+        vs, fs, cs, us, ts, n = [], [], [], [], [], 0
+        for prim in doc["meshes"][mi]["primitives"]:
+            if prim.get("mode", 4) != 4:
+                continue
+            att = prim["attributes"]
+            v = _glb_accessor(doc, binary, att["POSITION"])
+            f = (_glb_accessor(doc, binary, prim["indices"]).reshape(-1, 3) if "indices" in prim
+                 else np.arange(len(v) - len(v) % 3, dtype=np.int64).reshape(-1, 3))
+            mat = doc["materials"][prim["material"]] if "material" in prim else {}
+            pbr = mat.get("pbrMetallicRoughness", {})
+            c = np.ones((len(v), 3))
+            if "COLOR_0" in att:
+                c = _glb_accessor(doc, binary, att["COLOR_0"])[:, :3].astype(np.float64)
+            c = c * np.asarray(pbr.get("baseColorFactor", [1.0, 1.0, 1.0, 1.0])[:3], np.float64)
+            tex = texture(pbr["baseColorTexture"]["index"]) if "baseColorTexture" in pbr and "TEXCOORD_0" in att else -1
+            vs.append(v[:, :3])
+            fs.append(f + n)
+            cs.append(c)
+            us.append(_glb_accessor(doc, binary, att["TEXCOORD_0"]) if "TEXCOORD_0" in att else np.zeros((len(v), 2)))
+            ts.append(np.full(len(f), tex, np.int64))
+            n += len(v)
+        if not vs:
+            return None
+        has_uv = any("TEXCOORD_0" in p["attributes"] for p in doc["meshes"][mi]["primitives"])
+        return {"verts": np.concatenate(vs), "faces": np.concatenate(fs), "colors": np.concatenate(cs),
+                "uvs": np.concatenate(us) if has_uv else None, "face_tex": np.concatenate(ts)}
+
+    roots, meshes = [], []
+
+    def walk(ni, root, rel):
+        node = doc["nodes"][ni]
+        if "mesh" in node:
+            m = mesh(node["mesh"])
+            if m is not None:
+                m.update(root=root, local_to_root=rel)
+                meshes.append(m)
+        for ch in node.get("children", []):
+            walk(ch, root, rel @ _gltf_node_matrix(doc["nodes"][ch]))
+
+    if "scenes" in doc:
+        top = doc["scenes"][doc.get("scene", 0)].get("nodes", [])
+    else:   # no scene: every node that is nobody's child
+        kids = {c for n in doc.get("nodes", []) for c in n.get("children", [])}
+        top = [i for i in range(len(doc.get("nodes", []))) if i not in kids]
+    for ni in top:
+        before = len(meshes)
+        walk(ni, len(roots), np.eye(4))
+        if len(meshes) > before:
+            roots.append(_gltf_node_matrix(doc["nodes"][ni]))
+    return {"roots": roots, "meshes": meshes, "textures": textures}

@@ -413,3 +413,36 @@ def ray_composite(rays_d, mid, dists, sdf, grad, color, active, nvalid, inv_s, r
            float(background if has_bg else 0.0), _f(out["color"]), _f(out["depth"]), _f(out["weights"]),
            _f(out["cdf"]), _f(out["alpha"]), _f(out["weights_sum"]), _p(out["color_mask"], _u8), _stream())
     return out
+
+
+# ----------------------------------------------------------------------------- mesh rasterizer
+def raster(verts, faces, w2c, intr, W, H, near=0.1, shading=L.SHADE_UNLIT, colors=None, uvs=None, face_tex=None, texels=None,
+           tex_info=None):
+    """V views of one triangle mesh (csrc/raster.cu): verts [nv,3] world, faces [nf,3] int32, w2c [V,3,4] OpenCV, intr
+    [V,4] = (fx, fy, cx, cy); optional colors [nv,3], uvs [nv,2] with face_tex [nf] int32, texels RGBA8 uint8 and tex_info
+    [n_tex,5] int32.  Returns device tensors color [V,H,W,3], alpha [V,H,W], depth [V,H,W], normal [V,H,W,3], tri [V,H,W]
+    int32 (-1 background)."""
+    verts, w2c, intr = cf32(verts).view(-1, 3), cf32(w2c).view(-1, 3, 4), cf32(intr).view(-1, 4)
+    faces = faces.contiguous().view(-1, 3)
+    V, nv, nf, dev = w2c.shape[0], verts.shape[0], faces.shape[0], verts.device
+    if intr.shape[0] != V:
+        raise ValueError(f"{V} w2c matrices but {intr.shape[0]} intrinsics")
+    colors = None if colors is None else cf32(colors).view(-1, 3)
+    uvs = None if uvs is None else cf32(uvs).view(-1, 2)
+    for name, t, rows in (("colors", colors, nv), ("uvs", uvs, nv), ("face_tex", face_tex, nf)):
+        if t is not None and t.shape[0] != rows:
+            raise ValueError(f"{name} has {t.shape[0]} rows, expected {rows}")
+    mesh = L.RasterMesh(verts=_f(verts).value, colors=_f(colors).value if colors is not None else None,
+                        uvs=_f(uvs).value if uvs is not None else None, faces=_p(faces, _i32).value,
+                        face_tex=_p(face_tex, _i32).value if face_tex is not None else None,
+                        texels=_p(texels, _u8).value if texels is not None else None,
+                        tex_info=_p(tex_info, _i32).value if tex_info is not None else None,
+                        nv=nv, nf=nf, n_tex=0 if tex_info is None else tex_info.shape[0])
+    nbytes = L.load().o2345_raster_scratch_bytes(nv, nf, V, W, H)
+    scratch = torch.empty(nbytes, dtype=_u8, device=dev)
+    out = {"color": torch.empty(V, H, W, 3, dtype=_f32, device=dev), "alpha": torch.empty(V, H, W, dtype=_f32, device=dev),
+           "depth": torch.empty(V, H, W, dtype=_f32, device=dev), "normal": torch.empty(V, H, W, 3, dtype=_f32, device=dev),
+           "tri": torch.empty(V, H, W, dtype=_i32, device=dev)}
+    L.call("o2345_raster", C.byref(mesh), V, _f(w2c), _f(intr), int(W), int(H), float(near), int(shading), _p(scratch), nbytes,
+           _f(out["color"]), _f(out["alpha"]), _f(out["depth"]), _f(out["normal"]), _p(out["tri"], _i32), _stream())
+    return out
