@@ -12,7 +12,8 @@
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
  *   - all floating point data is fp32, dense and contiguous in the stated layout;
  *   - the caller allocates every buffer (outputs and scratch); nothing is allocated or
- *     freed behind the ABI and no call synchronises the device;
+ *     freed behind the ABI and no call synchronises the device (except the two that say so:
+ *     o2345_lod_children and o2345_surface_sample read a device-side check);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -32,14 +33,15 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 8  /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 9  /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
                                  6: rays of many cameras in one launch: render_blend dir_mode 2, o2345_ray_midpoints_per_ray
                                  7: the GEMM epilogue's GroupNorm column statistics are gone: o2345_epilogue lost its last two fields,
                                     and the norm + patch gather entry point that read the tables went with them
-                                 8: the mesh rasterizer: o2345_raster, o2345_raster_scratch_bytes, o2345_debug_raster_split */
+                                 8: the mesh rasterizer: o2345_raster, o2345_raster_scratch_bytes, o2345_debug_raster_split
+                                 9: mesh scoring: o2345_surface_sample(_scratch_bytes), o2345_nearest, o2345_nn_scratch_bytes */
 
 typedef void* o2345_stream_t;
 
@@ -489,6 +491,35 @@ int o2345_raster(const o2345_raster_mesh* mesh, int V, const float* w2c, const f
 /* Tuning hook (tools/time_raster.py): triangles whose clipped bounding box holds more than `pixels` pixel centres are
  * walked by a warp instead of one thread; 0 restores the default (64). */
 void o2345_debug_raster_split(int pixels);
+
+/* ------------------------------------------------------------------------------------------
+ * Mesh scoring (eval_mesh.py, o2345/mesh_metrics.py): F-Score and Chamfer distance between two surfaces from area-uniform
+ * samples and exact nearest neighbours.  The reference has no metric code; oracle/metrics_oracle.py restates every rule.
+ * ------------------------------------------------------------------------------------------ */
+/* Bytes of scratch o2345_surface_sample needs (-1 for nf < 1). */
+int64_t o2345_surface_sample_scratch_bytes(int64_t nf);
+/* n points drawn area-uniformly on the triangles faces [nf,3] (int32) of verts [nv,3] -> pts [n,3], face_id [n] (int32).
+ *   weight of face t   |(B - A) x (C - A)| in fp64 from the fp32 vertices, every operation rounded to nearest, no
+ *                      contraction; 0 for a face with an index outside [0, nv) or a non-finite weight;
+ *   CDF                sequential fp64 cumulative sums inside chunks of 1024 faces, a sequential scan of the chunk
+ *                      totals, each chunk's offset added to its entries;
+ *   sample i           u_k = top 53 bits of output 3i + k of splitmix64 seeded with `seed` (z = seed + (c + 1) *
+ *                      0x9E3779B97F4A7C15, then the splitmix64 finaliser), times 2^-53; the face is the first whose CDF
+ *                      exceeds u_0 * total (the first that reaches the total if the product rounds up to it); with
+ *                      s = sqrt(u_1): p = ((1 - s) A + s (1 - u_2) B) + s u_2 C in fp64, rounded once to fp32.
+ * Returns O2345_EINVAL when the weights sum to zero: that check reads the total on the host, so this call synchronises
+ * the stream once (after the CDF, before the sampling kernel).  scratch: 8-byte aligned. */
+int o2345_surface_sample(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int64_t n, uint64_t seed,
+                         void* scratch, int64_t scratch_bytes, float* pts, int32_t* face_id, o2345_stream_t stream);
+/* Bytes of scratch o2345_nearest needs (-1 for sizes out of range); a function of n_ref only (n_query is checked). */
+int64_t o2345_nn_scratch_bytes(int64_t n_ref, int64_t n_query);
+/* Exact nearest neighbour: for every query point (query [n_query,3]) the reference point (ref [n_ref,3]) with the least
+ * d2 = (dx*dx + dy*dy) + dz*dz, d = query - ref, every fp32 operation rounded to nearest; equal d2 go to the lower
+ * reference index.  -> dist2 [n_query] (that d2), index [n_query] (int32).  A uniform grid of cubic cells is built over
+ * the reference bbox on the device (at most 256 cells per axis); its search bound is conservative under rounding, so
+ * the result equals a brute-force search bit for bit.  Coordinates must be finite.  scratch: 16-byte aligned. */
+int o2345_nearest(const float* ref, int64_t n_ref, const float* query, int64_t n_query, void* scratch, int64_t scratch_bytes,
+                  float* dist2, int32_t* index, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

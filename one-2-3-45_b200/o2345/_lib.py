@@ -134,12 +134,16 @@ _SIGS = {
     "o2345_raster": (C.c_int, [C.POINTER(RasterMesh), C.c_int, c_fp, c_fp, C.c_int, C.c_int, C.c_float, C.c_int, c_fp, c_i64,
                                c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
     "o2345_debug_raster_split": (None, [C.c_int]),
+    "o2345_surface_sample_scratch_bytes": (c_i64, [c_i64]),
+    "o2345_surface_sample": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_i64, C.c_uint64, c_fp, c_i64, c_fp, c_fp, c_fp]),
+    "o2345_nn_scratch_bytes": (c_i64, [c_i64, c_i64]),
+    "o2345_nearest": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 8          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 9          # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 
@@ -178,7 +182,7 @@ def last_error() -> str:
 
 
 # kernels launched per successful entry-point call (memsets are not counted)
-_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4}
+_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4, "o2345_surface_sample": 5, "o2345_nearest": 7}
 _launches = 0
 
 

@@ -446,3 +446,33 @@ def raster(verts, faces, w2c, intr, W, H, near=0.1, shading=L.SHADE_UNLIT, color
     L.call("o2345_raster", C.byref(mesh), V, _f(w2c), _f(intr), int(W), int(H), float(near), int(shading), _p(scratch), nbytes,
            _f(out["color"]), _f(out["alpha"]), _f(out["depth"]), _f(out["normal"]), _p(out["tri"], _i32), _stream())
     return out
+
+
+# ----------------------------------------------------------------------------- mesh scoring
+def surface_sample(verts, faces, n, seed=0):
+    """n points drawn area-uniformly on a triangle mesh (csrc/metrics.cu): verts [nv,3] fp32, faces [nf,3] int32 (faces with
+    an index outside [0, nv) and zero-area faces get no samples) -> pts [n,3] fp32, face_id [n] int32.  Deterministic in
+    (mesh, n, seed).  Synchronises once; raises O2345Error when the faces have no area."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    n, seed = int(n), int(seed) & (2 ** 64 - 1)
+    nbytes = L.load().o2345_surface_sample_scratch_bytes(nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    pts = torch.empty(max(n, 0), 3, dtype=_f32, device=dev)
+    face_id = torch.empty(max(n, 0), dtype=_i32, device=dev)
+    L.call("o2345_surface_sample", _f(verts), nv, _p(faces, _i32), nf, n, seed, _p(scratch), nbytes, _f(pts), _p(face_id, _i32),
+           _stream())
+    return pts, face_id
+
+
+def nearest(query, ref):
+    """Exact nearest neighbour of every query point among the reference points (csrc/metrics.cu): query [nq,3], ref [nr,3]
+    fp32 -> dist2 [nq] fp32 ((dx*dx + dy*dy) + dz*dz, rounded as written), index [nq] int32 (ties: the lower index)."""
+    query, ref = cf32(query).view(-1, 3), cf32(ref).view(-1, 3)
+    nq, nr, dev = query.shape[0], ref.shape[0], query.device
+    nbytes = L.load().o2345_nn_scratch_bytes(nr, nq)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    dist2 = torch.empty(nq, dtype=_f32, device=dev)
+    index = torch.empty(nq, dtype=_i32, device=dev)
+    L.call("o2345_nearest", _f(ref), nr, _f(query), nq, _p(scratch), nbytes, _f(dist2), _p(index, _i32), _stream())
+    return dist2, index

@@ -336,6 +336,25 @@ def generate_views_multi(model, inputs_u8, polar_angles, ddim_steps=75, stage2_s
     return out
 
 
+def _checkpoint_state(ckpt):
+    """The state dict of a Zero123 checkpoint given as a path or as loaded: a Lightning file's `state_dict`, or the file itself."""
+    sd = torch.load(ckpt, map_location="cpu") if isinstance(ckpt, (str, os.PathLike)) else ckpt
+    return sd.get("state_dict", sd)
+
+
+def load_clip_image_embedder(ckpt, device="cpu"):
+    """FrozenCLIPImageEmbedder (the CLIP ViT-L/14 image tower) from a Zero123 checkpoint: only its
+    `cond_stage_model.model.visual.*` tensors are read and no UNet is built.  A missing tower tensor is an error."""
+    from .clip_image import FrozenCLIPImageEmbedder
+    prefix = "cond_stage_model."
+    sd = {k[len(prefix):]: v for k, v in _checkpoint_state(ckpt).items() if k.startswith(prefix + "model.visual.")}
+    m = FrozenCLIPImageEmbedder()
+    missing = m.load_state_dict(sd, strict=False).missing_keys
+    if missing:
+        raise KeyError(f"checkpoint lacks {len(missing)} tensors of the CLIP image tower, e.g. {missing[:3]}")
+    return m.requires_grad_(False).to(device)
+
+
 def load_zero123_checkpoint(ckpt, device="cpu", use_ema=True, unet_config=None, first_stage_config=None, clip=True,
                             report=print):
     """LatentDiffusion from a Zero123 checkpoint (`zero123-xl.ckpt`: a Lightning file with a `state_dict`, or the state
@@ -344,8 +363,7 @@ def load_zero123_checkpoint(ckpt, device="cpu", use_ema=True, unet_config=None, 
       * the CLIP ViT-L/14 image tower is attached and `cond_stage_model.*` loaded (text-side CLIP keys are ignored);
       * anything the sampling path needs and the file lacks is an ERROR, not a silent default."""
     from .checkpoints import zero123_sampling_state
-    sd = torch.load(ckpt, map_location="cpu") if isinstance(ckpt, (str, os.PathLike)) else ckpt
-    sd = sd.get("state_dict", sd)
+    sd = _checkpoint_state(ckpt)
     m = LatentDiffusion(unet_config=unet_config, first_stage_config=first_stage_config)
     if clip:
         from .clip_image import FrozenCLIPImageEmbedder
