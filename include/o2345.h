@@ -12,8 +12,9 @@
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
  *   - all floating point data is fp32, dense and contiguous in the stated layout;
  *   - the caller allocates every buffer (outputs and scratch); nothing is allocated or
- *     freed behind the ABI and no call synchronises the device (except the two that say so:
- *     o2345_lod_children and o2345_surface_sample read a device-side check);
+ *     freed behind the ABI and no call synchronises the device (except the three that say so:
+ *     o2345_lod_children and o2345_surface_sample read a device-side check, o2345_simplify reads
+ *     a count once per round);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -33,7 +34,7 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 9  /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 10 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
@@ -41,7 +42,8 @@ extern "C" {
                                  7: the GEMM epilogue's GroupNorm column statistics are gone: o2345_epilogue lost its last two fields,
                                     and the norm + patch gather entry point that read the tables went with them
                                  8: the mesh rasterizer: o2345_raster, o2345_raster_scratch_bytes, o2345_debug_raster_split
-                                 9: mesh scoring: o2345_surface_sample(_scratch_bytes), o2345_nearest, o2345_nn_scratch_bytes */
+                                 9: mesh scoring: o2345_surface_sample(_scratch_bytes), o2345_nearest, o2345_nn_scratch_bytes
+                                10: mesh simplification: o2345_simplify, o2345_simplify_scratch_bytes */
 
 typedef void* o2345_stream_t;
 
@@ -520,6 +522,35 @@ int64_t o2345_nn_scratch_bytes(int64_t n_ref, int64_t n_query);
  * the result equals a brute-force search bit for bit.  Coordinates must be finite.  scratch: 16-byte aligned. */
 int o2345_nearest(const float* ref, int64_t n_ref, const float* query, int64_t n_query, void* scratch, int64_t scratch_bytes,
                   float* dist2, int32_t* index, o2345_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Mesh simplification (simplify_mesh.py, run.py --target_faces, o2345/mesh_simplify.py): parallel half-edge collapse
+ * driven by quadric error.  Every output vertex is an input vertex.  The reference has no simplifier;
+ * oracle/simplify_oracle.py restates every rule.
+ * ------------------------------------------------------------------------------------------ */
+/* Bytes of scratch o2345_simplify needs (-1 for sizes out of range). */
+int64_t o2345_simplify_scratch_bytes(int64_t nv, int64_t nf);
+/* Reduces the triangles faces [nf,3] (int32) of verts [nv,3] to target_faces or target_faces - 1 faces, unless no legal
+ * collapse is left first.  Faces with a repeated index are dropped first.  Works in rounds on the mesh as it stood at the
+ * round's start:
+ *   quadrics   once: n = (B - A) x (C - A) in fp64, p = (n / |n|, -(n / |n|) . A), Q_f = |n| / 2 * p p^T (0 for |n| = 0);
+ *              a vertex sums its faces' Q_f in ascending face order;
+ *   locks      a vertex is kept when an edge at it does not have exactly two faces or its faces are not one closed fan;
+ *   u -> v     u unlocked, v a neighbour; the vertices adjacent to both are exactly the two opposite uv, each of valence
+ *              >= 4, val(u) + val(v) - 4 >= 3, and no face of u without v flips or collapses (n' . n > 0, fp64);
+ *   cost       (v, 1)^T (Q_u + Q_v) (v, 1) in fp64, rounded to fp32, non-positive results as +0; u proposes the legal v
+ *              with the least (cost, v) under the key (bits(cost) << 32) | u;
+ *   selection  each key is min-reduced onto the closed 1-rings of u and v and accepted where it holds every one of them
+ *              (at most ceil((F - target) / 2): the least keys); accepted collapses apply together: u -> v in u's faces
+ *              (winding kept), the two faces of uv deleted, Q_v += Q_u.
+ * Every floating-point operation is rounded to nearest in the order of csrc/simplify.cu, without FMA contraction.
+ * Outputs: vertex_index [nv] (capacity; the first out_counts[0] entries are the input indices of the referenced vertices,
+ * ascending), out_faces [nf,3] (capacity; the first out_counts[1] faces, renumbered into vertex_index, in ascending input
+ * order), out_counts [3] (int32: vertices, faces, rounds).  Returns O2345_EINVAL for a face index outside [0, nv) or a
+ * non-finite coordinate.  This call synchronises the stream once to read those checks and once per round to read the
+ * number of accepted collapses.  scratch: 16-byte aligned. */
+int o2345_simplify(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int64_t target_faces, void* scratch,
+                   int64_t scratch_bytes, int32_t* vertex_index, int32_t* out_faces, int32_t* out_counts, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

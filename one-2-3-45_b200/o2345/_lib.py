@@ -138,12 +138,14 @@ _SIGS = {
     "o2345_surface_sample": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_i64, C.c_uint64, c_fp, c_i64, c_fp, c_fp, c_fp]),
     "o2345_nn_scratch_bytes": (c_i64, [c_i64, c_i64]),
     "o2345_nearest": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp]),
+    "o2345_simplify_scratch_bytes": (c_i64, [c_i64, c_i64]),
+    "o2345_simplify": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 9          # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 10         # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 

@@ -476,3 +476,23 @@ def nearest(query, ref):
     index = torch.empty(nq, dtype=_i32, device=dev)
     L.call("o2345_nearest", _f(ref), nr, _f(query), nq, _p(scratch), nbytes, _f(dist2), _p(index, _i32), _stream())
     return dist2, index
+
+
+# ----------------------------------------------------------------------------- mesh simplification
+def simplify_mesh(verts, faces, target_faces):
+    """Quadric-driven half-edge collapse down to target_faces or target_faces - 1 faces (csrc/simplify.cu): verts [nv,3]
+    fp32, faces [nf,3] int32 -> vertex_index [nv'] int32 (the input indices of the kept vertices, ascending; every output
+    vertex is an input vertex), faces [nf',3] int32 renumbered into vertex_index, in ascending input order, and the number
+    of rounds.  Fewer faces than asked for are left only when no legal collapse remains.  Deterministic.  Synchronises
+    once per round; raises O2345Error for an index outside [0, nv) or a non-finite coordinate."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    nbytes = L.load().o2345_simplify_scratch_bytes(nv, nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    vertex_index = torch.empty(max(nv, 1), dtype=_i32, device=dev)
+    out = torch.empty(max(nf, 1), 3, dtype=_i32, device=dev)
+    counts = torch.empty(3, dtype=_i32, device=dev)
+    L.call("o2345_simplify", _f(verts), nv, _p(faces, _i32), nf, int(target_faces), _p(scratch), nbytes, _p(vertex_index, _i32),
+           _p(out, _i32), _p(counts, _i32), _stream())
+    n_v, n_f, rounds = counts.tolist()
+    return vertex_index[:n_v], out[:n_f], rounds

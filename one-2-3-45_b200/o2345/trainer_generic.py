@@ -67,13 +67,14 @@ class GenericTrainer(nn.Module):
         return obtain_pyramid_feature_maps(extractor, imgs)
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
-                alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360):
+                alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
                                  iter_step=iter_step, save_vis=save_vis)
         if mode == 'export_mesh':
-            return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution)
+            return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution,
+                                         target_faces=target_faces)
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -196,7 +197,9 @@ class GenericTrainer(nn.Module):
 
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
-    def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False):
+    def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None):
+        """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
+        after the vertex merge and before mesh.ply is written."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
         if self.num_lods > 1:
             # the lod-1 mesh is coloured with the lod-0 feature maps, as in the reference (:959-978)
@@ -208,7 +211,7 @@ class GenericTrainer(nn.Module):
                 conditional_valid_mask_volume=cond1['valid_mask_volume_scale1'], feature_maps=fmaps, color_maps=imgs,
                 w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
                 rendering_network=self.rendering_network_lod1, lod=1, threshold=0, query_c2w=sample['query_c2w'],
-                scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH])
+                scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces)
         return self.validate_colored_mesh(
             density_or_sdf_network=self.sdf_network_lod0,
             func_extract_geometry=self.sdf_renderer_lod0.extract_geometry, resolution=resolution,
@@ -216,7 +219,7 @@ class GenericTrainer(nn.Module):
             conditional_valid_mask_volume=cond['valid_mask_volume_scale0'], feature_maps=fmaps, color_maps=imgs,
             w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
             rendering_network=self.rendering_network_lod0, lod=0, threshold=0, query_c2w=sample['query_c2w'],
-            scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH])
+            scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces)
 
     @torch.no_grad()
     def validate_colored_mesh(self, density_or_sdf_network, func_extract_geometry, world_space=True, resolution=360,
@@ -224,7 +227,7 @@ class GenericTrainer(nn.Module):
                               feature_maps=None, color_maps=None, w2cs=None, target_candidate_w2cs=None,
                               intrinsics=None, rendering_network=None, rendering_projector=None, query_c2w=None,
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
-                              iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256)):
+                              iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None):
         bmin = torch.tensor(bound_min, dtype=torch.float32)
         bmax = torch.tensor(bound_max, dtype=torch.float32)
         vertices, triangles, fields = func_extract_geometry(
@@ -249,6 +252,9 @@ class GenericTrainer(nn.Module):
         # listed the vertices that sit on one (on the device), and only those are compared.
         vertices, triangles, colors = merge_vertices(vertices, triangles, colors,
                                                      candidates=getattr(renderer, "mc_lattice_candidates", None))
+        if target_faces is not None:
+            from .mesh_simplify import simplify
+            vertices, triangles, colors, _ = simplify(vertices, triangles, colors, target_faces, conditional_volume.device)
         if self.base_exp_dir is not None:
             os.makedirs(self.base_exp_dir, exist_ok=True)
             write_ply(os.path.join(self.base_exp_dir, 'mesh.ply'), vertices, triangles, colors)

@@ -1,5 +1,5 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--output_format .ply]`
+[--mesh_resolution R] [--target_faces N] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -11,7 +11,8 @@ plain (or transparent) background -- and the LoFTR elevation search (`--polar_an
 fetch the released ones).  With `--zero123_ckpt` the file is loaded the way the reference samples from it: the UNet takes
 the EMA shadow (`model_ema.*`, reference ldm/modules/ema.py:14-21 + ddpm.py:180-193), the CLIP ViT-L/14 image tower is
 attached and takes `cond_stage_model.*`; a file that lacks what the sampler needs is refused.  `--output_format .obj/.glb`
-follow reference utils/utils.py:31-45 (o2345/mesh_io.py).
+follow reference utils/utils.py:31-45 (o2345/mesh_io.py).  `--target_faces N` (not in the reference) simplifies the
+mesh to N faces on the GPU before mesh.ply is written (o2345/mesh_simplify.py); .obj / .glb are converted from that mesh.
 
 Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
 calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
@@ -48,6 +49,8 @@ def parse_args(argv=None):
     ap.add_argument('--half_precision', action='store_true', help='accepted for compatibility: the UNet / VAE kernels are fp16')
     ap.add_argument('--mesh_resolution', type=int, default=256, help='Mesh resolution')
     ap.add_argument('--output_format', type=str, default=".ply", help='Output format: .ply, .obj, .glb')
+    ap.add_argument('--target_faces', type=int, default=None,
+                    help='simplify the mesh to this many faces (quadric edge collapse; default: the full marching-cubes mesh)')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -55,7 +58,10 @@ def parse_args(argv=None):
                     help='base seed of the sampler noise: image i uses seed + i (default: unseeded for one image, 0 for several)')
     ap.add_argument('--zero123_ckpt', type=str, default=None, help='zero123-xl.ckpt (state_dict); default: seeded synthetic weights')
     ap.add_argument('--recon_ckpt', type=str, default=None, help='reconstruction checkpoint (ckpt_*.pth); default: seeded synthetic weights')
-    return ap.parse_args(argv)
+    args = ap.parse_args(argv)
+    if args.target_faces is not None and args.target_faces < 0:
+        ap.error("--target_faces must be >= 0")
+    return args
 
 
 def plan_inputs(paths, polar_angles):
@@ -123,7 +129,7 @@ def main(argv=None):
         if args.seed is not None:
             torch.cuda.manual_seed(args.seed)
         mesh = image_to_mesh(model, trainer, load_input(args.img_path[0]), polar_angle=polars[0],
-                             resolution=args.mesh_resolution, exp_dir=shape_dir)
+                             resolution=args.mesh_resolution, exp_dir=shape_dir, target_faces=args.target_faces)
         mesh_path = _write_format(shape_dir, args.output_format)
         print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", mesh_path)
@@ -135,7 +141,7 @@ def main(argv=None):
     paths = []
     for i, mesh in images_to_meshes(model, trainer, [load_input(args.img_path[i]) for i in mine], [polars[i] for i in mine],
                                     seed=0 if args.seed is None else args.seed, resolution=args.mesh_resolution,
-                                    exp_dirs=[shape_dirs[i] for i in mine], indices=mine):
+                                    exp_dirs=[shape_dirs[i] for i in mine], indices=mine, target_faces=args.target_faces):
         paths.append(_write_format(shape_dirs[i], args.output_format))
         print(f"{args.img_path[i]}: {len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", paths[-1])

@@ -1,0 +1,74 @@
+"""Simplifies a mesh on the GPU (o2345/mesh_simplify.py, csrc/simplify.cu):
+
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out small.glb --target_faces 20000
+
+Reads .ply (as run.py writes it) or .obj, welds coincident vertices first (mesh_io.merge_vertices: an OBJ written with
+one vertex per face corner would otherwise be all boundary, and boundary vertices are never removed), reduces it to
+--target_faces or one fewer faces by quadric-driven half-edge collapse and writes .ply, .obj or .glb by the output's
+extension, in the input's own coordinates.  Every output vertex is an input vertex with its colour.  Prints the face and
+vertex counts before and after and the number of rounds."""
+from __future__ import annotations
+
+import argparse
+import os
+import sys
+
+HERE = os.path.dirname(os.path.abspath(__file__))
+if HERE not in sys.path:
+    sys.path.insert(0, HERE)
+
+INPUTS = (".ply", ".obj")
+OUTPUTS = (".ply", ".obj", ".glb")
+
+
+def parse_args(argv=None):
+    ap = argparse.ArgumentParser(description=__doc__.split("\n\n")[0])
+    ap.add_argument("--in", dest="inp", required=True, help="input mesh (.ply or .obj)")
+    ap.add_argument("--out", required=True, help="output mesh (.ply, .obj or .glb)")
+    ap.add_argument("--target_faces", type=int, required=True, help="number of faces to reduce to")
+    args = ap.parse_args(argv)
+    if os.path.splitext(args.inp)[1].lower() not in INPUTS:
+        ap.error(f"{args.inp}: unsupported input format (only {', '.join(INPUTS)})")
+    if os.path.splitext(args.out)[1].lower() not in OUTPUTS:
+        ap.error(f"{args.out}: unsupported output format (only {', '.join(OUTPUTS)})")
+    if args.target_faces < 0:
+        ap.error("--target_faces must be >= 0")
+    return args
+
+
+def read_mesh(path):
+    """-> (vertices float32 [n,3], triangles [m,3], colors uint8 [n,4]); an OBJ without colours is white."""
+    import numpy as np
+    from o2345 import mesh_io
+    if path.lower().endswith(".ply"):
+        return mesh_io.read_ply(path)
+    v, f, c = mesh_io.read_obj(path)
+    c = np.ones((len(v), 3)) if c is None else c
+    rgba = np.concatenate([np.round(np.clip(c, 0, 1) * 255), np.full((len(v), 1), 255)], 1).astype(np.uint8)
+    return v.astype(np.float32), f, rgba
+
+
+def write_mesh(path, v, f, c):
+    from o2345 import mesh_io
+    ext = os.path.splitext(path)[1].lower()
+    {".ply": mesh_io.write_ply, ".obj": mesh_io.write_obj, ".glb": mesh_io.write_glb}[ext](path, v, f, c)
+
+
+def main(argv=None):
+    args = parse_args(argv)
+    from o2345 import mesh_io
+    from o2345.mesh_simplify import simplify
+    v, f, c = read_mesh(args.inp)
+    print(f"read {args.inp}: {len(v)} vertices, {len(f)} faces")
+    v, f, c = mesh_io.merge_vertices(v, f, c)
+    print(f"welded: {len(v)} vertices, {len(f)} faces")
+    v, f, c, rounds = simplify(v, f, c, args.target_faces)
+    print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
+    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+    write_mesh(args.out, v, f, c)
+    print("wrote", args.out)
+    return v, f, c, rounds
+
+
+if __name__ == "__main__":
+    main()
