@@ -12,9 +12,9 @@
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
  *   - all floating point data is fp32, dense and contiguous in the stated layout;
  *   - the caller allocates every buffer (outputs and scratch); nothing is allocated or
- *     freed behind the ABI and no call synchronises the device (except the three that say so:
+ *     freed behind the ABI and no call synchronises the device (except the four that say so:
  *     o2345_lod_children and o2345_surface_sample read a device-side check, o2345_simplify reads
- *     a count once per round);
+ *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -34,7 +34,7 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 10 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 11 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
@@ -43,7 +43,9 @@ extern "C" {
                                     and the norm + patch gather entry point that read the tables went with them
                                  8: the mesh rasterizer: o2345_raster, o2345_raster_scratch_bytes, o2345_debug_raster_split
                                  9: mesh scoring: o2345_surface_sample(_scratch_bytes), o2345_nearest, o2345_nn_scratch_bytes
-                                10: mesh simplification: o2345_simplify, o2345_simplify_scratch_bytes */
+                                10: mesh simplification: o2345_simplify, o2345_simplify_scratch_bytes
+                                11: texture baking: o2345_texture_atlas, o2345_texel_points, o2345_texture_fill,
+                                    o2345_transfer_colors and their scratch-size functions */
 
 typedef void* o2345_stream_t;
 
@@ -551,6 +553,63 @@ int64_t o2345_simplify_scratch_bytes(int64_t nv, int64_t nf);
  * number of accepted collapses.  scratch: 16-byte aligned. */
 int o2345_simplify(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int64_t target_faces, void* scratch,
                    int64_t scratch_bytes, int32_t* vertex_index, int32_t* out_faces, int32_t* out_counts, o2345_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * Texture baking (o2345/mesh_texture.py, run.py / simplify_mesh.py --texture_size): one isometric chart per face packed
+ * into an N x N atlas, the surface point behind every texel a chart owns, push-pull fill of the rest, and colours taken
+ * from a source mesh.  The reference has no texture baking; oracle/texture_oracle.py restates every rule.
+ * N is a power of two in [64, 8192].  Every floating-point operation is rounded to nearest in the order of
+ * csrc/texture.cu, without FMA contraction.
+ * ------------------------------------------------------------------------------------------ */
+/* Bytes of scratch o2345_texture_atlas needs (-1 for sizes out of range). */
+int64_t o2345_texture_atlas_scratch_bytes(int64_t nf);
+/* The atlas of the triangles faces [nf,3] (int32) of verts [nv,3]:
+ *   chart    base = the longest of the edges (v0v1, v1v2, v2v0) by fp32 squared length, the first on ties; a = its first
+ *            vertex, b its second, c the third; L = |b - a|, d = (c - a).(b - a) / L, h = |(b - a) x (c - a)| / L in fp64
+ *            from the fp32 vertices, rounded once to fp32 (d and h are 0 for L = 0; d is clamped to [0, L]);
+ *   box      w = ceil(L rho) + 4, hgt = ceil(h rho) + 4 texels (a padding of 2 on each side);
+ *   packing  boxes sorted by height descending, then face index; next-fit shelves: a box goes at the cursor unless it
+ *            would cross x = N, when a new shelf opens below the tallest box of the current one; it fits when every box
+ *            lies inside N x N;
+ *   scale    rho0 = sqrt(0.5 N^2 / S), S = the sum of L h in fp64 (sequential inside chunks of 1024 faces, then over the
+ *            chunk totals); rho_j = rho0 * j / 64; j = 1 must fit (else O2345_EINVAL), then a binary search over
+ *            lo = 1, hi = 257 keeps the largest j that fits.
+ * Outputs: uv [nf,3,2] (row k for corner faces[f,k]: a at (x+2, y+2), b at (x+2+L rho, y+2), c at (x+2+d rho, y+2+h rho),
+ * divided by N; texel i's centre is at (i + 0.5) / N), boxes [nf,4] int32 (x, y, w, hgt), owner [N*N] int32 (the face whose
+ * box holds the texel, -1 where none does), *rung_host = j and *rho_host = rho_j (either may be NULL).  Returns
+ * O2345_EINVAL for a face index outside [0, nv), a non-finite coordinate, faces without area or charts that do not fit
+ * at j = 1.  This call synchronises the stream once to read the checks and the sum, then once per trial of the search
+ * (about 9 times).  scratch: 16-byte aligned. */
+int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int N, void* scratch,
+                        int64_t scratch_bytes, float* uv, int32_t* boxes, int32_t* owner, int32_t* rung_host,
+                        double* rho_host, o2345_stream_t stream);
+/* Bytes of scratch o2345_texel_points needs (-1 for an invalid N). */
+int64_t o2345_texel_points_scratch_bytes(int N);
+/* For the faces and the uv / owner of o2345_texture_atlas: texel_index [N*N] (capacity; the first *count entries are the
+ * owned texels, ascending), texel_face [N*N] their faces and points [N*N,3] their surface points: the point of the chart's
+ * triangle (uv * N, corners a, b, c as in the atlas) closest to the texel centre as barycentrics (la, lb, lc) in fp64
+ * (the 7-region test), then (la A + lb B) + lc C in fp32 with the weights rounded to fp32.  A texel whose closest point
+ * is a corner gets that vertex's position exactly.  count: one int32 on the device.  Faces must be ones the atlas
+ * accepted (a face index outside [0, nv) gives NaN points).  scratch: 16-byte aligned. */
+int o2345_texel_points(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
+                       const int32_t* owner, int N, void* scratch, int64_t scratch_bytes, int32_t* texel_index,
+                       float* points, int32_t* texel_face, int32_t* count, o2345_stream_t stream);
+/* Bytes of scratch o2345_texture_fill needs (-1 for an invalid N). */
+int64_t o2345_texture_fill_scratch_bytes(int N);
+/* texture [N,N,3] fp32 := rgb [*count,3] at texel_index (as o2345_texel_points lists them); every texel with owner < 0 is
+ * filled by push-pull: pull builds levels N/2 .. 1 where a texel's weight is the sum of its 2 x 2 children's (an owned
+ * texel weighs 1) and its colour their weight-normalised mean (((w0 c0 + w1 c1) + w2 c2) + w3 c3) / (((w0 + w1) + w2) + w3)
+ * in fp32 (children row-major), 0 without weight; push, from coarse to fine, gives every texel of weight 0 its parent's
+ * colour.  Owned texels are never changed.  scratch: 16-byte aligned. */
+int o2345_texture_fill(const int32_t* texel_index, const int32_t* count, const float* rgb, const int32_t* owner, int N,
+                       void* scratch, int64_t scratch_bytes, float* texture, o2345_stream_t stream);
+/* Colour transfer from a source mesh verts [nv,3], faces [nf,3], colors [nv,3] fp32: for point i of points [n,3], face f =
+ * sample_face[nn_index[i]] (the face of its nearest surface sample, o2345_surface_sample + o2345_nearest), the closest
+ * point of f to the point as in o2345_texel_points (corners in face order) and rgb [n,3] = (l0 C0 + l1 C1) + l2 C2 in fp32.
+ * An index out of range gives NaN. */
+int o2345_transfer_colors(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* colors,
+                          const float* points, int64_t n, const int32_t* nn_index, const int32_t* sample_face,
+                          int64_t n_samples, float* rgb, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -1,0 +1,565 @@
+// Texture baking (ops.texture_atlas / texel_points / texture_fill / transfer_colors, o2345/mesh_texture.py): one isometric
+// chart per face, packed on shelves into an N x N atlas, the surface point behind every texel of a chart, push-pull fill
+// of the texels no chart owns, and the colour of a point taken from the nearest face of a source mesh.
+//
+//   atlas         one thread per face: the chart (base = the longest edge by fp32 squared length, first on ties; L, d, h in
+//                 fp64 rounded once to fp32) and L * h in fp64; the sum of L * h in a fixed order (sequential inside chunks
+//                 of 1024 faces, then over the chunk totals, as metrics.cu's CDF); rho0 = sqrt(0.5 N^2 / sum) on the host;
+//                 per trial of the ladder rho_j = rho0 * j / 64 (a binary search over j in [1, 256]): the boxes (one
+//                 thread per face) and next-fit shelf packing in one warp (stable counting sort by height descending, then
+//                 the shelves in sorted order, 32 boxes per step through shuffles); the fit flag is read on the host;
+//                 finally the uv of every corner (one thread per face) and the owner map (one block per box);
+//   texel points  ordered compaction of the owned texels (o2345_compact), one thread per owned texel: the closest point of
+//                 its chart's triangle to the texel centre (the 7-region test in fp64) and the surface point it maps to;
+//   fill          the owned texels' colours scattered into the texture, a pull pyramid of weighted 2 x 2 means and a push
+//                 pass that hands every empty texel its parent's value;
+//   transfer      one thread per point: the closest point of the source face behind the point's nearest surface sample
+//                 and the face's vertex colours interpolated there.
+//
+// Every floating-point operation is an explicit round-to-nearest intrinsic in the order oracle/texture_oracle.py repeats
+// with numpy (no FMA contraction), so every output is bit-identical to the oracle and independent of thread scheduling.
+#include <math.h>
+
+#include "common.cuh"
+
+namespace o2345 {
+namespace {
+
+constexpr int kChunk = 1024;   // faces per sequential chunk of the L * h sum (the oracle restates this chunking)
+constexpr int kPad = 2;        // texels of padding on every side of a chart's box
+constexpr int kMinN = 64, kMaxN = 8192;
+constexpr int kRungs = 256, kRungDen = 64;   // rho_j = rho0 * j / 64, j in [1, 256]
+enum { kErr = 0, kFits = 1, kCtr = 4 };
+
+struct D3 {
+  double x, y, z;
+};
+
+__device__ __forceinline__ D3 sub3(D3 a, D3 b) { return {__dsub_rn(a.x, b.x), __dsub_rn(a.y, b.y), __dsub_rn(a.z, b.z)}; }
+__device__ __forceinline__ double dot3(D3 a, D3 b) {
+  return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
+}
+
+__device__ __forceinline__ D3 vert(const float* __restrict__ V, int i) {
+  return {(double)__ldg(V + 3 * (int64_t)i), (double)__ldg(V + 3 * (int64_t)i + 1), (double)__ldg(V + 3 * (int64_t)i + 2)};
+}
+
+// The corner that starts the longest edge of the three (v0v1, v1v2, v2v0) by fp32 squared length, the first on ties.
+__device__ __forceinline__ int base_corner(const float* __restrict__ V, const int c[3]) {
+  float best = -1.f;
+  int k0 = 0;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    const float* p = V + 3 * (int64_t)c[k];
+    const float* q = V + 3 * (int64_t)c[(k + 1) % 3];
+    float dx = __fsub_rn(__ldg(q), __ldg(p)), dy = __fsub_rn(__ldg(q + 1), __ldg(p + 1)), dz = __fsub_rn(__ldg(q + 2), __ldg(p + 2));
+    float l2 = __fadd_rn(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy)), __fmul_rn(dz, dz));
+    if (l2 > best) best = l2, k0 = k;
+  }
+  return k0;
+}
+
+// Barycentrics (of a, b, c) of the point of triangle abc closest to p: the 7-region test (three corners, three edges,
+// the interior), in fp64.  A zero-length edge or a zero-area interior cannot divide by zero: the corner a is taken.
+struct Bary {
+  double a, b, c;
+};
+
+__device__ __forceinline__ Bary closest_point(D3 p, D3 a, D3 b, D3 c) {
+  D3 ab = sub3(b, a), ac = sub3(c, a), ap = sub3(p, a);
+  double d1 = dot3(ab, ap), d2 = dot3(ac, ap);
+  if (d1 <= 0.0 && d2 <= 0.0) return {1.0, 0.0, 0.0};
+  D3 bp = sub3(p, b);
+  double d3 = dot3(ab, bp), d4 = dot3(ac, bp);
+  if (d3 >= 0.0 && d4 <= d3) return {0.0, 1.0, 0.0};
+  double vc = __dsub_rn(__dmul_rn(d1, d4), __dmul_rn(d3, d2));
+  if (vc <= 0.0 && d1 >= 0.0 && d3 <= 0.0) {
+    double t = __dsub_rn(d1, d3), v = t > 0.0 ? __ddiv_rn(d1, t) : 0.0;
+    return {__dsub_rn(1.0, v), v, 0.0};
+  }
+  D3 cp = sub3(p, c);
+  double d5 = dot3(ab, cp), d6 = dot3(ac, cp);
+  if (d6 >= 0.0 && d5 <= d6) return {0.0, 0.0, 1.0};
+  double vb = __dsub_rn(__dmul_rn(d5, d2), __dmul_rn(d1, d6));
+  if (vb <= 0.0 && d2 >= 0.0 && d6 <= 0.0) {
+    double t = __dsub_rn(d2, d6), w = t > 0.0 ? __ddiv_rn(d2, t) : 0.0;
+    return {__dsub_rn(1.0, w), 0.0, w};
+  }
+  double va = __dsub_rn(__dmul_rn(d3, d6), __dmul_rn(d5, d4));
+  double e43 = __dsub_rn(d4, d3), e56 = __dsub_rn(d5, d6);
+  if (va <= 0.0 && e43 >= 0.0 && e56 >= 0.0) {
+    double t = __dadd_rn(e43, e56), w = t > 0.0 ? __ddiv_rn(e43, t) : 0.0;
+    return {0.0, __dsub_rn(1.0, w), w};
+  }
+  double den = __dadd_rn(__dadd_rn(va, vb), vc);
+  if (!(den > 0.0)) return {1.0, 0.0, 0.0};
+  double v = __ddiv_rn(vb, den), w = __ddiv_rn(vc, den);
+  return {__dsub_rn(__dsub_rn(1.0, v), w), v, w};
+}
+
+// (la * A + lb * B) + lc * C per component in fp32, the weights rounded to fp32 first
+__device__ __forceinline__ void blend3(const Bary& l, const float* A, const float* B, const float* C, float* out) {
+  float la = __double2float_rn(l.a), lb = __double2float_rn(l.b), lc = __double2float_rn(l.c);
+#pragma unroll
+  for (int k = 0; k < 3; ++k) out[k] = __fadd_rn(__fadd_rn(__fmul_rn(la, A[k]), __fmul_rn(lb, B[k])), __fmul_rn(lc, C[k]));
+}
+
+// ----------------------------------------------------------------------------- atlas
+// err bit 1: a face index outside [0, nv), bit 2: a non-finite coordinate
+__global__ void check_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
+                             int32_t* __restrict__ ctr) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < nf) {
+    int a = F[3 * i], b = F[3 * i + 1], c = F[3 * i + 2];
+    if (!(a >= 0 && a < nv && b >= 0 && b < nv && c >= 0 && c < nv)) atomicOr(ctr + kErr, 1);
+  }
+  if (i < nv) {
+    for (int k = 0; k < 3; ++k)
+      if (!isfinite(V[3 * i + k])) atomicOr(ctr + kErr, 2);
+  }
+}
+
+// chart[f] = (L, d, h, base corner bits), lh[f] = L * h in fp64 (exact: two fp32 factors)
+__global__ void chart_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
+                             float4* __restrict__ chart, double* __restrict__ lh) {
+  int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= nf) return;
+  int c[3] = {F[3 * f], F[3 * f + 1], F[3 * f + 2]};
+  if (!(c[0] >= 0 && c[0] < nv && c[1] >= 0 && c[1] < nv && c[2] >= 0 && c[2] < nv)) {   // refused on the host
+    chart[f] = make_float4(0.f, 0.f, 0.f, 0.f), lh[f] = 0.0;
+    return;
+  }
+  int k0 = base_corner(V, c);
+  D3 a = vert(V, c[k0]), b = vert(V, c[(k0 + 1) % 3]), q = vert(V, c[(k0 + 2) % 3]);
+  D3 e1 = sub3(b, a), e2 = sub3(q, a);
+  double L = __dsqrt_rn(dot3(e1, e1)), d = 0.0, h = 0.0;
+  if (L > 0.0) {
+    D3 n = {__dsub_rn(__dmul_rn(e1.y, e2.z), __dmul_rn(e1.z, e2.y)), __dsub_rn(__dmul_rn(e1.z, e2.x), __dmul_rn(e1.x, e2.z)),
+            __dsub_rn(__dmul_rn(e1.x, e2.y), __dmul_rn(e1.y, e2.x))};
+    d = __ddiv_rn(dot3(e2, e1), L);
+    h = __ddiv_rn(__dsqrt_rn(dot3(n, n)), L);
+  }
+  float Lf = __double2float_rn(L), df = __double2float_rn(d), hf = __double2float_rn(h);
+  df = fminf(fmaxf(df, 0.f), Lf);   // 0 <= d <= L up to rounding: clamped so the chart stays inside its box
+  chart[f] = make_float4(Lf, df, hf, __int_as_float(k0));
+  lh[f] = __dmul_rn((double)Lf, (double)hf);
+}
+
+// one thread per chunk: tot[chunk] = sequential sum of the chunk's L * h
+__global__ void chunk_sum_kernel(const double* __restrict__ lh, int64_t nf, double* __restrict__ tot, int64_t nchunks) {
+  int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= nchunks) return;
+  int64_t a = k * kChunk, b = min(a + kChunk, nf);
+  double run = 0.0;
+  for (int64_t t = a; t < b; ++t) run = __dadd_rn(run, lh[t]);
+  tot[k] = run;
+}
+
+// one thread: tot[nchunks] = sum of the chunk totals in order
+__global__ void total_kernel(double* __restrict__ tot, int64_t nchunks) {
+  double run = 0.0;
+  for (int64_t k = 0; k < nchunks; ++k) run = __dadd_rn(run, tot[k]);
+  tot[nchunks] = run;
+}
+
+// box side of a chart extent e at scale rho: ceil(e * rho) + 2P (anything wider than N is N + 1: it cannot fit)
+__device__ __forceinline__ int box_side(float e, double rho, int N) {
+  double s = ceil(__dmul_rn((double)e, rho));
+  return s > (double)N ? N + 1 : (int)s + 2 * kPad;
+}
+
+// boxes[f] = (x, y, w, hgt): w and hgt at scale rho (x and y come from the packing)
+__global__ void box_kernel(const float4* __restrict__ chart, int64_t nf, double rho, int N, int32_t* __restrict__ boxes) {
+  int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= nf) return;
+  float4 ch = chart[f];
+  boxes[4 * f + 2] = box_side(ch.x, rho, N);
+  boxes[4 * f + 3] = box_side(ch.z, rho, N);
+}
+
+// One warp.  Stable counting sort of the boxes by height descending (order), then next-fit shelves: a box goes at the
+// cursor unless it would cross x = N, in which case a new shelf opens below the tallest box (the first) of the current
+// one.  *fits = every box lies inside N x N; boxes[f].x, .y are written up to the first box that does not fit.
+__global__ void __launch_bounds__(32) pack_kernel(int32_t* __restrict__ boxes, int nf, int N, int32_t* __restrict__ order,
+                                                  int32_t* __restrict__ fits) {
+  __shared__ int start[kMaxN + 2];
+  const int lane = threadIdx.x;
+  for (int i = lane; i <= N; i += 32) start[i] = 0;
+  __syncwarp();
+  bool over = false;
+  for (int f = lane; f < nf; f += 32) {
+    int w = boxes[4 * f + 2], h = boxes[4 * f + 3];
+    if (w > N || h > N) over = true;
+    else atomicAdd(start + h, 1);
+  }
+  __syncwarp();
+  if (__any_sync(0xffffffffu, over)) {
+    if (lane == 0) *fits = 0;
+    return;
+  }
+  // exclusive start of every height, heights descending: lane l scans the rank chunk [l c, (l + 1) c) of r = N - h
+  const int c = (N + 1 + 31) / 32, r0 = min(lane * c, N + 1), r1 = min(r0 + c, N + 1);
+  int sum = 0;
+  for (int r = r0; r < r1; ++r) sum += start[N - r];
+  int incl = sum;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    int t = __shfl_up_sync(0xffffffffu, incl, o);
+    if (lane >= o) incl += t;
+  }
+  __syncwarp();
+  int run = incl - sum;
+  for (int r = r0; r < r1; ++r) {
+    int n = start[N - r];
+    start[N - r] = run;
+    run += n;
+  }
+  __syncwarp();
+  const unsigned lt = (1u << lane) - 1u;
+  for (int base = 0; base < nf; base += 32) {   // scatter in face order: stable
+    int f = base + lane;
+    int h = f < nf ? boxes[4 * f + 3] : -1;
+    unsigned m = __match_any_sync(0xffffffffu, h);
+    int pos = f < nf ? start[h] + __popc(m & lt) : 0;
+    __syncwarp();
+    if (f < nf) {
+      order[pos] = f;
+      if (lane == 31 - __clz(m)) start[h] += __popc(m);
+    }
+    __syncwarp();
+  }
+  int cx = 0, cy = 0, sh = 0;
+  bool ok = true;
+  for (int base = 0; base < nf && ok; base += 32) {
+    int i = base + lane, f = i < nf ? order[i] : 0;
+    int w = i < nf ? boxes[4 * f + 2] : 0, h = i < nf ? boxes[4 * f + 3] : 0, x = 0, y = 0;
+    int n = min(32, nf - base);
+    for (int k = 0; k < n; ++k) {
+      int wk = __shfl_sync(0xffffffffu, w, k), hk = __shfl_sync(0xffffffffu, h, k);
+      if (cx > 0 && cx + wk > N) cy += sh, cx = 0, sh = 0;
+      if (cx + wk > N || cy + hk > N) {
+        ok = false;
+        n = k;
+        break;
+      }
+      if (lane == k) x = cx, y = cy;
+      cx += wk, sh = max(sh, hk);
+    }
+    if (lane < n) boxes[4 * f] = x, boxes[4 * f + 1] = y;
+  }
+  if (lane == 0) *fits = ok ? 1 : 0;
+}
+
+// uv[f][k] of corner k: a at (x + P, y + P), b at (x + P + L rho, y + P), c at (x + P + d rho, y + P + h rho), / N
+__global__ void uv_kernel(const int32_t* __restrict__ F, const float4* __restrict__ chart, const int32_t* __restrict__ boxes,
+                          int64_t nf, double rho, int N, float* __restrict__ uv) {
+  int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (f >= nf) return;
+  float4 ch = chart[f];
+  int k0 = __float_as_int(ch.w);
+  double x = (double)(boxes[4 * f] + kPad), y = (double)(boxes[4 * f + 1] + kPad), n = (double)N;
+  double px[3] = {x, __dadd_rn(x, __dmul_rn((double)ch.x, rho)), __dadd_rn(x, __dmul_rn((double)ch.y, rho))};
+  double py[3] = {y, y, __dadd_rn(y, __dmul_rn((double)ch.z, rho))};
+#pragma unroll
+  for (int j = 0; j < 3; ++j) {
+    int k = (k0 + j) % 3;
+    uv[6 * f + 2 * k] = __double2float_rn(__ddiv_rn(px[j], n));
+    uv[6 * f + 2 * k + 1] = __double2float_rn(__ddiv_rn(py[j], n));
+  }
+}
+
+// one block per face: owner[texel] = f for every texel of its box
+__global__ void owner_kernel(const int32_t* __restrict__ boxes, int N, int32_t* __restrict__ owner) {
+  const int f = blockIdx.x;
+  const int x = boxes[4 * f], y = boxes[4 * f + 1], w = boxes[4 * f + 2], h = boxes[4 * f + 3];
+  for (int t = threadIdx.x; t < w * h; t += blockDim.x) owner[(int64_t)(y + t / w) * N + x + t % w] = f;
+}
+
+struct AtlasLayout {
+  int64_t chart, lh, tot, order, ctr, bytes;
+};
+
+int64_t align16(int64_t x) { return (x + 15) & ~(int64_t)15; }
+
+AtlasLayout atlas_layout(int64_t nf) {
+  AtlasLayout L;
+  int64_t o = 0, nchunks = (nf + kChunk - 1) / kChunk;
+  auto take = [&](int64_t& at, int64_t bytes) { at = o, o = align16(o + bytes); };
+  take(L.chart, 16 * nf);
+  take(L.lh, 8 * nf);
+  take(L.tot, 8 * (nchunks + 1));
+  take(L.order, 4 * nf);
+  take(L.ctr, 4 * kCtr);
+  L.bytes = o;
+  return L;
+}
+
+bool valid_size(int N) { return N >= kMinN && N <= kMaxN && (N & (N - 1)) == 0; }
+
+// ----------------------------------------------------------------------------- texel points
+__global__ void owned_kernel(const int32_t* __restrict__ owner, int64_t n, uint8_t* __restrict__ flags) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) flags[i] = owner[i] >= 0;
+}
+
+// One thread per owned texel (the compacted list): the chart's triangle is its face's uv times N (exact), the base corner
+// as in chart_kernel; the closest point of it to the texel centre maps to la A + lb B + lc C.
+__global__ void texel_points_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
+                                    const float* __restrict__ uv, const int32_t* __restrict__ owner, int N,
+                                    const int32_t* __restrict__ texel_index, const int32_t* __restrict__ count,
+                                    float* __restrict__ points, int32_t* __restrict__ texel_face) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= *count) return;
+  int t = texel_index[i], f = owner[t];
+  texel_face[i] = f;
+  int c[3] = {-1, -1, -1};
+  if (f >= 0 && f < nf) c[0] = F[3 * (int64_t)f], c[1] = F[3 * (int64_t)f + 1], c[2] = F[3 * (int64_t)f + 2];
+  if (!(c[0] >= 0 && c[0] < nv && c[1] >= 0 && c[1] < nv && c[2] >= 0 && c[2] < nv)) {   // not a face the atlas accepted
+    points[3 * i] = points[3 * i + 1] = points[3 * i + 2] = __int_as_float(0x7fc00000);
+    return;
+  }
+  int k0 = base_corner(V, c);
+  int ka = k0, kb = (k0 + 1) % 3, kc = (k0 + 2) % 3;
+  const float n = (float)N;
+  auto corner = [&](int k) {
+    return D3{(double)__fmul_rn(uv[6 * (int64_t)f + 2 * k], n), (double)__fmul_rn(uv[6 * (int64_t)f + 2 * k + 1], n), 0.0};
+  };
+  D3 q = {__dadd_rn((double)(t % N), 0.5), __dadd_rn((double)(t / N), 0.5), 0.0};
+  Bary l = closest_point(q, corner(ka), corner(kb), corner(kc));
+  blend3(l, V + 3 * (int64_t)c[ka], V + 3 * (int64_t)c[kb], V + 3 * (int64_t)c[kc], points + 3 * i);
+}
+
+// ----------------------------------------------------------------------------- fill
+__global__ void scatter_kernel(const int32_t* __restrict__ texel_index, const int32_t* __restrict__ count,
+                               const float* __restrict__ rgb, float* __restrict__ tex) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= *count) return;
+  int64_t t = texel_index[i];
+#pragma unroll
+  for (int k = 0; k < 3; ++k) tex[3 * t + k] = rgb[3 * i + k];
+}
+
+// level n (n x n, rgb + weight) from its 2n x 2n children: weights summed, rgb the weight-normalised mean (0 without
+// weight).  The finest children are the texture itself with weight 1 where owned.
+__device__ __forceinline__ float4 child(const float4* __restrict__ lvl, const float* __restrict__ tex,
+                                        const int32_t* __restrict__ owner, int64_t j) {
+  if (lvl) return lvl[j];
+  return make_float4(tex[3 * j], tex[3 * j + 1], tex[3 * j + 2], owner[j] >= 0 ? 1.f : 0.f);
+}
+
+__global__ void pull_kernel(const float4* __restrict__ fine, const float* __restrict__ tex, const int32_t* __restrict__ owner,
+                            int n, float4* __restrict__ coarse) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n * n) return;
+  int64_t y = i / n, x = i % n, w2 = 2 * (int64_t)n;
+  float4 c[4] = {child(fine, tex, owner, 2 * y * w2 + 2 * x), child(fine, tex, owner, 2 * y * w2 + 2 * x + 1),
+                 child(fine, tex, owner, (2 * y + 1) * w2 + 2 * x), child(fine, tex, owner, (2 * y + 1) * w2 + 2 * x + 1)};
+  float sw = __fadd_rn(__fadd_rn(__fadd_rn(c[0].w, c[1].w), c[2].w), c[3].w);
+  float4 o = make_float4(0.f, 0.f, 0.f, sw);
+  if (sw > 0.f) {
+    float s[3];
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+      float v0 = k == 0 ? c[0].x : k == 1 ? c[0].y : c[0].z, v1 = k == 0 ? c[1].x : k == 1 ? c[1].y : c[1].z;
+      float v2 = k == 0 ? c[2].x : k == 1 ? c[2].y : c[2].z, v3 = k == 0 ? c[3].x : k == 1 ? c[3].y : c[3].z;
+      s[k] = __fdiv_rn(__fadd_rn(__fadd_rn(__fadd_rn(__fmul_rn(c[0].w, v0), __fmul_rn(c[1].w, v1)), __fmul_rn(c[2].w, v2)),
+                                 __fmul_rn(c[3].w, v3)),
+                       sw);
+    }
+    o.x = s[0], o.y = s[1], o.z = s[2];
+  }
+  coarse[i] = o;
+}
+
+// every empty texel of an n x n level (the texture itself when lvl is null) takes its parent's rgb
+__global__ void push_kernel(float4* __restrict__ lvl, float* __restrict__ tex, const int32_t* __restrict__ owner, int n,
+                            const float4* __restrict__ parent) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)n * n) return;
+  float4 p = parent[(i / n / 2) * (n / 2) + (i % n) / 2];
+  if (lvl) {
+    if (lvl[i].w == 0.f) lvl[i] = make_float4(p.x, p.y, p.z, 0.f);
+  } else if (owner[i] < 0) {
+    tex[3 * i] = p.x, tex[3 * i + 1] = p.y, tex[3 * i + 2] = p.z;
+  }
+}
+
+// ----------------------------------------------------------------------------- transfer
+__global__ void transfer_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
+                                const float* __restrict__ colors, const float* __restrict__ pts, int64_t n,
+                                const int32_t* __restrict__ nn_index, const int32_t* __restrict__ sample_face,
+                                int64_t n_samples, float* __restrict__ rgb) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int s = nn_index[i], f = s >= 0 && s < n_samples ? sample_face[s] : -1;
+  int c[3] = {-1, -1, -1};
+  if (f >= 0 && f < nf) c[0] = F[3 * (int64_t)f], c[1] = F[3 * (int64_t)f + 1], c[2] = F[3 * (int64_t)f + 2];
+  if (!(c[0] >= 0 && c[0] < nv && c[1] >= 0 && c[1] < nv && c[2] >= 0 && c[2] < nv)) {
+    rgb[3 * i] = rgb[3 * i + 1] = rgb[3 * i + 2] = __int_as_float(0x7fc00000);
+    return;
+  }
+  D3 p = {(double)pts[3 * i], (double)pts[3 * i + 1], (double)pts[3 * i + 2]};
+  Bary l = closest_point(p, vert(V, c[0]), vert(V, c[1]), vert(V, c[2]));
+  blend3(l, colors + 3 * (int64_t)c[0], colors + 3 * (int64_t)c[1], colors + 3 * (int64_t)c[2], rgb + 3 * i);
+}
+
+}  // namespace
+}  // namespace o2345
+
+using namespace o2345;
+
+extern "C" int64_t o2345_texture_atlas_scratch_bytes(int64_t nf) {
+  if (nf < 1 || nf > INT32_MAX / 3) return -1;
+  return atlas_layout(nf).bytes;
+}
+
+extern "C" int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int N, void* scratch,
+                                   int64_t scratch_bytes, float* uv, int32_t* boxes, int32_t* owner, int32_t* rung_host,
+                                   double* rho_host, o2345_stream_t stream) {
+  O2345_CHECK_ARG(verts && faces && uv && boxes && owner, "verts, faces, uv, boxes and owner are required");
+  O2345_CHECK_ARG(nv >= 1 && nv <= INT32_MAX && nf >= 1 && nf <= INT32_MAX / 3, "need 1 <= nv <= 2^31-1 and 1 <= nf <= (2^31-1)/3");
+  O2345_CHECK_ARG(valid_size(N), "N must be a power of two in [64, 8192]");
+  O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_texture_atlas_scratch_bytes(nf),
+                  "scratch smaller than o2345_texture_atlas_scratch_bytes");
+  O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
+  cudaStream_t s = (cudaStream_t)stream;
+  AtlasLayout Lo = atlas_layout(nf);
+  char* p = (char*)scratch;
+  auto* chart = (float4*)(p + Lo.chart);
+  auto* lh = (double*)(p + Lo.lh);
+  auto* tot = (double*)(p + Lo.tot);
+  auto* order = (int32_t*)(p + Lo.order);
+  auto* ctr = (int32_t*)(p + Lo.ctr);
+  const int64_t nchunks = (nf + kChunk - 1) / kChunk;
+  O2345_CUDA(cudaMemsetAsync(ctr, 0, 4 * kCtr, s));
+  check_kernel<<<cdiv(nv > nf ? nv : nf, 256), 256, 0, s>>>(verts, nv, faces, nf, ctr);
+  chart_kernel<<<cdiv(nf, 256), 256, 0, s>>>(verts, nv, faces, nf, chart, lh);
+  chunk_sum_kernel<<<cdiv(nchunks, 64), 64, 0, s>>>(lh, nf, tot, nchunks);
+  total_kernel<<<1, 1, 0, s>>>(tot, nchunks);
+  O2345_LAUNCH_CHECK();
+  int32_t err = 0;
+  double sum = 0.0;   // host reads: the input checks and the sum, then one fit flag per trial
+  O2345_CUDA(cudaMemcpyAsync(&err, ctr + kErr, 4, cudaMemcpyDeviceToHost, s));
+  O2345_CUDA(cudaMemcpyAsync(&sum, tot + nchunks, 8, cudaMemcpyDeviceToHost, s));
+  O2345_CUDA(cudaStreamSynchronize(s));
+  if (err & 1) {
+    set_error("%s: a face index is outside [0, nv)", __func__);
+    return O2345_EINVAL;
+  }
+  if (err & 2) {
+    set_error("%s: a vertex coordinate is not finite", __func__);
+    return O2345_EINVAL;
+  }
+  if (!(sum > 0.0)) {
+    set_error("%s: the faces have no area", __func__);
+    return O2345_EINVAL;
+  }
+  const double rho0 = sqrt(0.5 * ((double)N * (double)N) / sum);
+  auto rho_of = [&](int j) { return rho0 * (double)j / (double)kRungDen; };
+  auto trial = [&](int j, int32_t& fits) {
+    box_kernel<<<cdiv(nf, 256), 256, 0, s>>>(chart, nf, rho_of(j), N, boxes);
+    pack_kernel<<<1, 32, 0, s>>>(boxes, (int)nf, N, order, ctr + kFits);
+    O2345_LAUNCH_CHECK();
+    O2345_CUDA(cudaMemcpyAsync(&fits, ctr + kFits, 4, cudaMemcpyDeviceToHost, s));
+    O2345_CUDA(cudaStreamSynchronize(s));
+    return O2345_OK;
+  };
+  int rc;
+  int32_t fits = 0;
+  if ((rc = trial(1, fits)) != O2345_OK) return rc;
+  if (!fits) {
+    set_error("%s: %d^2 texels cannot hold %lld charts", __func__, N, (long long)nf);
+    return O2345_EINVAL;
+  }
+  int lo = 1, hi = kRungs + 1, last = 1;
+  while (hi - lo > 1) {
+    int mid = (lo + hi) / 2;
+    if ((rc = trial(mid, fits)) != O2345_OK) return rc;
+    last = mid;
+    if (fits) lo = mid;
+    else hi = mid;
+  }
+  if (last != lo && (rc = trial(lo, fits)) != O2345_OK) return rc;   // the boxes of the chosen rung
+  const double rho = rho_of(lo);
+  uv_kernel<<<cdiv(nf, 256), 256, 0, s>>>(faces, chart, boxes, nf, rho, N, uv);
+  O2345_CUDA(cudaMemsetAsync(owner, 0xff, 4 * (int64_t)N * N, s));
+  owner_kernel<<<(unsigned)nf, 128, 0, s>>>(boxes, N, owner);
+  O2345_LAUNCH_CHECK();
+  if (rung_host) *rung_host = lo;
+  if (rho_host) *rho_host = rho;
+  return O2345_OK;
+}
+
+extern "C" int64_t o2345_texel_points_scratch_bytes(int N) {
+  if (!valid_size(N)) return -1;
+  int64_t n = (int64_t)N * N;
+  return align16(n) + 4 * o2345_compact_scratch_ints(n);
+}
+
+extern "C" int o2345_texel_points(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
+                                  const int32_t* owner, int N, void* scratch, int64_t scratch_bytes, int32_t* texel_index,
+                                  float* points, int32_t* texel_face, int32_t* count, o2345_stream_t stream) {
+  O2345_CHECK_ARG(verts && faces && uv && owner && texel_index && points && texel_face && count,
+                  "verts, faces, uv, owner, texel_index, points, texel_face and count are required");
+  O2345_CHECK_ARG(nv >= 1 && nv <= INT32_MAX && nf >= 1 && nf <= INT32_MAX / 3, "need 1 <= nv <= 2^31-1 and 1 <= nf <= (2^31-1)/3");
+  O2345_CHECK_ARG(valid_size(N), "N must be a power of two in [64, 8192]");
+  O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_texel_points_scratch_bytes(N), "scratch smaller than o2345_texel_points_scratch_bytes");
+  O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t n = (int64_t)N * N;
+  auto* flags = (uint8_t*)scratch;
+  auto* cs = (int32_t*)((char*)scratch + align16(n));
+  owned_kernel<<<cdiv(n, 256), 256, 0, s>>>(owner, n, flags);
+  O2345_LAUNCH_CHECK();
+  int rc = o2345_compact(flags, n, texel_index, nullptr, count, cs, stream);
+  if (rc != O2345_OK) return rc;
+  texel_points_kernel<<<cdiv(n, 128), 128, 0, s>>>(verts, nv, faces, nf, uv, owner, N, texel_index, count, points, texel_face);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+extern "C" int64_t o2345_texture_fill_scratch_bytes(int N) {
+  if (!valid_size(N)) return -1;
+  int64_t b = 0;
+  for (int n = N / 2; n >= 1; n /= 2) b += 16 * (int64_t)n * n;
+  return b;
+}
+
+extern "C" int o2345_texture_fill(const int32_t* texel_index, const int32_t* count, const float* rgb, const int32_t* owner,
+                                  int N, void* scratch, int64_t scratch_bytes, float* texture, o2345_stream_t stream) {
+  O2345_CHECK_ARG(texel_index && count && rgb && owner && texture, "texel_index, count, rgb, owner and texture are required");
+  O2345_CHECK_ARG(valid_size(N), "N must be a power of two in [64, 8192]");
+  O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_texture_fill_scratch_bytes(N), "scratch smaller than o2345_texture_fill_scratch_bytes");
+  O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
+  cudaStream_t s = (cudaStream_t)stream;
+  const int64_t n = (int64_t)N * N;
+  float4* lvl[16];
+  int levels = 0;
+  int64_t o = 0;
+  for (int m = N / 2; m >= 1; m /= 2) lvl[levels++] = (float4*)((char*)scratch + o), o += 16 * (int64_t)m * m;
+  O2345_CUDA(cudaMemsetAsync(texture, 0, 12 * n, s));
+  scatter_kernel<<<cdiv(n, 256), 256, 0, s>>>(texel_index, count, rgb, texture);
+  for (int l = 0; l < levels; ++l) {   // pull: level l + 1 of the pyramid (N >> (l + 1) texels a side)
+    int m = N >> (l + 1);
+    pull_kernel<<<cdiv((int64_t)m * m, 256), 256, 0, s>>>(l ? lvl[l - 1] : nullptr, texture, owner, m, lvl[l]);
+  }
+  for (int l = levels - 2; l >= -1; --l) {   // push: coarse to fine, the texture last
+    int m = N >> (l + 1);
+    push_kernel<<<cdiv((int64_t)m * m, 256), 256, 0, s>>>(l >= 0 ? lvl[l] : nullptr, texture, owner, m, lvl[l + 1]);
+  }
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+extern "C" int o2345_transfer_colors(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* colors,
+                                     const float* points, int64_t n, const int32_t* nn_index, const int32_t* sample_face,
+                                     int64_t n_samples, float* rgb, o2345_stream_t stream) {
+  O2345_CHECK_ARG(verts && faces && colors && points && nn_index && sample_face && rgb,
+                  "verts, faces, colors, points, nn_index, sample_face and rgb are required");
+  O2345_CHECK_ARG(nv >= 1 && nv <= INT32_MAX && nf >= 1 && nf <= INT32_MAX / 3, "need 1 <= nv <= 2^31-1 and 1 <= nf <= (2^31-1)/3");
+  O2345_CHECK_ARG(n >= 1 && n <= INT32_MAX && n_samples >= 1 && n_samples <= INT32_MAX, "need 1 <= n, n_samples <= 2^31-1");
+  cudaStream_t s = (cudaStream_t)stream;
+  transfer_kernel<<<cdiv(n, 128), 128, 0, s>>>(verts, nv, faces, nf, colors, points, n, nn_index, sample_face, n_samples, rgb);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}

@@ -140,12 +140,20 @@ _SIGS = {
     "o2345_nearest": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp]),
     "o2345_simplify_scratch_bytes": (c_i64, [c_i64, c_i64]),
     "o2345_simplify": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp]),
+    "o2345_texture_atlas_scratch_bytes": (c_i64, [c_i64]),
+    "o2345_texture_atlas": (C.c_int, [c_fp, c_i64, c_fp, c_i64, C.c_int, c_fp, c_i64, c_fp, c_fp, c_fp,
+                                      C.POINTER(C.c_int32), C.POINTER(C.c_double), c_fp]),
+    "o2345_texel_points_scratch_bytes": (c_i64, [C.c_int]),
+    "o2345_texel_points": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, C.c_int, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp, c_fp]),
+    "o2345_texture_fill_scratch_bytes": (c_i64, [C.c_int]),
+    "o2345_texture_fill": (C.c_int, [c_fp, c_fp, c_fp, c_fp, C.c_int, c_fp, c_i64, c_fp, c_fp]),
+    "o2345_transfer_colors": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 10         # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 11         # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 
@@ -184,7 +192,7 @@ def last_error() -> str:
 
 
 # kernels launched per successful entry-point call (memsets are not counted)
-_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4, "o2345_surface_sample": 5, "o2345_nearest": 7}
+_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4, "o2345_surface_sample": 5, "o2345_nearest": 7, "o2345_texel_points": 5}
 _launches = 0
 
 

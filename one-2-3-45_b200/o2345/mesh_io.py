@@ -11,6 +11,9 @@ Restates, on plain numpy arrays:
                             reference utils/utils.py:31-45 `convert_mesh_format`: rotate +90 degrees about x, 180 degrees
                             about z, negate x, reverse the face winding -- altogether (x, y, z) -> (x, z, y) with flipped
                             faces -- then `.obj` with `v x y z r g b` lines (trimesh's include_color=True) or a binary glTF.
+  * `write_textured_glb` / `write_textured_obj`
+                            a mesh with per-corner uv and a colour texture (o2345/mesh_texture.py; not in the reference):
+                            glTF with an embedded PNG as baseColorTexture, or OBJ + MTL (map_Kd) + PNG.
 """
 from __future__ import annotations
 
@@ -89,14 +92,17 @@ def read_ply(path):
     return vrec["p"].copy(), frec["i"].copy(), vrec["c"].copy()
 
 
-def to_viewer_frame(vertices, triangles):
-    """convert_mesh_format's transform chain (reference utils/utils.py:35-41), applied exactly in its order."""
+def to_viewer_frame(vertices, triangles, uv=None):
+    """convert_mesh_format's transform chain (reference utils/utils.py:35-41), applied exactly in its order.  With uv
+    [m,3,2] (one row per face corner) the rows of each face are reversed with its corners and returned third."""
     v = np.asarray(vertices, np.float64)
     rx = np.array([[1, 0, 0], [0, 0, -1], [0, 1, 0]], np.float64)        # rotation_matrix(pi / 2, [1, 0, 0])
     rz = np.array([[-1, 0, 0], [0, -1, 0], [0, 0, 1]], np.float64)       # rotation_matrix(pi, [0, 0, 1])
     v = v @ rx.T
     v = v @ rz.T
     v[:, 0] = -v[:, 0]
+    if uv is not None:
+        return v, np.fliplr(np.asarray(triangles)).copy(), np.asarray(uv)[:, ::-1].copy()
     return v, np.fliplr(np.asarray(triangles)).copy()
 
 
@@ -149,6 +155,94 @@ def write_glb(path, vertices, triangles, colors):
         fh.write(js)
         fh.write(struct.pack("<II", len(bin_chunk), 0x004E4942))
         fh.write(bytes(bin_chunk))
+
+
+def _png_bytes(texture):
+    import io
+    from PIL import Image
+    buf = io.BytesIO()
+    Image.fromarray(np.ascontiguousarray(texture, np.uint8)).save(buf, format="PNG")
+    return buf.getvalue()
+
+
+def write_textured_glb(path, vertices, triangles, uv, texture):
+    """Binary glTF 2.0 of a textured mesh: vertices [n,3], triangles [m,3], uv [m,3,2] (row k for corner k, glTF's
+    convention), texture uint8 [N,N,3].  Vertices are split per corner (3m of them: POSITION float32, TEXCOORD_0 float32,
+    uint32 indices 0 .. 3m-1) and the material is unlit-friendly PBR: the texture as an embedded PNG baseColorTexture
+    (CLAMP_TO_EDGE, LINEAR), metallic 0, roughness 1.  No COLOR_0."""
+    f = np.asarray(triangles, np.int64).reshape(-1, 3)
+    v = np.ascontiguousarray(np.asarray(vertices, np.float32)[f.reshape(-1)])
+    t = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 2))
+    if len(t) != len(v):
+        raise ValueError(f"uv has {len(t) // 3} faces, triangles {len(f)}")
+    idx = np.arange(len(v), dtype=np.uint32)
+    blobs = [v.tobytes(), t.tobytes(), idx.tobytes(), _png_bytes(texture)]
+    offs, total = [], 0
+    for b in blobs:
+        offs.append(total)
+        total += (len(b) + 3) // 4 * 4
+    bin_chunk = bytearray(total)
+    for o, b in zip(offs, blobs):
+        bin_chunk[o:o + len(b)] = b
+    doc = {
+        "asset": {"version": "2.0", "generator": "o2345-b200"},
+        "scene": 0, "scenes": [{"nodes": [0]}], "nodes": [{"mesh": 0}],
+        "meshes": [{"primitives": [{"attributes": {"POSITION": 0, "TEXCOORD_0": 1}, "indices": 2, "material": 0, "mode": 4}]}],
+        "materials": [{"pbrMetallicRoughness": {"baseColorTexture": {"index": 0}, "metallicFactor": 0.0, "roughnessFactor": 1.0}}],
+        "textures": [{"sampler": 0, "source": 0}],
+        "samplers": [{"magFilter": 9729, "minFilter": 9729, "wrapS": 33071, "wrapT": 33071}],
+        "images": [{"bufferView": 3, "mimeType": "image/png"}],
+        "buffers": [{"byteLength": total}],
+        "bufferViews": [{"buffer": 0, "byteOffset": offs[0], "byteLength": len(blobs[0]), "target": 34962},
+                        {"buffer": 0, "byteOffset": offs[1], "byteLength": len(blobs[1]), "target": 34962},
+                        {"buffer": 0, "byteOffset": offs[2], "byteLength": len(blobs[2]), "target": 34963},
+                        {"buffer": 0, "byteOffset": offs[3], "byteLength": len(blobs[3])}],
+        "accessors": [{"bufferView": 0, "componentType": 5126, "count": int(len(v)), "type": "VEC3",
+                       "min": v.min(0).tolist() if len(v) else [0, 0, 0], "max": v.max(0).tolist() if len(v) else [0, 0, 0]},
+                      {"bufferView": 1, "componentType": 5126, "count": int(len(t)), "type": "VEC2"},
+                      {"bufferView": 2, "componentType": 5125, "count": int(len(idx)), "type": "SCALAR"}],
+    }
+    js = json.dumps(doc, separators=(",", ":")).encode("utf-8")
+    js += b" " * ((4 - len(js) % 4) % 4)
+    with open(path, "wb") as fh:
+        fh.write(struct.pack("<III", 0x46546C67, 2, 12 + 8 + len(js) + 8 + len(bin_chunk)))
+        fh.write(struct.pack("<II", len(js), 0x4E4F534A))
+        fh.write(js)
+        fh.write(struct.pack("<II", len(bin_chunk), 0x004E4942))
+        fh.write(bytes(bin_chunk))
+
+
+def write_textured_obj(path, vertices, triangles, uv, texture):
+    """Wavefront OBJ of a textured mesh beside its material: `v x y z`, then one `vt u (1 - v)` per face corner (OBJ's v
+    points up the image), then `f a/t b/t c/t`; <stem>.mtl (`map_Kd <stem>_albedo.png`) and the PNG next to it."""
+    import os
+    stem = os.path.splitext(os.path.basename(path))[0]
+    folder = os.path.dirname(os.path.abspath(path))
+    v = np.asarray(vertices, np.float64)
+    f = np.asarray(triangles, np.int64).reshape(-1, 3)
+    t = np.asarray(uv, np.float64).reshape(-1, 2)
+    with open(os.path.join(folder, stem + "_albedo.png"), "wb") as fh:
+        fh.write(_png_bytes(texture))
+    with open(os.path.join(folder, stem + ".mtl"), "w") as fh:
+        fh.write("# o2345-b200\nnewmtl albedo\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd %s_albedo.png\n" % stem)
+    with open(path, "w") as fh:
+        fh.write("# o2345-b200\nmtllib %s.mtl\n" % stem)
+        for p in v:
+            fh.write("v %.8f %.8f %.8f\n" % (p[0], p[1], p[2]))
+        for q in t:
+            fh.write("vt %.8f %.8f\n" % (q[0], 1.0 - q[1]))
+        fh.write("usemtl albedo\n")
+        for i, q in enumerate(f + 1):
+            fh.write("f %d/%d %d/%d %d/%d\n" % (q[0], 3 * i + 1, q[1], 3 * i + 2, q[2], 3 * i + 3))
+
+
+def write_textured(path, vertices, triangles, uv, texture):
+    """write_textured_glb or write_textured_obj by the extension of path."""
+    if path.lower().endswith(".glb"):
+        return write_textured_glb(path, vertices, triangles, uv, texture)
+    if path.lower().endswith(".obj"):
+        return write_textured_obj(path, vertices, triangles, uv, texture)
+    raise ValueError(f"{path}: a textured mesh is written as .glb or .obj")
 
 
 def convert_mesh_format(exp_dir, output_format=".obj"):

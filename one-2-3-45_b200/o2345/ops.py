@@ -496,3 +496,68 @@ def simplify_mesh(verts, faces, target_faces):
            _p(out, _i32), _p(counts, _i32), _stream())
     n_v, n_f, rounds = counts.tolist()
     return vertex_index[:n_v], out[:n_f], rounds
+
+
+# ----------------------------------------------------------------------------- texture baking
+def texture_atlas(verts, faces, N):
+    """One isometric chart per face packed into an N x N atlas (csrc/texture.cu): verts [nv,3] fp32, faces [nf,3] int32
+    -> dict(uv [nf,3,2] fp32 (row k for corner k, glTF convention: texel i's centre at (i + 0.5) / N), boxes [nf,4] int32
+    (x, y, w, hgt), owner [N*N] int32 (-1 where no box is), j (the ladder rung), rho (texels per unit length)).
+    Synchronises about 9 times; raises O2345Error for bad input or charts that do not fit."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    nbytes = L.load().o2345_texture_atlas_scratch_bytes(nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    uv = torch.empty(max(nf, 1), 3, 2, dtype=_f32, device=dev)
+    boxes = torch.empty(max(nf, 1), 4, dtype=_i32, device=dev)
+    owner = torch.empty(int(N) * int(N), dtype=_i32, device=dev)
+    j, rho = C.c_int32(0), C.c_double(0.0)
+    L.call("o2345_texture_atlas", _f(verts), nv, _p(faces, _i32), nf, int(N), _p(scratch), nbytes, _f(uv), _p(boxes, _i32),
+           _p(owner, _i32), C.byref(j), C.byref(rho), _stream())
+    return {"uv": uv[:nf], "boxes": boxes[:nf], "owner": owner, "j": j.value, "rho": rho.value}
+
+
+def texel_points(verts, faces, uv, owner, N):
+    """The owned texels of an atlas (texture_atlas) and the surface points behind them: -> texel_index [T] int32
+    (ascending), points [T,3] fp32, texel_face [T] int32.  Reads T on the host."""
+    verts, faces, uv = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3), cf32(uv).view(-1, 3, 2)
+    nv, nf, dev, n = verts.shape[0], faces.shape[0], verts.device, int(N) * int(N)
+    nbytes = L.load().o2345_texel_points_scratch_bytes(int(N))
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    index = torch.empty(n, dtype=_i32, device=dev)
+    points = torch.empty(n, 3, dtype=_f32, device=dev)
+    face = torch.empty(n, dtype=_i32, device=dev)
+    count = torch.empty(1, dtype=_i32, device=dev)
+    L.call("o2345_texel_points", _f(verts), nv, _p(faces, _i32), nf, _f(uv), _p(owner.contiguous(), _i32), int(N), _p(scratch),
+           nbytes, _p(index, _i32), _f(points), _p(face, _i32), _p(count, _i32), _stream())
+    T = int(count.item())
+    return index[:T], points[:T], face[:T]
+
+
+def texture_fill(texel_index, rgb, owner, N):
+    """texture [N,N,3] fp32: rgb [T,3] at texel_index [T] and push-pull fill of every texel with owner < 0."""
+    rgb, dev = cf32(rgb).view(-1, 3), owner.device
+    if rgb.shape[0] != texel_index.shape[0]:
+        raise ValueError(f"{rgb.shape[0]} colours for {texel_index.shape[0]} texels")
+    count = torch.tensor([texel_index.shape[0]], dtype=_i32, device=dev)
+    nbytes = L.load().o2345_texture_fill_scratch_bytes(int(N))
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    tex = torch.empty(int(N), int(N), 3, dtype=_f32, device=dev)
+    L.call("o2345_texture_fill", _p(texel_index.contiguous(), _i32), _p(count, _i32), _f(rgb), _p(owner.contiguous(), _i32),
+           int(N), _p(scratch), nbytes, _f(tex), _stream())
+    return tex
+
+
+def transfer_colors(verts, faces, colors, points, nn_index, sample_face):
+    """Colours [n,3] fp32 of a source mesh (verts [nv,3], faces [nf,3], colors [nv,3] fp32) at points [n,3]: each point is
+    projected onto the face of its nearest surface sample (nn_index [n] into sample_face [m]) and the face's vertex
+    colours are interpolated there."""
+    verts, faces, colors = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3), cf32(colors).view(-1, 3)
+    points = cf32(points).view(-1, 3)
+    n, dev = points.shape[0], points.device
+    rgb = torch.empty(n, 3, dtype=_f32, device=dev)
+    if n == 0:
+        return rgb
+    L.call("o2345_transfer_colors", _f(verts), verts.shape[0], _p(faces, _i32), faces.shape[0], _f(colors), _f(points), n,
+           _p(nn_index.contiguous(), _i32), _p(sample_face.contiguous(), _i32), sample_face.shape[0], _f(rgb), _stream())
+    return rgb

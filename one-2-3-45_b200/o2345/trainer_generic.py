@@ -67,14 +67,15 @@ class GenericTrainer(nn.Module):
         return obtain_pyramid_feature_maps(extractor, imgs)
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
-                alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None):
+                alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None,
+                texture_size=None):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
                                  iter_step=iter_step, save_vis=save_vis)
         if mode == 'export_mesh':
             return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution,
-                                         target_faces=target_faces)
+                                         target_faces=target_faces, texture_size=texture_size)
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -197,9 +198,12 @@ class GenericTrainer(nn.Module):
 
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
-    def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None):
+    def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None,
+                         texture_size=None):
         """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
-        after the vertex merge and before mesh.ply is written."""
+        after the vertex merge and before mesh.ply is written.  With texture_size N the final mesh's colours are also baked
+        into an N x N texture (o2345/mesh_texture.py): the result gains uv [F,3,2] and texture uint8 [N,N,3]; mesh.ply is
+        written as without it."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
         if self.num_lods > 1:
             # the lod-1 mesh is coloured with the lod-0 feature maps, as in the reference (:959-978)
@@ -211,7 +215,8 @@ class GenericTrainer(nn.Module):
                 conditional_valid_mask_volume=cond1['valid_mask_volume_scale1'], feature_maps=fmaps, color_maps=imgs,
                 w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
                 rendering_network=self.rendering_network_lod1, lod=1, threshold=0, query_c2w=sample['query_c2w'],
-                scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces)
+                scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces,
+                texture_size=texture_size)
         return self.validate_colored_mesh(
             density_or_sdf_network=self.sdf_network_lod0,
             func_extract_geometry=self.sdf_renderer_lod0.extract_geometry, resolution=resolution,
@@ -219,7 +224,8 @@ class GenericTrainer(nn.Module):
             conditional_valid_mask_volume=cond['valid_mask_volume_scale0'], feature_maps=fmaps, color_maps=imgs,
             w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
             rendering_network=self.rendering_network_lod0, lod=0, threshold=0, query_c2w=sample['query_c2w'],
-            scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces)
+            scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces,
+                texture_size=texture_size)
 
     @torch.no_grad()
     def validate_colored_mesh(self, density_or_sdf_network, func_extract_geometry, world_space=True, resolution=360,
@@ -227,7 +233,8 @@ class GenericTrainer(nn.Module):
                               feature_maps=None, color_maps=None, w2cs=None, target_candidate_w2cs=None,
                               intrinsics=None, rendering_network=None, rendering_projector=None, query_c2w=None,
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
-                              iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None):
+                              iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None,
+                              texture_size=None, colour_chunk=1 << 20):
         bmin = torch.tensor(bound_min, dtype=torch.float32)
         bmax = torch.tensor(bound_max, dtype=torch.float32)
         vertices, triangles, fields = func_extract_geometry(
@@ -236,9 +243,12 @@ class GenericTrainer(nn.Module):
             occupancy_mask=occupancy_mask)
         renderer = self.sdf_renderer_lod1 if lod == 1 else self.sdf_renderer_lod0
         vt = torch.tensor(vertices).to(conditional_volume)
-        rgb, _ = renderer.blend_points(vt, density_or_sdf_network, rendering_network, conditional_volume,
-                                                     conditional_valid_mask_volume, feature_maps, color_maps, w2cs,
-                                                     intrinsics, img_wh)
+
+        def colour(points):
+            return renderer.blend_points(points, density_or_sdf_network, rendering_network, conditional_volume,
+                                         conditional_valid_mask_volume, feature_maps, color_maps, w2cs, intrinsics, img_wh)[0]
+        rgb = colour(vt)
+        normalised = vertices
         if scale_mat is not None:
             sm = scale_mat.cpu().numpy()
             vertices = vertices * sm[0][0, 0] + sm[0][:3, 3][None]
@@ -250,12 +260,20 @@ class GenericTrainer(nn.Module):
         # trimesh.Trimesh(vertices, triangles, vertex_colors=...) with its default process=True merges coincident vertices
         # before the export (reference :1374-1380).  Marching-cubes vertices can only coincide on lattice points: the renderer
         # listed the vertices that sit on one (on the device), and only those are compared.
-        vertices, triangles, colors = merge_vertices(vertices, triangles, colors,
-                                                     candidates=getattr(renderer, "mc_lattice_candidates", None))
+        # each kept vertex's index into the extraction's arrays rides along with the colours (merge and simplify gather)
+        vertices, triangles, kept = merge_vertices(vertices, triangles, np.arange(len(colors)),
+                                                   candidates=getattr(renderer, "mc_lattice_candidates", None))
         if target_faces is not None:
             from .mesh_simplify import simplify
-            vertices, triangles, colors, _ = simplify(vertices, triangles, colors, target_faces, conditional_volume.device)
+            vertices, triangles, kept, _ = simplify(vertices, triangles, kept, target_faces, conditional_volume.device)
+        colors = colors[kept]
         if self.base_exp_dir is not None:
             os.makedirs(self.base_exp_dir, exist_ok=True)
             write_ply(os.path.join(self.base_exp_dir, 'mesh.ply'), vertices, triangles, colors)
-        return {"vertices": vertices, "triangles": triangles, "colors": colors, "fields": fields}
+        out = {"vertices": vertices, "triangles": triangles, "colors": colors, "fields": fields}
+        if texture_size is not None:
+            # baked in the normalised frame, where blend_points evaluates (the charts only scale with scale_mat)
+            from .mesh_texture import bake
+            chunked = lambda p: torch.cat([colour(c) for c in p.split(colour_chunk)]) if len(p) else p
+            out["uv"], out["texture"] = bake(normalised[kept], triangles, texture_size, chunked, conditional_volume.device)
+        return out

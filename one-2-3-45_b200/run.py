@@ -1,5 +1,5 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--target_faces N] [--output_format .ply]`
+[--mesh_resolution R] [--target_faces N] [--texture_size N] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -13,6 +13,9 @@ the EMA shadow (`model_ema.*`, reference ldm/modules/ema.py:14-21 + ddpm.py:180-
 attached and takes `cond_stage_model.*`; a file that lacks what the sampler needs is refused.  `--output_format .obj/.glb`
 follow reference utils/utils.py:31-45 (o2345/mesh_io.py).  `--target_faces N` (not in the reference) simplifies the
 mesh to N faces on the GPU before mesh.ply is written (o2345/mesh_simplify.py); .obj / .glb are converted from that mesh.
+`--texture_size N` (not in the reference; .obj or .glb only) bakes the reconstruction's colours into an N x N texture on
+the GPU (o2345/mesh_texture.py) and writes mesh.glb, or mesh.obj + mesh.mtl + mesh_albedo.png, textured; mesh.ply is
+written as without it.
 
 Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
 calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
@@ -51,6 +54,8 @@ def parse_args(argv=None):
     ap.add_argument('--output_format', type=str, default=".ply", help='Output format: .ply, .obj, .glb')
     ap.add_argument('--target_faces', type=int, default=None,
                     help='simplify the mesh to this many faces (quadric edge collapse; default: the full marching-cubes mesh)')
+    ap.add_argument('--texture_size', type=int, default=None,
+                    help='bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output only)')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -61,6 +66,12 @@ def parse_args(argv=None):
     args = ap.parse_args(argv)
     if args.target_faces is not None and args.target_faces < 0:
         ap.error("--target_faces must be >= 0")
+    if args.texture_size is not None:
+        n = args.texture_size
+        if n < 64 or n > 8192 or n & (n - 1):
+            ap.error("--texture_size must be a power of two in [64, 8192]")
+        if args.output_format not in (".obj", ".glb"):
+            ap.error("--texture_size needs --output_format .obj or .glb")
     return args
 
 
@@ -77,7 +88,13 @@ def plan_inputs(paths, polar_angles):
     return [os.path.join("exp", i) for i in ids], polars
 
 
-def _write_format(shape_dir, output_format):
+def _write_format(shape_dir, output_format, mesh=None):
+    if mesh is not None and "texture" in mesh:
+        from o2345.mesh_io import to_viewer_frame, write_textured
+        v, f, uv = to_viewer_frame(mesh["vertices"], mesh["triangles"], mesh["uv"])
+        mesh_path = os.path.join(shape_dir, f"mesh{output_format}")
+        write_textured(mesh_path, v, f, uv, mesh["texture"])
+        return mesh_path
     mesh_path = os.path.join(shape_dir, "mesh.ply")
     if output_format == ".ply":          # reference run.py:113-118
         pass
@@ -87,6 +104,10 @@ def _write_format(shape_dir, output_format):
         from o2345.mesh_io import convert_mesh_format
         mesh_path = convert_mesh_format(shape_dir, output_format)
     return mesh_path
+
+
+def _texture_kw(args):
+    return {} if args.texture_size is None else {"texture_size": args.texture_size}
 
 
 def main(argv=None):
@@ -129,8 +150,9 @@ def main(argv=None):
         if args.seed is not None:
             torch.cuda.manual_seed(args.seed)
         mesh = image_to_mesh(model, trainer, load_input(args.img_path[0]), polar_angle=polars[0],
-                             resolution=args.mesh_resolution, exp_dir=shape_dir, target_faces=args.target_faces)
-        mesh_path = _write_format(shape_dir, args.output_format)
+                             resolution=args.mesh_resolution, exp_dir=shape_dir, target_faces=args.target_faces,
+                             **_texture_kw(args))
+        mesh_path = _write_format(shape_dir, args.output_format, mesh)
         print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", mesh_path)
         return mesh_path
@@ -141,8 +163,9 @@ def main(argv=None):
     paths = []
     for i, mesh in images_to_meshes(model, trainer, [load_input(args.img_path[i]) for i in mine], [polars[i] for i in mine],
                                     seed=0 if args.seed is None else args.seed, resolution=args.mesh_resolution,
-                                    exp_dirs=[shape_dirs[i] for i in mine], indices=mine, target_faces=args.target_faces):
-        paths.append(_write_format(shape_dirs[i], args.output_format))
+                                    exp_dirs=[shape_dirs[i] for i in mine], indices=mine, target_faces=args.target_faces,
+                                    **_texture_kw(args)):
+        paths.append(_write_format(shape_dirs[i], args.output_format, mesh))
         print(f"{args.img_path[i]}: {len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", paths[-1])
     if world > 1:

@@ -6,7 +6,13 @@ Reads .ply (as run.py writes it) or .obj, welds coincident vertices first (mesh_
 one vertex per face corner would otherwise be all boundary, and boundary vertices are never removed), reduces it to
 --target_faces or one fewer faces by quadric-driven half-edge collapse and writes .ply, .obj or .glb by the output's
 extension, in the input's own coordinates.  Every output vertex is an input vertex with its colour.  Prints the face and
-vertex counts before and after and the number of rounds."""
+vertex counts before and after and the number of rounds.
+
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out small.glb --target_faces 5000 --texture_size 2048
+
+--texture_size N (.glb or .obj output) also bakes the welded input's vertex colours into an N x N texture of the
+simplified mesh (o2345/mesh_texture.py: each texel takes the colour of the input surface at its nearest point) and
+writes it textured: .glb with the texture embedded, .obj beside <stem>.mtl and <stem>_albedo.png."""
 from __future__ import annotations
 
 import argparse
@@ -19,6 +25,7 @@ if HERE not in sys.path:
 
 INPUTS = (".ply", ".obj")
 OUTPUTS = (".ply", ".obj", ".glb")
+TEXTURED = (".obj", ".glb")
 
 
 def parse_args(argv=None):
@@ -26,6 +33,8 @@ def parse_args(argv=None):
     ap.add_argument("--in", dest="inp", required=True, help="input mesh (.ply or .obj)")
     ap.add_argument("--out", required=True, help="output mesh (.ply, .obj or .glb)")
     ap.add_argument("--target_faces", type=int, required=True, help="number of faces to reduce to")
+    ap.add_argument("--texture_size", type=int, default=None,
+                    help="bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output)")
     args = ap.parse_args(argv)
     if os.path.splitext(args.inp)[1].lower() not in INPUTS:
         ap.error(f"{args.inp}: unsupported input format (only {', '.join(INPUTS)})")
@@ -33,6 +42,12 @@ def parse_args(argv=None):
         ap.error(f"{args.out}: unsupported output format (only {', '.join(OUTPUTS)})")
     if args.target_faces < 0:
         ap.error("--target_faces must be >= 0")
+    if args.texture_size is not None:
+        n = args.texture_size
+        if n < 64 or n > 8192 or n & (n - 1):
+            ap.error("--texture_size must be a power of two in [64, 8192]")
+        if os.path.splitext(args.out)[1].lower() not in TEXTURED:
+            ap.error(f"--texture_size needs a {' or '.join(TEXTURED)} output")
     return args
 
 
@@ -62,9 +77,17 @@ def main(argv=None):
     print(f"read {args.inp}: {len(v)} vertices, {len(f)} faces")
     v, f, c = mesh_io.merge_vertices(v, f, c)
     print(f"welded: {len(v)} vertices, {len(f)} faces")
+    src = (v, f, c)
     v, f, c, rounds = simplify(v, f, c, args.target_faces)
     print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+    if args.texture_size is not None:
+        from o2345.mesh_texture import bake, transfer_fn
+        uv, tex = bake(v, f, args.texture_size, transfer_fn(*src, texture_size=args.texture_size))
+        print(f"baked a {args.texture_size} x {args.texture_size} texture")
+        mesh_io.write_textured(args.out, v, f, uv, tex)
+        print("wrote", args.out)
+        return v, f, c, rounds, uv, tex
     write_mesh(args.out, v, f, c)
     print("wrote", args.out)
     return v, f, c, rounds
