@@ -30,7 +30,42 @@ void set_error(const char* fmt, ...);
 
 #define O2345_LAUNCH_CHECK() O2345_CUDA(cudaGetLastError())
 
+// returns the status of an o2345 call that failed (its error text is already set)
+#define O2345_TRY(call)                \
+  do {                                 \
+    int rc__ = (call);                 \
+    if (rc__ != O2345_OK) return rc__; \
+  } while (0)
+
 static inline int cdiv(int64_t a, int64_t b) { return (int)((a + b - 1) / b); }
+
+// Hands out 16-byte-aligned blocks of one scratch buffer in the order of the take() calls.  A Carver without a base
+// only measures: after the same calls, `bytes` is the size the buffer needs.  Every offset is a multiple of 16, so each
+// block is as aligned as the base (up to 16 bytes).
+struct Carver {
+  char* base = nullptr;
+  int64_t bytes = 0;
+  template <typename T>
+  T* take(int64_t count) {
+    T* p = base ? reinterpret_cast<T*>(base + bytes) : nullptr;
+    bytes += (count * (int64_t)sizeof(T) + 15) & ~(int64_t)15;
+    return p;
+  }
+};
+
+// ---- scan.cu
+constexpr int kScanBlock = 1024;   // elements per block of an int32 prefix sum
+inline int64_t scan_blocks(int64_t n) { return (n + kScanBlock - 1) / kScanBlock; }
+// vals[0, n) := its exclusive prefix sum in place (three launches); block_sums: scan_blocks(n) int32; *total := the sum
+// (when total is not null).
+int scan_i32(int32_t* vals, int64_t n, int32_t* block_sums, int32_t* total, cudaStream_t stream);
+
+constexpr int kSumChunk = 1024;    // elements per sequential chunk of cumsum_f64_chunked
+inline int64_t sum_chunks(int64_t n) { return (n + kSumChunk - 1) / kSumChunk; }
+// x[0, n) := its inclusive prefix sum in fp64, in a fixed order that does not depend on the launch: sequential inside
+// chunks of kSumChunk elements, then over the chunk totals (three launches).  chunk_tot: sum_chunks(n) + 1 doubles; on
+// return chunk_tot[k] is the sum of the chunks before k and chunk_tot[sum_chunks(n)] the total.
+int cumsum_f64_chunked(double* x, int64_t n, double* chunk_tot, cudaStream_t stream);
 
 // "Once per device" guard for per-function attributes (cudaFuncSetAttribute applies to the CURRENT device only, and a
 // process may drive several devices, e.g. run.py --gpu_idx): need() is true the first time it is called on a device.

@@ -1,11 +1,10 @@
-// Cost-volume build: frustum mask, ordered compaction, fused back-project + variance/mean.
-// Rows B3/B4/B5/B7 of SURVEY.md section 8.
+// Cost-volume build: frustum mask, fused back-project + variance/mean.
+// Rows B3/B4/B5/B7 of SURVEY.md section 8.  The kept voxels are compacted by o2345_compact (scan.cu) in ascending
+// x*D*D + y*D + z order, as reference sparse_sdf_network.py:321-334 keeps them.
 //
 //   frustum_mask_kernel   one thread per lattice voxel, all views: bit-exact restatement of
 //                         reference ops/back_project.py:44-61 (separately rounded mul/add so
 //                         that the CPU oracle reproduces every threshold decision);
-//   compact_*             ascending-order stream compaction (kept-voxel order = ascending
-//                         x*D*D + y*D + z, reference sparse_sdf_network.py:321-334);
 //   costvol_gather_kernel four threads per kept voxel, each owning 4 of the 16 channels:
 //                         per view one projection, four 16-byte taps from the channel-last
 //                         feature map, running sum / sum of squares; the [Nv,V,16] tensor of
@@ -62,82 +61,6 @@ __global__ void frustum_mask_kernel(const float* __restrict__ proj, int V, const
     if (project(sP + 12 * v, wx, wy, wz, size_w1, size_h1).vis) m |= (1u << v);
   bits[lin] = m;
   keep[lin] = __popc(m) > min_views ? 1 : 0;
-}
-
-// ---------------------------------------------------------------------------------------
-// ordered compaction, 1024 elements per block
-// ---------------------------------------------------------------------------------------
-constexpr int CB = 1024;
-
-__global__ void compact_count_kernel(const uint8_t* __restrict__ flags, int64_t n, int32_t* __restrict__ block_sums) {
-  int64_t i = (int64_t)blockIdx.x * CB + threadIdx.x;
-  int f = (i < n && flags[i]) ? 1 : 0;
-  int c = __syncthreads_count(f);
-  if (threadIdx.x == 0) block_sums[blockIdx.x] = c;
-}
-
-// single block: exclusive scan of block_sums[nb] in place, total -> *count
-__global__ void compact_scan_kernel(int32_t* __restrict__ block_sums, int nb, int32_t* __restrict__ count) {
-  __shared__ int32_t warp_tot[32];
-  __shared__ int32_t carry;
-  if (threadIdx.x == 0) carry = 0;
-  __syncthreads();
-  for (int base = 0; base < nb; base += CB) {
-    int i = base + threadIdx.x;
-    int v = i < nb ? block_sums[i] : 0;
-    int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-    int s = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int t = __shfl_up_sync(0xffffffffu, s, o);
-      if (lane >= o) s += t;
-    }
-    if (lane == 31) warp_tot[w] = s;
-    __syncthreads();
-    if (w == 0) {
-      int t = warp_tot[lane];
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        int u = __shfl_up_sync(0xffffffffu, t, o);
-        if (lane >= o) t += u;
-      }
-      warp_tot[lane] = t;
-    }
-    __syncthreads();
-    int excl = s - v + (w > 0 ? warp_tot[w - 1] : 0) + carry;
-    if (i < nb) block_sums[i] = excl;
-    __syncthreads();
-    if (threadIdx.x == CB - 1) carry = excl + v;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0) *count = carry;
-}
-
-__global__ void compact_scatter_kernel(const uint8_t* __restrict__ flags, int64_t n,
-                                       const int32_t* __restrict__ block_offs, int32_t* __restrict__ rows,
-                                       int32_t* __restrict__ index) {
-  __shared__ int32_t warp_tot[32];
-  int64_t i = (int64_t)blockIdx.x * CB + threadIdx.x;
-  int f = (i < n && flags[i]) ? 1 : 0;
-  unsigned b = __ballot_sync(0xffffffffu, f);
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
-  if (lane == 0) warp_tot[w] = __popc(b);
-  __syncthreads();
-  if (w == 0) {
-    int t = warp_tot[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int u = __shfl_up_sync(0xffffffffu, t, o);
-      if (lane >= o) t += u;
-    }
-    warp_tot[lane] = t;
-  }
-  __syncthreads();
-  int pos = block_offs[blockIdx.x] + (w > 0 ? warp_tot[w - 1] : 0) + __popc(b & ((1u << lane) - 1u));
-  if (i < n) {
-    if (f) rows[pos] = (int32_t)i;
-    if (index) index[i] = f ? pos : -1;
-  }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -353,21 +276,6 @@ extern "C" int o2345_frustum_mask(const float* proj, int V, const float* origin,
   int64_t n = (int64_t)D * D * D;
   frustum_mask_kernel<<<cdiv(n, 256), 256, V * 12 * sizeof(float), (cudaStream_t)stream>>>(
       proj, V, origin, voxel_size, D, (float)(sizeW - 1), (float)(sizeH - 1), min_views, mask_bits, keep);
-  O2345_LAUNCH_CHECK();
-  return O2345_OK;
-}
-
-extern "C" int64_t o2345_compact_scratch_ints(int64_t n) { return (n + CB - 1) / CB + 1; }
-
-extern "C" int o2345_compact(const uint8_t* flags, int64_t n, int32_t* rows, int32_t* index, int32_t* count,
-                             int32_t* scratch, o2345_stream_t stream) {
-  O2345_CHECK_ARG(flags && rows && count && scratch, "null pointer");
-  O2345_CHECK_ARG(n > 0 && n < ((int64_t)1 << 31), "element count out of range");
-  int nb = cdiv(n, CB);
-  cudaStream_t st = (cudaStream_t)stream;
-  compact_count_kernel<<<nb, CB, 0, st>>>(flags, n, scratch);
-  compact_scan_kernel<<<1, CB, 0, st>>>(scratch, nb, count);
-  compact_scatter_kernel<<<nb, CB, 0, st>>>(flags, n, scratch, rows, index);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

@@ -4,7 +4,7 @@
 //
 //   classify   one thread per lattice point: the 8-corner case index of the cell it anchors,
 //              and one flag per owned lattice edge (+x,+y,+z) whose end points straddle iso;
-//   compact    (costvol.cu) -> shared vertex ids, one per crossing edge, ascending edge order;
+//   compact    (o2345_compact) -> shared vertex ids, one per crossing edge, ascending edge order;
 //   emit       vertices by linear interpolation in float64 index units (PyMCubes semantics),
 //              triangles through the generated case table (o2345/mc_tables.py).
 #include "common.cuh"
@@ -60,47 +60,6 @@ __global__ void mc_tri_counts_kernel(const uint8_t* __restrict__ cases, const in
   counts[i] = i < *count ? n_tri[cases[cells[i]]] : 0;
 }
 
-// exclusive scan of int32 values, same three-phase scheme as the flag compaction
-constexpr int SB = 1024;
-__global__ void scan_block_kernel(int32_t* __restrict__ vals, int64_t n, int32_t* __restrict__ block_sums) {
-  __shared__ int32_t warp_tot[32];
-  int64_t i = (int64_t)blockIdx.x * SB + threadIdx.x;
-  int v = i < n ? vals[i] : 0;
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5, s = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, s, o);
-    if (lane >= o) s += t;
-  }
-  if (lane == 31) warp_tot[w] = s;
-  __syncthreads();
-  if (w == 0) {
-    int t = warp_tot[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int q = __shfl_up_sync(0xffffffffu, t, o);
-      if (lane >= o) t += q;
-    }
-    warp_tot[lane] = t;
-  }
-  __syncthreads();
-  int excl = s - v + (w > 0 ? warp_tot[w - 1] : 0);
-  if (i < n) vals[i] = excl;
-  if (threadIdx.x == SB - 1) block_sums[blockIdx.x] = excl + v;
-}
-__global__ void scan_tops_kernel(int32_t* __restrict__ block_sums, int nb, int32_t* __restrict__ total) {
-  // nb is small (<= a few thousand): serial scan by one thread keeps this trivially correct
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    int run = 0;
-    for (int i = 0; i < nb; ++i) { int v = block_sums[i]; block_sums[i] = run; run += v; }
-    *total = run;
-  }
-}
-__global__ void scan_add_kernel(int32_t* __restrict__ vals, int64_t n, const int32_t* __restrict__ block_sums) {
-  int64_t i = (int64_t)blockIdx.x * SB + threadIdx.x;
-  if (i < n) vals[i] += block_sums[blockIdx.x];
-}
-
 __global__ void mc_triangles_kernel(const uint8_t* __restrict__ cases, int R, const int32_t* __restrict__ cells,
                                     const int32_t* __restrict__ count, const int32_t* __restrict__ tri_offs,
                                     const int8_t* __restrict__ tri_table, const uint8_t* __restrict__ n_tri,
@@ -147,21 +106,15 @@ extern "C" int o2345_mc_vertices(const float* u, int R, float iso, const int32_t
   return O2345_OK;
 }
 
-extern "C" int64_t o2345_scan_scratch_ints(int64_t n) { return (n + SB - 1) / SB + 1; }
-
 extern "C" int o2345_mc_tri_offsets(const uint8_t* cases, const int32_t* cells, const int32_t* count,
                                     int64_t max_cells, const uint8_t* n_tri_table, int32_t* offsets,
                                     int32_t* total, int32_t* scratch, o2345_stream_t stream) {
   O2345_CHECK_ARG(cases && cells && count && n_tri_table && offsets && total && scratch, "null pointer");
   if (max_cells == 0) return O2345_OK;
   cudaStream_t st = (cudaStream_t)stream;
-  int nb = cdiv(max_cells, SB);
   mc_tri_counts_kernel<<<cdiv(max_cells, 256), 256, 0, st>>>(cases, cells, count, n_tri_table, offsets, max_cells);
-  scan_block_kernel<<<nb, SB, 0, st>>>(offsets, max_cells, scratch);
-  scan_tops_kernel<<<1, 32, 0, st>>>(scratch, nb, total);
-  scan_add_kernel<<<nb, SB, 0, st>>>(offsets, max_cells, scratch);
   O2345_LAUNCH_CHECK();
-  return O2345_OK;
+  return scan_i32(offsets, max_cells, scratch, total, st);
 }
 
 extern "C" int o2345_mc_triangles(const uint8_t* cases, int R, const int32_t* cells, const int32_t* count,

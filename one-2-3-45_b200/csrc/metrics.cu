@@ -1,8 +1,8 @@
 // Mesh scoring (o2345/mesh_metrics.py, eval_mesh.py): area-uniform surface samples and an exact fp32 nearest neighbour.
 //
 //   surface sample  face weights = twice the area in fp64 (one thread per face), cumulative sums in a fixed order
-//                   (sequential inside chunks of 1024 faces, then over the chunk totals), one thread per sample: three
-//                   splitmix64 uniforms, an upper-bound search of the CDF, the barycentric point in fp64 rounded once;
+//                   (cumsum_f64_chunked, scan.cu), one thread per sample: three splitmix64 uniforms, an upper-bound search
+//                   of the CDF, the barycentric point in fp64 rounded once;
 //   nearest         uniform grid of cubic cells over the reference points (bbox reduction, count, scan, scatter), one
 //                   thread per query visiting rows of cells ring by ring around it until a conservative lower bound on
 //                   the distance of every unvisited cell exceeds the best distance found.
@@ -10,13 +10,11 @@
 // Every floating-point operation is an explicit round-to-nearest intrinsic in the order oracle/metrics_oracle.py repeats
 // with numpy (no FMA contraction), so samples, neighbour indices and squared distances are bit-identical to the oracle
 // and do not depend on thread scheduling (ties go to the lower reference index).
-#include "common.cuh"
+#include "mesh_common.cuh"
 
 namespace o2345 {
 namespace {
 
-constexpr int kChunk = 1024;        // faces per sequential CDF chunk (the oracle restates this chunking)
-constexpr int kSB = 1024;           // elements per block of the cell-count scan
 constexpr int kMaxSide = 256;       // cells per grid axis at most: 2^24 cells, 64 MiB of cell offsets
 constexpr int kPtsPerCell = 4;      // target points per occupied cell of a surface: side ~ sqrt(n_ref / 4)
 constexpr float kCellSlack = 1e-3f; // cells: bound on the rounding of a coordinate's cell position (binning and bound)
@@ -40,53 +38,14 @@ __global__ void face_weights_kernel(const float* __restrict__ verts, int64_t nv,
                                     double* __restrict__ cdf) {
   int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= nf) return;
-  int i[3];
-  bool ok = true;
-#pragma unroll
-  for (int k = 0; k < 3; ++k) i[k] = __ldg(faces + 3 * t + k), ok = ok && i[k] >= 0 && i[k] < nv;
+  int i[3] = {__ldg(faces + 3 * t), __ldg(faces + 3 * t + 1), __ldg(faces + 3 * t + 2)};
   double w = 0.0;
-  if (ok) {
-    double e1[3], e2[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      double a = (double)__ldg(verts + 3 * (int64_t)i[0] + c);
-      e1[c] = __dsub_rn((double)__ldg(verts + 3 * (int64_t)i[1] + c), a);
-      e2[c] = __dsub_rn((double)__ldg(verts + 3 * (int64_t)i[2] + c), a);
-    }
-    double cx = __dsub_rn(__dmul_rn(e1[1], e2[2]), __dmul_rn(e1[2], e2[1]));
-    double cy = __dsub_rn(__dmul_rn(e1[2], e2[0]), __dmul_rn(e1[0], e2[2]));
-    double cz = __dsub_rn(__dmul_rn(e1[0], e2[1]), __dmul_rn(e1[1], e2[0]));
-    w = __dsqrt_rn(__dadd_rn(__dadd_rn(__dmul_rn(cx, cx), __dmul_rn(cy, cy)), __dmul_rn(cz, cz)));
+  if (face_ok(i, nv)) {
+    D3 n = cross3(vert(verts, i[0]), vert(verts, i[1]), vert(verts, i[2]));
+    w = __dsqrt_rn(dot3(n, n));
     if (!isfinite(w)) w = 0.0;
   }
   cdf[t] = w;
-}
-
-// one thread per chunk: in-place sequential cumulative sum of the chunk, its total -> tot[chunk]
-__global__ void chunk_scan_kernel(double* __restrict__ cdf, int64_t nf, double* __restrict__ tot, int64_t nchunks) {
-  int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= nchunks) return;
-  int64_t a = k * kChunk, b = min(a + kChunk, nf);
-  double run = 0.0;
-#pragma unroll 8
-  for (int64_t t = a; t < b; ++t) run = __dadd_rn(run, cdf[t]), cdf[t] = run;
-  tot[k] = run;
-}
-
-// one thread: tot[k] := sum of the totals of chunks 0 .. k-1 (sequential), tot[nchunks] := the total
-__global__ void chunk_offsets_kernel(double* __restrict__ tot, int64_t nchunks) {
-  double run = 0.0;
-  for (int64_t k = 0; k < nchunks; ++k) {
-    double v = tot[k];
-    tot[k] = run;
-    run = __dadd_rn(run, v);
-  }
-  tot[nchunks] = run;
-}
-
-__global__ void chunk_add_kernel(double* __restrict__ cdf, int64_t nf, const double* __restrict__ off) {
-  int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t < nf) cdf[t] = __dadd_rn(cdf[t], off[t / kChunk]);
 }
 
 __global__ void sample_kernel(const float* __restrict__ verts, const int32_t* __restrict__ faces, const double* __restrict__ cdf,
@@ -200,57 +159,6 @@ __global__ void bin_kernel(const float* __restrict__ ref, int64_t n, const uint3
   rank[i] = atomicAdd(counts + id, 1);
 }
 
-// block-wide exclusive scan of one int per thread (blockDim.x == kSB); *total := the block's sum
-__device__ __forceinline__ int block_exclusive_scan(int v, int& total) {
-  __shared__ int warp_tot[32];
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5, s = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, s, o);
-    if (lane >= o) s += t;
-  }
-  if (lane == 31) warp_tot[w] = s;
-  __syncthreads();
-  if (w == 0) {
-    int t = warp_tot[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int q = __shfl_up_sync(0xffffffffu, t, o);
-      if (lane >= o) t += q;
-    }
-    warp_tot[lane] = t;
-  }
-  __syncthreads();
-  int excl = s - v + (w > 0 ? warp_tot[w - 1] : 0);
-  total = warp_tot[31];
-  __syncthreads();
-  return excl;
-}
-
-__global__ void __launch_bounds__(kSB) scan_block_kernel(int32_t* __restrict__ vals, int64_t n, int32_t* __restrict__ block_sums) {
-  int64_t i = (int64_t)blockIdx.x * kSB + threadIdx.x;
-  int v = i < n ? vals[i] : 0, total;
-  int excl = block_exclusive_scan(v, total);
-  if (i < n) vals[i] = excl;
-  if (threadIdx.x == 0) block_sums[blockIdx.x] = total;
-}
-
-// one block: exclusive scan of the nb block sums in place, tile by tile
-__global__ void __launch_bounds__(kSB) scan_tops_kernel(int32_t* __restrict__ block_sums, int nb) {
-  int carry = 0;
-  for (int base = 0; base < nb; base += kSB) {
-    int i = base + threadIdx.x, v = i < nb ? block_sums[i] : 0, total;
-    int excl = block_exclusive_scan(v, total);
-    if (i < nb) block_sums[i] = carry + excl;
-    carry += total;
-  }
-}
-
-__global__ void scan_add_kernel(int32_t* __restrict__ vals, int64_t n, const int32_t* __restrict__ block_sums) {
-  int64_t i = (int64_t)blockIdx.x * kSB + threadIdx.x;
-  if (i < n) vals[i] += block_sums[blockIdx.x];
-}
-
 // sorted[start[cell] + rank] = (x, y, z, index bits): the points of a cell, and of a row of cells along x, are contiguous
 __global__ void scatter_kernel(const float* __restrict__ ref, int64_t n, const int32_t* __restrict__ start,
                                const int32_t* __restrict__ cell, const int32_t* __restrict__ rank, float4* __restrict__ sorted) {
@@ -334,29 +242,27 @@ __global__ void nearest_kernel(const float4* __restrict__ sorted, const int32_t*
   index[i] = bi == INT32_MAX ? -1 : bi;
 }
 
-struct NNLayout {
-  int side;
-  int64_t cells, nb, bytes;
-  int64_t off_sorted, off_start, off_sums, off_cell, off_rank, off_keys;
+// The scratch of o2345_surface_sample: the CDF, then the chunk offsets and the total.
+struct SampleScratch {
+  int64_t nf;
+  Carver c;
+  double* cdf = c.take<double>(nf);
+  double* tot = c.take<double>(sum_chunks(nf) + 1);
 };
 
-int64_t align16(int64_t x) { return (x + 15) & ~(int64_t)15; }
-
-NNLayout nn_layout(int64_t n_ref) {
-  NNLayout L;
-  L.side = grid_side(n_ref);
-  L.cells = (int64_t)L.side * L.side * L.side;
-  L.nb = (L.cells + 1 + kSB - 1) / kSB;
-  int64_t o = 0;
-  L.off_sorted = o, o = align16(o + 16 * n_ref);
-  L.off_start = o, o = align16(o + 4 * (L.cells + 1));
-  L.off_sums = o, o = align16(o + 4 * L.nb);
-  L.off_cell = o, o = align16(o + 4 * n_ref);
-  L.off_rank = o, o = align16(o + 4 * n_ref);
-  L.off_keys = o, o = align16(o + 4 * 6);
-  L.bytes = o;
-  return L;
-}
+// The scratch of o2345_nearest, carved in this order (a Carver without a base only measures it).
+struct NNScratch {
+  int64_t n_ref;
+  Carver c;
+  int side = grid_side(n_ref);
+  int64_t cells = (int64_t)side * side * side;
+  float4* sorted = c.take<float4>(n_ref);
+  int32_t* start = c.take<int32_t>(cells + 1);
+  int32_t* sums = c.take<int32_t>(scan_blocks(cells + 1));
+  int32_t* cell = c.take<int32_t>(n_ref);
+  int32_t* rank = c.take<int32_t>(n_ref);
+  uint32_t* keys = c.take<uint32_t>(6);
+};
 
 }  // namespace
 }  // namespace o2345
@@ -365,7 +271,7 @@ using namespace o2345;
 
 extern "C" int64_t o2345_surface_sample_scratch_bytes(int64_t nf) {
   if (nf < 1) return -1;
-  return 8 * (nf + (nf + kChunk - 1) / kChunk + 1);
+  return SampleScratch{nf, {}}.c.bytes;
 }
 
 extern "C" int o2345_surface_sample(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int64_t n, uint64_t seed,
@@ -377,32 +283,25 @@ extern "C" int o2345_surface_sample(const float* verts, int64_t nv, const int32_
                   "scratch smaller than o2345_surface_sample_scratch_bytes");
   O2345_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
-  int64_t nchunks = (nf + kChunk - 1) / kChunk;
-  double* cdf = (double*)scratch;
-  double* tot = cdf + nf;
-  face_weights_kernel<<<cdiv(nf, 256), 256, 0, s>>>(verts, nv, faces, nf, cdf);
+  SampleScratch S{nf, {(char*)scratch}};
+  face_weights_kernel<<<cdiv(nf, 256), 256, 0, s>>>(verts, nv, faces, nf, S.cdf);
   O2345_LAUNCH_CHECK();
-  chunk_scan_kernel<<<cdiv(nchunks, 64), 64, 0, s>>>(cdf, nf, tot, nchunks);
-  O2345_LAUNCH_CHECK();
-  chunk_offsets_kernel<<<1, 1, 0, s>>>(tot, nchunks);
-  O2345_LAUNCH_CHECK();
-  chunk_add_kernel<<<cdiv(nf, 256), 256, 0, s>>>(cdf, nf, tot);
-  O2345_LAUNCH_CHECK();
+  O2345_TRY(cumsum_f64_chunked(S.cdf, nf, S.tot, s));
   double total = 0.0;   // the one host synchronisation: a surface without area has nothing to sample
-  O2345_CUDA(cudaMemcpyAsync(&total, tot + nchunks, sizeof(double), cudaMemcpyDeviceToHost, s));
+  O2345_CUDA(cudaMemcpyAsync(&total, S.tot + sum_chunks(nf), sizeof(double), cudaMemcpyDeviceToHost, s));
   O2345_CUDA(cudaStreamSynchronize(s));
   if (!(total > 0.0)) {
     set_error("%s: the faces have no area (every face is degenerate or has an index outside [0, nv))", __func__);
     return O2345_EINVAL;
   }
-  sample_kernel<<<cdiv(n, 256), 256, 0, s>>>(verts, faces, cdf, nf, total, n, seed, pts, face_id);
+  sample_kernel<<<cdiv(n, 256), 256, 0, s>>>(verts, faces, S.cdf, nf, total, n, seed, pts, face_id);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }
 
 extern "C" int64_t o2345_nn_scratch_bytes(int64_t n_ref, int64_t n_query) {
   if (n_ref < 1 || n_ref > INT32_MAX - 1 || n_query < 1 || n_query > INT32_MAX) return -1;
-  return nn_layout(n_ref).bytes;
+  return NNScratch{n_ref, {}}.c.bytes;
 }
 
 extern "C" int o2345_nearest(const float* ref, int64_t n_ref, const float* query, int64_t n_query, void* scratch,
@@ -413,30 +312,18 @@ extern "C" int o2345_nearest(const float* ref, int64_t n_ref, const float* query
   O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_nn_scratch_bytes(n_ref, n_query), "scratch smaller than o2345_nn_scratch_bytes");
   O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
-  NNLayout L = nn_layout(n_ref);
-  char* p = (char*)scratch;
-  auto* sorted = (float4*)(p + L.off_sorted);
-  auto* start = (int32_t*)(p + L.off_start);
-  auto* sums = (int32_t*)(p + L.off_sums);
-  auto* cell = (int32_t*)(p + L.off_cell);
-  auto* rank = (int32_t*)(p + L.off_rank);
-  auto* keys = (uint32_t*)(p + L.off_keys);
-  O2345_CUDA(cudaMemsetAsync(keys, 0xff, 12, s));
-  O2345_CUDA(cudaMemsetAsync(keys + 3, 0, 12, s));
-  O2345_CUDA(cudaMemsetAsync(start, 0, 4 * (L.cells + 1), s));
-  bbox_kernel<<<min(cdiv(n_ref, 256), sm_count() * 8), 256, 0, s>>>(ref, n_ref, keys);
+  NNScratch S{n_ref, {(char*)scratch}};
+  O2345_CUDA(cudaMemsetAsync(S.keys, 0xff, 12, s));
+  O2345_CUDA(cudaMemsetAsync(S.keys + 3, 0, 12, s));
+  O2345_CUDA(cudaMemsetAsync(S.start, 0, 4 * (S.cells + 1), s));
+  bbox_kernel<<<min(cdiv(n_ref, 256), sm_count() * 8), 256, 0, s>>>(ref, n_ref, S.keys);
   O2345_LAUNCH_CHECK();
-  bin_kernel<<<cdiv(n_ref, 256), 256, 0, s>>>(ref, n_ref, keys, L.side, start, cell, rank);
+  bin_kernel<<<cdiv(n_ref, 256), 256, 0, s>>>(ref, n_ref, S.keys, S.side, S.start, S.cell, S.rank);
   O2345_LAUNCH_CHECK();
-  scan_block_kernel<<<(int)L.nb, kSB, 0, s>>>(start, L.cells + 1, sums);
+  O2345_TRY(scan_i32(S.start, S.cells + 1, S.sums, nullptr, s));
+  scatter_kernel<<<cdiv(n_ref, 256), 256, 0, s>>>(ref, n_ref, S.start, S.cell, S.rank, S.sorted);
   O2345_LAUNCH_CHECK();
-  scan_tops_kernel<<<1, kSB, 0, s>>>(sums, (int)L.nb);
-  O2345_LAUNCH_CHECK();
-  scan_add_kernel<<<(int)L.nb, kSB, 0, s>>>(start, L.cells + 1, sums);
-  O2345_LAUNCH_CHECK();
-  scatter_kernel<<<cdiv(n_ref, 256), 256, 0, s>>>(ref, n_ref, start, cell, rank, sorted);
-  O2345_LAUNCH_CHECK();
-  nearest_kernel<<<cdiv(n_query, 128), 128, 0, s>>>(sorted, start, keys, L.side, query, n_query, dist2, index);
+  nearest_kernel<<<cdiv(n_query, 128), 128, 0, s>>>(S.sorted, S.start, S.keys, S.side, query, n_query, dist2, index);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

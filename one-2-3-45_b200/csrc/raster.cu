@@ -291,6 +291,17 @@ __global__ void raster_resolve_kernel(o2345_raster_mesh m, int V, const float* _
 
 int64_t queue_cap(int64_t nf, int V) { return min((int64_t)V * nf, (int64_t)1 << 22); }
 
+// The scratch of o2345_raster, carved in this order (a Carver without a base only measures it).
+struct Scratch {
+  int64_t npix, nvv, qcap;   // V * H * W, V * nv, queue_cap
+  Carver c;
+  unsigned long long* zbuf = c.take<unsigned long long>(npix);
+  int2* xy = c.take<int2>(nvv);
+  int64_t* queue = c.take<int64_t>(qcap);
+  float* zc = c.take<float>(nvv);
+  int* qcount = c.take<int>(1);
+};
+
 }  // namespace
 }  // namespace o2345
 
@@ -298,7 +309,7 @@ using namespace o2345;
 
 extern "C" int64_t o2345_raster_scratch_bytes(int64_t nv, int64_t nf, int V, int W, int H) {
   if (nv < 0 || nf < 0 || V < 1 || W < 1 || H < 1) return -1;
-  return 8 * (int64_t)V * H * W + 8 * (int64_t)V * nv + 4 * (int64_t)V * nv + 8 * queue_cap(nf, V) + 16;
+  return Scratch{(int64_t)V * H * W, (int64_t)V * nv, queue_cap(nf, V), {}}.c.bytes;
 }
 
 extern "C" void o2345_debug_raster_split(int pixels) { g_split = pixels > 0 ? pixels : 0; }
@@ -317,32 +328,23 @@ extern "C" int o2345_raster(const o2345_raster_mesh* mesh, int V, const float* w
   O2345_CHECK_ARG(!m.face_tex || (m.uvs && m.texels && m.tex_info && m.n_tex >= 1), "face_tex needs uvs, texels and tex_info");
   O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_raster_scratch_bytes(m.nv, m.nf, V, W, H),
                   "scratch smaller than o2345_raster_scratch_bytes");
+  O2345_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");   // 64-bit atomics, int2 stores
   cudaStream_t s = (cudaStream_t)stream;
-  int64_t npix = (int64_t)V * H * W, nvv = (int64_t)V * m.nv, qcap = queue_cap(m.nf, V);
-  char* p = (char*)scratch;
-  auto* zbuf = (unsigned long long*)p;
-  p += 8 * npix;
-  auto* xy = (int2*)p;
-  p += 8 * nvv;
-  auto* queue = (int64_t*)p;
-  p += 8 * qcap;
-  auto* zc = (float*)p;
-  p += 4 * nvv;
-  auto* qcount = (int*)p;
-  O2345_CUDA(cudaMemsetAsync(zbuf, 0xff, 8 * npix, s));
-  O2345_CUDA(cudaMemsetAsync(qcount, 0, sizeof(int), s));
-  raster_vertices_kernel<<<cdiv(nvv, 256), 256, 0, s>>>(m.verts, m.nv, V, w2c, intr, near, xy, zc);
+  Scratch S{(int64_t)V * H * W, (int64_t)V * m.nv, queue_cap(m.nf, V), {(char*)scratch}};
+  O2345_CUDA(cudaMemsetAsync(S.zbuf, 0xff, 8 * S.npix, s));
+  O2345_CUDA(cudaMemsetAsync(S.qcount, 0, sizeof(int), s));
+  raster_vertices_kernel<<<cdiv(S.nvv, 256), 256, 0, s>>>(m.verts, m.nv, V, w2c, intr, near, S.xy, S.zc);
   O2345_LAUNCH_CHECK();
   if (m.nf > 0) {
-    raster_triangles_kernel<<<cdiv((int64_t)V * m.nf, 256), 256, 0, s>>>(m.faces, m.nv, m.nf, V, W, H, xy, zc,
-                                                                         g_split ? g_split : kDefaultSplit, zbuf, queue,
-                                                                         qcap, qcount);
+    raster_triangles_kernel<<<cdiv((int64_t)V * m.nf, 256), 256, 0, s>>>(m.faces, m.nv, m.nf, V, W, H, S.xy, S.zc,
+                                                                         g_split ? g_split : kDefaultSplit, S.zbuf, S.queue,
+                                                                         S.qcap, S.qcount);
     O2345_LAUNCH_CHECK();
-    raster_big_kernel<<<sm_count() * 8, 256, 0, s>>>(m.faces, m.nv, m.nf, W, H, xy, zc, zbuf, queue, qcap, qcount);
+    raster_big_kernel<<<sm_count() * 8, 256, 0, s>>>(m.faces, m.nv, m.nf, W, H, S.xy, S.zc, S.zbuf, S.queue, S.qcap, S.qcount);
     O2345_LAUNCH_CHECK();
   }
-  raster_resolve_kernel<<<cdiv(npix, 256), 256, 0, s>>>(m, V, w2c, W, H, xy, zc, shading, zbuf, color, alpha, depth, normal,
-                                                        tri);
+  raster_resolve_kernel<<<cdiv(S.npix, 256), 256, 0, s>>>(m, V, w2c, W, H, S.xy, S.zc, shading, S.zbuf, color, alpha, depth,
+                                                          normal, tri);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

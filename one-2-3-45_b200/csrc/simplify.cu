@@ -2,7 +2,7 @@
 //
 //   input      one thread per face / vertex: index and finiteness checks, faces with a repeated index dropped (ordered
 //              compaction, o2345_compact);
-//   per round  vertex -> face adjacency (degree count, scan, scatter, per-vertex sort by face index), then one thread per
+//   per round  vertex -> face adjacency (degree count, scan_i32, scatter, per-vertex sort by face index), then one thread per
 //              vertex: locks and valence; the vertex quadrics (first round only, summed in ascending face order); the
 //              proposal of every unlocked vertex (its legal neighbour with the least (cost, index)) and its claim, an
 //              atomicMin of the 64-bit key over the closed 1-rings of both ends; acceptance where the key holds every
@@ -14,85 +14,14 @@
 // order.  The count of accepted proposals is read on the host once per round (the loop's only synchronisation).  Every
 // floating-point operation is an explicit round-to-nearest intrinsic in the order oracle/simplify_oracle.py repeats with
 // numpy (no FMA contraction), so the output is bit-identical to the oracle.
-#include "common.cuh"
+#include "mesh_common.cuh"
 
 namespace o2345 {
 namespace {
 
-constexpr int kSB = 1024;                     // elements per block of the degree scan
+constexpr int kSelect = 1024;                 // threads of the k-th key search
 constexpr uint64_t kNone = ~0ull;             // no proposal / no claim
 enum { kErr = 0, kFaces = 1, kAccepted = 2, kAlive = 3, kUsed = 4, kCtr = 8 };
-
-// ----------------------------------------------------------------------------- exclusive scan of int32
-__device__ __forceinline__ int block_exclusive_scan(int v, int& total) {
-  __shared__ int warp_tot[32];
-  int lane = threadIdx.x & 31, w = threadIdx.x >> 5, s = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int t = __shfl_up_sync(0xffffffffu, s, o);
-    if (lane >= o) s += t;
-  }
-  if (lane == 31) warp_tot[w] = s;
-  __syncthreads();
-  if (w == 0) {
-    int t = warp_tot[lane];
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int q = __shfl_up_sync(0xffffffffu, t, o);
-      if (lane >= o) t += q;
-    }
-    warp_tot[lane] = t;
-  }
-  __syncthreads();
-  int excl = s - v + (w > 0 ? warp_tot[w - 1] : 0);
-  total = warp_tot[31];
-  __syncthreads();
-  return excl;
-}
-
-__global__ void __launch_bounds__(kSB) scan_block_kernel(int32_t* __restrict__ vals, int64_t n, int32_t* __restrict__ sums) {
-  int64_t i = (int64_t)blockIdx.x * kSB + threadIdx.x;
-  int v = i < n ? vals[i] : 0, total;
-  int excl = block_exclusive_scan(v, total);
-  if (i < n) vals[i] = excl;
-  if (threadIdx.x == 0) sums[blockIdx.x] = total;
-}
-
-__global__ void __launch_bounds__(kSB) scan_tops_kernel(int32_t* __restrict__ sums, int nb) {
-  int carry = 0;
-  for (int base = 0; base < nb; base += kSB) {
-    int i = base + threadIdx.x, v = i < nb ? sums[i] : 0, total;
-    int excl = block_exclusive_scan(v, total);
-    if (i < nb) sums[i] = carry + excl;
-    carry += total;
-  }
-}
-
-__global__ void scan_add_kernel(int32_t* __restrict__ vals, int64_t n, const int32_t* __restrict__ sums) {
-  int64_t i = (int64_t)blockIdx.x * kSB + threadIdx.x;
-  if (i < n) vals[i] += sums[blockIdx.x];
-}
-
-// ----------------------------------------------------------------------------- geometry, fp64 from the fp32 vertices
-struct D3 {
-  double x, y, z;
-};
-
-__device__ __forceinline__ D3 vert(const float* __restrict__ V, int i) {
-  return {(double)__ldg(V + 3 * (int64_t)i), (double)__ldg(V + 3 * (int64_t)i + 1), (double)__ldg(V + 3 * (int64_t)i + 2)};
-}
-
-// (b - a) x (c - a), as metrics.cu's face weights
-__device__ __forceinline__ D3 cross3(D3 a, D3 b, D3 c) {
-  double e1x = __dsub_rn(b.x, a.x), e1y = __dsub_rn(b.y, a.y), e1z = __dsub_rn(b.z, a.z);
-  double e2x = __dsub_rn(c.x, a.x), e2y = __dsub_rn(c.y, a.y), e2z = __dsub_rn(c.z, a.z);
-  return {__dsub_rn(__dmul_rn(e1y, e2z), __dmul_rn(e1z, e2y)), __dsub_rn(__dmul_rn(e1z, e2x), __dmul_rn(e1x, e2z)),
-          __dsub_rn(__dmul_rn(e1x, e2y), __dmul_rn(e1y, e2x))};
-}
-
-__device__ __forceinline__ double dot3(D3 a, D3 b) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
-}
 
 // the two other corners of face f (in corner order after u)
 __device__ __forceinline__ void others(const int32_t* __restrict__ F, int f, int u, int& a, int& b) {
@@ -107,22 +36,6 @@ __device__ __forceinline__ bool has(const int32_t* __restrict__ F, int f, int x)
 }
 
 // ----------------------------------------------------------------------------- input
-// flags[f] = face f has three distinct indices; err bit 1: an index outside [0, nv), bit 2: a non-finite coordinate
-__global__ void check_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
-                             uint8_t* __restrict__ flags, int32_t* __restrict__ ctr) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nf) {
-    int a = F[3 * i], b = F[3 * i + 1], c = F[3 * i + 2];
-    bool in = a >= 0 && a < nv && b >= 0 && b < nv && c >= 0 && c < nv;
-    if (!in) atomicOr(ctr + kErr, 1);
-    flags[i] = in && a != b && b != c && a != c;
-  }
-  if (i < nv) {
-    for (int k = 0; k < 3; ++k)
-      if (!isfinite(V[3 * i + k])) atomicOr(ctr + kErr, 2);
-  }
-}
-
 // dst[i] = src[rows[i]] (faces)
 __global__ void gather_faces_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ rows, int64_t n,
                                     int32_t* __restrict__ dst) {
@@ -340,14 +253,14 @@ __global__ void accept_kernel(const int32_t* __restrict__ F, const int32_t* __re
 }
 
 // one block: *thresh = the k-th least key of the m accepted proposals (keys are distinct)
-__global__ void __launch_bounds__(kSB) select_kernel(const int32_t* __restrict__ list, int m, const uint64_t* __restrict__ key,
+__global__ void __launch_bounds__(kSelect) select_kernel(const int32_t* __restrict__ list, int m, const uint64_t* __restrict__ key,
                                                      int k, uint64_t* __restrict__ thresh) {
   __shared__ int tot;
   uint64_t lo = 0, hi = kNone;
   while (lo < hi) {
     uint64_t mid = lo + ((hi - lo) >> 1);
     int c = 0;
-    for (int i = threadIdx.x; i < m; i += kSB) c += key[list[i]] <= mid;
+    for (int i = threadIdx.x; i < m; i += kSelect) c += key[list[i]] <= mid;
     if (threadIdx.x == 0) tot = 0;
     __syncthreads();
     atomicAdd(&tot, c);
@@ -399,40 +312,30 @@ __global__ void counts_kernel(const int32_t* __restrict__ ctr, int64_t nf, int r
   out[0] = ctr[kUsed], out[1] = (int32_t)nf, out[2] = rounds;
 }
 
-struct Layout {
-  int64_t nb, bytes;
-  int64_t faces_a, faces_b, flags, acc, locked, rows, cscratch, off, sums, cursor, adj, val, target, remap, Q, key, claim, ctr;
-};
-
-int64_t align16(int64_t x) { return (x + 15) & ~(int64_t)15; }
-
-Layout layout(int64_t nv, int64_t nf) {
-  Layout L;
+// The scratch of o2345_simplify, carved in this order (a Carver without a base only measures it).
+struct Scratch {
+  int64_t nv, nf;
+  Carver c;
   int64_t nmax = nv > nf ? nv : nf;
-  L.nb = (nv + 1 + kSB - 1) / kSB;
-  int64_t o = 0;
-  auto take = [&](int64_t& at, int64_t bytes) { at = o, o = align16(o + bytes); };
-  take(L.Q, 80 * nv);
-  take(L.key, 8 * nv);
-  take(L.claim, 8 * nv);
-  take(L.ctr, 4 * kCtr + 8);            // counters, then the 64-bit selection threshold
-  take(L.faces_a, 12 * nf);
-  take(L.faces_b, 12 * nf);
-  take(L.adj, 12 * nf);
-  take(L.rows, 4 * nmax);
-  take(L.cscratch, 4 * o2345_compact_scratch_ints(nmax));
-  take(L.off, 4 * (nv + 1));
-  take(L.sums, 4 * L.nb);
-  take(L.cursor, 4 * nv);
-  take(L.val, 4 * nv);
-  take(L.target, 4 * nv);
-  take(L.remap, 4 * nv);
-  take(L.flags, nmax);
-  take(L.acc, nv);
-  take(L.locked, nv);
-  L.bytes = o;
-  return L;
-}
+  double* Q = c.take<double>(10 * nv);
+  uint64_t* key = c.take<uint64_t>(nv);
+  uint64_t* claim = c.take<uint64_t>(nv);
+  int32_t* ctr = c.take<int32_t>(kCtr + 2);   // counters, then the 64-bit selection threshold
+  int32_t* faces_a = c.take<int32_t>(3 * nf);
+  int32_t* faces_b = c.take<int32_t>(3 * nf);
+  int32_t* adj = c.take<int32_t>(3 * nf);
+  int32_t* rows = c.take<int32_t>(nmax);
+  int32_t* cscratch = c.take<int32_t>(o2345_compact_scratch_ints(nmax));
+  int32_t* off = c.take<int32_t>(nv + 1);
+  int32_t* sums = c.take<int32_t>(scan_blocks(nv + 1));
+  int32_t* cursor = c.take<int32_t>(nv);
+  int32_t* val = c.take<int32_t>(nv);
+  int32_t* target = c.take<int32_t>(nv);
+  int32_t* remap = c.take<int32_t>(nv);
+  uint8_t* flags = c.take<uint8_t>(nmax);
+  uint8_t* acc = c.take<uint8_t>(nv);
+  uint8_t* locked = c.take<uint8_t>(nv);
+};
 
 }  // namespace
 }  // namespace o2345
@@ -441,7 +344,7 @@ using namespace o2345;
 
 extern "C" int64_t o2345_simplify_scratch_bytes(int64_t nv, int64_t nf) {
   if (nv < 1 || nv > INT32_MAX - 1 || nf < 1 || nf > INT32_MAX / 3) return -1;
-  return layout(nv, nf).bytes;
+  return Scratch{nv, nf, {}}.c.bytes;
 }
 
 extern "C" int o2345_simplify(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int64_t target_faces,
@@ -453,97 +356,64 @@ extern "C" int o2345_simplify(const float* verts, int64_t nv, const int32_t* fac
   O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_simplify_scratch_bytes(nv, nf), "scratch smaller than o2345_simplify_scratch_bytes");
   O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
-  Layout Lo = layout(nv, nf);
-  char* p = (char*)scratch;
-  auto* fa = (int32_t*)(p + Lo.faces_a);
-  auto* fb = (int32_t*)(p + Lo.faces_b);
-  auto* flags = (uint8_t*)(p + Lo.flags);
-  auto* acc = (uint8_t*)(p + Lo.acc);
-  auto* locked = (uint8_t*)(p + Lo.locked);
-  auto* rows = (int32_t*)(p + Lo.rows);
-  auto* cs = (int32_t*)(p + Lo.cscratch);
-  auto* off = (int32_t*)(p + Lo.off);
-  auto* sums = (int32_t*)(p + Lo.sums);
-  auto* cursor = (int32_t*)(p + Lo.cursor);
-  auto* adj = (int32_t*)(p + Lo.adj);
-  auto* val = (int32_t*)(p + Lo.val);
-  auto* target = (int32_t*)(p + Lo.target);
-  auto* remap = (int32_t*)(p + Lo.remap);
-  auto* Q = (double*)(p + Lo.Q);
-  auto* key = (uint64_t*)(p + Lo.key);
-  auto* claim = (uint64_t*)(p + Lo.claim);
-  auto* ctr = (int32_t*)(p + Lo.ctr);
-  auto* thresh = (uint64_t*)(ctr + kCtr);
+  Scratch S{nv, nf, {(char*)scratch}};
+  uint64_t* thresh = (uint64_t*)(S.ctr + kCtr);
   int32_t host[kCtr];
   auto read_counters = [&]() {
-    O2345_CUDA(cudaMemcpyAsync(host, ctr, sizeof(host), cudaMemcpyDeviceToHost, s));
+    O2345_CUDA(cudaMemcpyAsync(host, S.ctr, sizeof(host), cudaMemcpyDeviceToHost, s));
     O2345_CUDA(cudaStreamSynchronize(s));
     return O2345_OK;
   };
-  int rc;
-#define O2345_TRY(x) \
-  if ((rc = (x)) != O2345_OK) return rc
 
-  O2345_CUDA(cudaMemsetAsync(ctr, 0, 4 * kCtr, s));
-  int64_t nmax = nv > nf ? nv : nf;
-  check_kernel<<<cdiv(nmax, 256), 256, 0, s>>>(verts, nv, faces, nf, flags, ctr);
-  O2345_LAUNCH_CHECK();
-  O2345_TRY(o2345_compact(flags, nf, rows, nullptr, ctr + kFaces, cs, stream));
+  O2345_CUDA(cudaMemsetAsync(S.ctr, 0, 4 * kCtr, s));
+  O2345_TRY(mesh_check(verts, nv, faces, nf, S.flags, S.ctr + kErr, s));
+  O2345_TRY(o2345_compact(S.flags, nf, S.rows, nullptr, S.ctr + kFaces, S.cscratch, stream));
   O2345_TRY(read_counters());
-  if (host[kErr] & 1) {
-    set_error("%s: a face index is outside [0, nv)", __func__);
-    return O2345_EINVAL;
-  }
-  if (host[kErr] & 2) {
-    set_error("%s: a vertex coordinate is not finite", __func__);
-    return O2345_EINVAL;
-  }
+  O2345_TRY(mesh_check_status(host[kErr], __func__));
   int64_t F = host[kFaces];
   if (F > 0) {
-    gather_faces_kernel<<<cdiv(F, 256), 256, 0, s>>>(faces, rows, F, fa);
+    gather_faces_kernel<<<cdiv(F, 256), 256, 0, s>>>(faces, S.rows, F, S.faces_a);
     O2345_LAUNCH_CHECK();
   }
-  int32_t *cur = fa, *nxt = fb;
+  int32_t *cur = S.faces_a, *nxt = S.faces_b;
   int rounds = 0;
   const int vb = cdiv(nv, 128);
   while (F > target_faces) {
     const int64_t n3 = 3 * F;
-    O2345_CUDA(cudaMemsetAsync(off, 0, 4 * (nv + 1), s));
-    O2345_CUDA(cudaMemsetAsync(cursor, 0, 4 * nv, s));
-    degree_kernel<<<cdiv(n3, 256), 256, 0, s>>>(cur, n3, off);
-    scan_block_kernel<<<(int)Lo.nb, kSB, 0, s>>>(off, nv + 1, sums);
-    scan_tops_kernel<<<1, kSB, 0, s>>>(sums, (int)Lo.nb);
-    scan_add_kernel<<<(int)Lo.nb, kSB, 0, s>>>(off, nv + 1, sums);
-    fill_kernel<<<cdiv(n3, 256), 256, 0, s>>>(cur, n3, off, cursor, adj);
-    vertex_kernel<<<vb, 128, 0, s>>>(cur, off, adj, (int)nv, locked, val);
-    if (rounds == 0) quadric_kernel<<<vb, 128, 0, s>>>(verts, cur, off, adj, (int)nv, Q);
-    O2345_CUDA(cudaMemsetAsync(claim, 0xff, 8 * nv, s));
-    propose_kernel<<<vb, 128, 0, s>>>(verts, cur, off, adj, locked, val, Q, (int)nv, target, key, claim);
-    accept_kernel<<<vb, 128, 0, s>>>(cur, off, adj, target, key, claim, (int)nv, acc);
+    O2345_CUDA(cudaMemsetAsync(S.off, 0, 4 * (nv + 1), s));
+    O2345_CUDA(cudaMemsetAsync(S.cursor, 0, 4 * nv, s));
+    degree_kernel<<<cdiv(n3, 256), 256, 0, s>>>(cur, n3, S.off);
     O2345_LAUNCH_CHECK();
-    O2345_TRY(o2345_compact(acc, nv, rows, nullptr, ctr + kAccepted, cs, stream));
+    O2345_TRY(scan_i32(S.off, nv + 1, S.sums, nullptr, s));
+    fill_kernel<<<cdiv(n3, 256), 256, 0, s>>>(cur, n3, S.off, S.cursor, S.adj);
+    vertex_kernel<<<vb, 128, 0, s>>>(cur, S.off, S.adj, (int)nv, S.locked, S.val);
+    if (rounds == 0) quadric_kernel<<<vb, 128, 0, s>>>(verts, cur, S.off, S.adj, (int)nv, S.Q);
+    O2345_CUDA(cudaMemsetAsync(S.claim, 0xff, 8 * nv, s));
+    propose_kernel<<<vb, 128, 0, s>>>(verts, cur, S.off, S.adj, S.locked, S.val, S.Q, (int)nv, S.target, S.key, S.claim);
+    accept_kernel<<<vb, 128, 0, s>>>(cur, S.off, S.adj, S.target, S.key, S.claim, (int)nv, S.acc);
+    O2345_LAUNCH_CHECK();
+    O2345_TRY(o2345_compact(S.acc, nv, S.rows, nullptr, S.ctr + kAccepted, S.cscratch, stream));
     O2345_TRY(read_counters());   // the round's one host synchronisation
     const int64_t m = host[kAccepted], k = (F - target_faces + 1) / 2;
     if (m == 0) break;            // no legal collapse is left
     O2345_CUDA(cudaMemsetAsync(thresh, 0xff, 8, s));
-    if (m > k) select_kernel<<<1, kSB, 0, s>>>(rows, (int)m, key, (int)k, thresh);
-    O2345_CUDA(cudaMemsetAsync(flags, 1, F, s));
-    apply_kernel<<<cdiv(m, 128), 128, 0, s>>>(rows, (int)m, key, thresh, target, off, adj, cur, flags, Q);
+    if (m > k) select_kernel<<<1, kSelect, 0, s>>>(S.rows, (int)m, S.key, (int)k, thresh);
+    O2345_CUDA(cudaMemsetAsync(S.flags, 1, F, s));
+    apply_kernel<<<cdiv(m, 128), 128, 0, s>>>(S.rows, (int)m, S.key, thresh, S.target, S.off, S.adj, cur, S.flags, S.Q);
     O2345_LAUNCH_CHECK();
-    O2345_TRY(o2345_compact(flags, F, rows, nullptr, ctr + kAlive, cs, stream));
+    O2345_TRY(o2345_compact(S.flags, F, S.rows, nullptr, S.ctr + kAlive, S.cscratch, stream));
     F -= 2 * (m < k ? m : k);
-    if (F > 0) gather_faces_kernel<<<cdiv(F, 256), 256, 0, s>>>(cur, rows, F, nxt);
+    if (F > 0) gather_faces_kernel<<<cdiv(F, 256), 256, 0, s>>>(cur, S.rows, F, nxt);
     O2345_LAUNCH_CHECK();
     int32_t* t = cur;
     cur = nxt, nxt = t;
     ++rounds;
   }
-  O2345_CUDA(cudaMemsetAsync(flags, 0, nv, s));
-  if (F > 0) mark_kernel<<<cdiv(3 * F, 256), 256, 0, s>>>(cur, 3 * F, flags);
-  O2345_TRY(o2345_compact(flags, nv, vertex_index, remap, ctr + kUsed, cs, stream));
-  if (F > 0) renumber_kernel<<<cdiv(3 * F, 256), 256, 0, s>>>(cur, 3 * F, remap, out_faces);
-  counts_kernel<<<1, 1, 0, s>>>(ctr, F, rounds, out_counts);
+  O2345_CUDA(cudaMemsetAsync(S.flags, 0, nv, s));
+  if (F > 0) mark_kernel<<<cdiv(3 * F, 256), 256, 0, s>>>(cur, 3 * F, S.flags);
+  O2345_TRY(o2345_compact(S.flags, nv, vertex_index, S.remap, S.ctr + kUsed, S.cscratch, stream));
+  if (F > 0) renumber_kernel<<<cdiv(3 * F, 256), 256, 0, s>>>(cur, 3 * F, S.remap, out_faces);
+  counts_kernel<<<1, 1, 0, s>>>(S.ctr, F, rounds, out_counts);
   O2345_LAUNCH_CHECK();
-#undef O2345_TRY
   return O2345_OK;
 }

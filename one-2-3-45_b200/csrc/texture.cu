@@ -3,8 +3,8 @@
 // of the texels no chart owns, and the colour of a point taken from the nearest face of a source mesh.
 //
 //   atlas         one thread per face: the chart (base = the longest edge by fp32 squared length, first on ties; L, d, h in
-//                 fp64 rounded once to fp32) and L * h in fp64; the sum of L * h in a fixed order (sequential inside chunks
-//                 of 1024 faces, then over the chunk totals, as metrics.cu's CDF); rho0 = sqrt(0.5 N^2 / sum) on the host;
+//                 fp64 rounded once to fp32) and L * h in fp64; the sum of L * h in a fixed order (cumsum_f64_chunked, scan.cu:
+//                 sequential inside chunks of 1024 faces, then over the chunk totals); rho0 = sqrt(0.5 N^2 / sum) on the host;
 //                 per trial of the ladder rho_j = rho0 * j / 64 (a binary search over j in [1, 256]): the boxes (one
 //                 thread per face) and next-fit shelf packing in one warp (stable counting sort by height descending, then
 //                 the shelves in sorted order, 32 boxes per step through shuffles); the fit flag is read on the host;
@@ -20,29 +20,15 @@
 // with numpy (no FMA contraction), so every output is bit-identical to the oracle and independent of thread scheduling.
 #include <math.h>
 
-#include "common.cuh"
+#include "mesh_common.cuh"
 
 namespace o2345 {
 namespace {
 
-constexpr int kChunk = 1024;   // faces per sequential chunk of the L * h sum (the oracle restates this chunking)
 constexpr int kPad = 2;        // texels of padding on every side of a chart's box
 constexpr int kMinN = 64, kMaxN = 8192;
 constexpr int kRungs = 256, kRungDen = 64;   // rho_j = rho0 * j / 64, j in [1, 256]
 enum { kErr = 0, kFits = 1, kCtr = 4 };
-
-struct D3 {
-  double x, y, z;
-};
-
-__device__ __forceinline__ D3 sub3(D3 a, D3 b) { return {__dsub_rn(a.x, b.x), __dsub_rn(a.y, b.y), __dsub_rn(a.z, b.z)}; }
-__device__ __forceinline__ double dot3(D3 a, D3 b) {
-  return __dadd_rn(__dadd_rn(__dmul_rn(a.x, b.x), __dmul_rn(a.y, b.y)), __dmul_rn(a.z, b.z));
-}
-
-__device__ __forceinline__ D3 vert(const float* __restrict__ V, int i) {
-  return {(double)__ldg(V + 3 * (int64_t)i), (double)__ldg(V + 3 * (int64_t)i + 1), (double)__ldg(V + 3 * (int64_t)i + 2)};
-}
 
 // The corner that starts the longest edge of the three (v0v1, v1v2, v2v0) by fp32 squared length, the first on ties.
 __device__ __forceinline__ int base_corner(const float* __restrict__ V, const int c[3]) {
@@ -105,27 +91,13 @@ __device__ __forceinline__ void blend3(const Bary& l, const float* A, const floa
 }
 
 // ----------------------------------------------------------------------------- atlas
-// err bit 1: a face index outside [0, nv), bit 2: a non-finite coordinate
-__global__ void check_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
-                             int32_t* __restrict__ ctr) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nf) {
-    int a = F[3 * i], b = F[3 * i + 1], c = F[3 * i + 2];
-    if (!(a >= 0 && a < nv && b >= 0 && b < nv && c >= 0 && c < nv)) atomicOr(ctr + kErr, 1);
-  }
-  if (i < nv) {
-    for (int k = 0; k < 3; ++k)
-      if (!isfinite(V[3 * i + k])) atomicOr(ctr + kErr, 2);
-  }
-}
-
 // chart[f] = (L, d, h, base corner bits), lh[f] = L * h in fp64 (exact: two fp32 factors)
 __global__ void chart_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
                              float4* __restrict__ chart, double* __restrict__ lh) {
   int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (f >= nf) return;
   int c[3] = {F[3 * f], F[3 * f + 1], F[3 * f + 2]};
-  if (!(c[0] >= 0 && c[0] < nv && c[1] >= 0 && c[1] < nv && c[2] >= 0 && c[2] < nv)) {   // refused on the host
+  if (!face_ok(c, nv)) {   // refused on the host
     chart[f] = make_float4(0.f, 0.f, 0.f, 0.f), lh[f] = 0.0;
     return;
   }
@@ -134,8 +106,7 @@ __global__ void chart_kernel(const float* __restrict__ V, int64_t nv, const int3
   D3 e1 = sub3(b, a), e2 = sub3(q, a);
   double L = __dsqrt_rn(dot3(e1, e1)), d = 0.0, h = 0.0;
   if (L > 0.0) {
-    D3 n = {__dsub_rn(__dmul_rn(e1.y, e2.z), __dmul_rn(e1.z, e2.y)), __dsub_rn(__dmul_rn(e1.z, e2.x), __dmul_rn(e1.x, e2.z)),
-            __dsub_rn(__dmul_rn(e1.x, e2.y), __dmul_rn(e1.y, e2.x))};
+    D3 n = cross3(a, b, q);
     d = __ddiv_rn(dot3(e2, e1), L);
     h = __ddiv_rn(__dsqrt_rn(dot3(n, n)), L);
   }
@@ -143,23 +114,6 @@ __global__ void chart_kernel(const float* __restrict__ V, int64_t nv, const int3
   df = fminf(fmaxf(df, 0.f), Lf);   // 0 <= d <= L up to rounding: clamped so the chart stays inside its box
   chart[f] = make_float4(Lf, df, hf, __int_as_float(k0));
   lh[f] = __dmul_rn((double)Lf, (double)hf);
-}
-
-// one thread per chunk: tot[chunk] = sequential sum of the chunk's L * h
-__global__ void chunk_sum_kernel(const double* __restrict__ lh, int64_t nf, double* __restrict__ tot, int64_t nchunks) {
-  int64_t k = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (k >= nchunks) return;
-  int64_t a = k * kChunk, b = min(a + kChunk, nf);
-  double run = 0.0;
-  for (int64_t t = a; t < b; ++t) run = __dadd_rn(run, lh[t]);
-  tot[k] = run;
-}
-
-// one thread: tot[nchunks] = sum of the chunk totals in order
-__global__ void total_kernel(double* __restrict__ tot, int64_t nchunks) {
-  double run = 0.0;
-  for (int64_t k = 0; k < nchunks; ++k) run = __dadd_rn(run, tot[k]);
-  tot[nchunks] = run;
 }
 
 // box side of a chart extent e at scale rho: ceil(e * rho) + 2P (anything wider than N is N + 1: it cannot fit)
@@ -275,26 +229,36 @@ __global__ void owner_kernel(const int32_t* __restrict__ boxes, int N, int32_t* 
   for (int t = threadIdx.x; t < w * h; t += blockDim.x) owner[(int64_t)(y + t / w) * N + x + t % w] = f;
 }
 
-struct AtlasLayout {
-  int64_t chart, lh, tot, order, ctr, bytes;
+// The scratch of o2345_texture_atlas, carved in this order (a Carver without a base only measures it).
+struct AtlasScratch {
+  int64_t nf;
+  Carver c;
+  float4* chart = c.take<float4>(nf);
+  double* lh = c.take<double>(nf);
+  double* tot = c.take<double>(sum_chunks(nf) + 1);
+  int32_t* order = c.take<int32_t>(nf);
+  int32_t* ctr = c.take<int32_t>(kCtr);
 };
 
-int64_t align16(int64_t x) { return (x + 15) & ~(int64_t)15; }
-
-AtlasLayout atlas_layout(int64_t nf) {
-  AtlasLayout L;
-  int64_t o = 0, nchunks = (nf + kChunk - 1) / kChunk;
-  auto take = [&](int64_t& at, int64_t bytes) { at = o, o = align16(o + bytes); };
-  take(L.chart, 16 * nf);
-  take(L.lh, 8 * nf);
-  take(L.tot, 8 * (nchunks + 1));
-  take(L.order, 4 * nf);
-  take(L.ctr, 4 * kCtr);
-  L.bytes = o;
-  return L;
-}
-
 bool valid_size(int N) { return N >= kMinN && N <= kMaxN && (N & (N - 1)) == 0; }
+
+// The scratch of o2345_texel_points: the owned flags and the compaction's scratch.
+struct TexelScratch {
+  int64_t n;
+  Carver c;
+  uint8_t* flags = c.take<uint8_t>(n);
+  int32_t* cscratch = c.take<int32_t>(o2345_compact_scratch_ints(n));
+};
+
+// The scratch of o2345_texture_fill: the push-pull levels N/2 .. 1 (rgb, weight), finest first.
+struct FillScratch {
+  Carver c;
+  float4* lvl[16];
+  int levels = 0;
+  FillScratch(char* base, int N) : c{base} {
+    for (int m = N / 2; m >= 1; m /= 2) lvl[levels++] = c.take<float4>((int64_t)m * m);
+  }
+};
 
 // ----------------------------------------------------------------------------- texel points
 __global__ void owned_kernel(const int32_t* __restrict__ owner, int64_t n, uint8_t* __restrict__ flags) {
@@ -314,7 +278,7 @@ __global__ void texel_points_kernel(const float* __restrict__ V, int64_t nv, con
   texel_face[i] = f;
   int c[3] = {-1, -1, -1};
   if (f >= 0 && f < nf) c[0] = F[3 * (int64_t)f], c[1] = F[3 * (int64_t)f + 1], c[2] = F[3 * (int64_t)f + 2];
-  if (!(c[0] >= 0 && c[0] < nv && c[1] >= 0 && c[1] < nv && c[2] >= 0 && c[2] < nv)) {   // not a face the atlas accepted
+  if (!face_ok(c, nv)) {   // not a face the atlas accepted
     points[3 * i] = points[3 * i + 1] = points[3 * i + 2] = __int_as_float(0x7fc00000);
     return;
   }
@@ -394,7 +358,7 @@ __global__ void transfer_kernel(const float* __restrict__ V, int64_t nv, const i
   int s = nn_index[i], f = s >= 0 && s < n_samples ? sample_face[s] : -1;
   int c[3] = {-1, -1, -1};
   if (f >= 0 && f < nf) c[0] = F[3 * (int64_t)f], c[1] = F[3 * (int64_t)f + 1], c[2] = F[3 * (int64_t)f + 2];
-  if (!(c[0] >= 0 && c[0] < nv && c[1] >= 0 && c[1] < nv && c[2] >= 0 && c[2] < nv)) {
+  if (!face_ok(c, nv)) {
     rgb[3 * i] = rgb[3 * i + 1] = rgb[3 * i + 2] = __int_as_float(0x7fc00000);
     return;
   }
@@ -410,7 +374,7 @@ using namespace o2345;
 
 extern "C" int64_t o2345_texture_atlas_scratch_bytes(int64_t nf) {
   if (nf < 1 || nf > INT32_MAX / 3) return -1;
-  return atlas_layout(nf).bytes;
+  return AtlasScratch{nf, {}}.c.bytes;
 }
 
 extern "C" int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int N, void* scratch,
@@ -423,33 +387,18 @@ extern "C" int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t
                   "scratch smaller than o2345_texture_atlas_scratch_bytes");
   O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
-  AtlasLayout Lo = atlas_layout(nf);
-  char* p = (char*)scratch;
-  auto* chart = (float4*)(p + Lo.chart);
-  auto* lh = (double*)(p + Lo.lh);
-  auto* tot = (double*)(p + Lo.tot);
-  auto* order = (int32_t*)(p + Lo.order);
-  auto* ctr = (int32_t*)(p + Lo.ctr);
-  const int64_t nchunks = (nf + kChunk - 1) / kChunk;
-  O2345_CUDA(cudaMemsetAsync(ctr, 0, 4 * kCtr, s));
-  check_kernel<<<cdiv(nv > nf ? nv : nf, 256), 256, 0, s>>>(verts, nv, faces, nf, ctr);
-  chart_kernel<<<cdiv(nf, 256), 256, 0, s>>>(verts, nv, faces, nf, chart, lh);
-  chunk_sum_kernel<<<cdiv(nchunks, 64), 64, 0, s>>>(lh, nf, tot, nchunks);
-  total_kernel<<<1, 1, 0, s>>>(tot, nchunks);
+  AtlasScratch S{nf, {(char*)scratch}};
+  O2345_CUDA(cudaMemsetAsync(S.ctr, 0, 4 * kCtr, s));
+  O2345_TRY(mesh_check(verts, nv, faces, nf, nullptr, S.ctr + kErr, s));
+  chart_kernel<<<cdiv(nf, 256), 256, 0, s>>>(verts, nv, faces, nf, S.chart, S.lh);
   O2345_LAUNCH_CHECK();
+  O2345_TRY(cumsum_f64_chunked(S.lh, nf, S.tot, s));   // lh becomes its prefix sums: only the total is used
   int32_t err = 0;
   double sum = 0.0;   // host reads: the input checks and the sum, then one fit flag per trial
-  O2345_CUDA(cudaMemcpyAsync(&err, ctr + kErr, 4, cudaMemcpyDeviceToHost, s));
-  O2345_CUDA(cudaMemcpyAsync(&sum, tot + nchunks, 8, cudaMemcpyDeviceToHost, s));
+  O2345_CUDA(cudaMemcpyAsync(&err, S.ctr + kErr, 4, cudaMemcpyDeviceToHost, s));
+  O2345_CUDA(cudaMemcpyAsync(&sum, S.tot + sum_chunks(nf), 8, cudaMemcpyDeviceToHost, s));
   O2345_CUDA(cudaStreamSynchronize(s));
-  if (err & 1) {
-    set_error("%s: a face index is outside [0, nv)", __func__);
-    return O2345_EINVAL;
-  }
-  if (err & 2) {
-    set_error("%s: a vertex coordinate is not finite", __func__);
-    return O2345_EINVAL;
-  }
+  O2345_TRY(mesh_check_status(err, __func__));
   if (!(sum > 0.0)) {
     set_error("%s: the faces have no area", __func__);
     return O2345_EINVAL;
@@ -457,16 +406,15 @@ extern "C" int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t
   const double rho0 = sqrt(0.5 * ((double)N * (double)N) / sum);
   auto rho_of = [&](int j) { return rho0 * (double)j / (double)kRungDen; };
   auto trial = [&](int j, int32_t& fits) {
-    box_kernel<<<cdiv(nf, 256), 256, 0, s>>>(chart, nf, rho_of(j), N, boxes);
-    pack_kernel<<<1, 32, 0, s>>>(boxes, (int)nf, N, order, ctr + kFits);
+    box_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.chart, nf, rho_of(j), N, boxes);
+    pack_kernel<<<1, 32, 0, s>>>(boxes, (int)nf, N, S.order, S.ctr + kFits);
     O2345_LAUNCH_CHECK();
-    O2345_CUDA(cudaMemcpyAsync(&fits, ctr + kFits, 4, cudaMemcpyDeviceToHost, s));
+    O2345_CUDA(cudaMemcpyAsync(&fits, S.ctr + kFits, 4, cudaMemcpyDeviceToHost, s));
     O2345_CUDA(cudaStreamSynchronize(s));
     return O2345_OK;
   };
-  int rc;
   int32_t fits = 0;
-  if ((rc = trial(1, fits)) != O2345_OK) return rc;
+  O2345_TRY(trial(1, fits));
   if (!fits) {
     set_error("%s: %d^2 texels cannot hold %lld charts", __func__, N, (long long)nf);
     return O2345_EINVAL;
@@ -474,14 +422,14 @@ extern "C" int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t
   int lo = 1, hi = kRungs + 1, last = 1;
   while (hi - lo > 1) {
     int mid = (lo + hi) / 2;
-    if ((rc = trial(mid, fits)) != O2345_OK) return rc;
+    O2345_TRY(trial(mid, fits));
     last = mid;
     if (fits) lo = mid;
     else hi = mid;
   }
-  if (last != lo && (rc = trial(lo, fits)) != O2345_OK) return rc;   // the boxes of the chosen rung
+  if (last != lo) O2345_TRY(trial(lo, fits));   // the boxes of the chosen rung
   const double rho = rho_of(lo);
-  uv_kernel<<<cdiv(nf, 256), 256, 0, s>>>(faces, chart, boxes, nf, rho, N, uv);
+  uv_kernel<<<cdiv(nf, 256), 256, 0, s>>>(faces, S.chart, boxes, nf, rho, N, uv);
   O2345_CUDA(cudaMemsetAsync(owner, 0xff, 4 * (int64_t)N * N, s));
   owner_kernel<<<(unsigned)nf, 128, 0, s>>>(boxes, N, owner);
   O2345_LAUNCH_CHECK();
@@ -492,8 +440,7 @@ extern "C" int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t
 
 extern "C" int64_t o2345_texel_points_scratch_bytes(int N) {
   if (!valid_size(N)) return -1;
-  int64_t n = (int64_t)N * N;
-  return align16(n) + 4 * o2345_compact_scratch_ints(n);
+  return TexelScratch{(int64_t)N * N, {}}.c.bytes;
 }
 
 extern "C" int o2345_texel_points(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
@@ -507,12 +454,10 @@ extern "C" int o2345_texel_points(const float* verts, int64_t nv, const int32_t*
   O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t n = (int64_t)N * N;
-  auto* flags = (uint8_t*)scratch;
-  auto* cs = (int32_t*)((char*)scratch + align16(n));
-  owned_kernel<<<cdiv(n, 256), 256, 0, s>>>(owner, n, flags);
+  TexelScratch S{n, {(char*)scratch}};
+  owned_kernel<<<cdiv(n, 256), 256, 0, s>>>(owner, n, S.flags);
   O2345_LAUNCH_CHECK();
-  int rc = o2345_compact(flags, n, texel_index, nullptr, count, cs, stream);
-  if (rc != O2345_OK) return rc;
+  O2345_TRY(o2345_compact(S.flags, n, texel_index, nullptr, count, S.cscratch, stream));
   texel_points_kernel<<<cdiv(n, 128), 128, 0, s>>>(verts, nv, faces, nf, uv, owner, N, texel_index, count, points, texel_face);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
@@ -520,9 +465,7 @@ extern "C" int o2345_texel_points(const float* verts, int64_t nv, const int32_t*
 
 extern "C" int64_t o2345_texture_fill_scratch_bytes(int N) {
   if (!valid_size(N)) return -1;
-  int64_t b = 0;
-  for (int n = N / 2; n >= 1; n /= 2) b += 16 * (int64_t)n * n;
-  return b;
+  return FillScratch(nullptr, N).c.bytes;
 }
 
 extern "C" int o2345_texture_fill(const int32_t* texel_index, const int32_t* count, const float* rgb, const int32_t* owner,
@@ -533,19 +476,16 @@ extern "C" int o2345_texture_fill(const int32_t* texel_index, const int32_t* cou
   O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
   cudaStream_t s = (cudaStream_t)stream;
   const int64_t n = (int64_t)N * N;
-  float4* lvl[16];
-  int levels = 0;
-  int64_t o = 0;
-  for (int m = N / 2; m >= 1; m /= 2) lvl[levels++] = (float4*)((char*)scratch + o), o += 16 * (int64_t)m * m;
+  FillScratch S((char*)scratch, N);
   O2345_CUDA(cudaMemsetAsync(texture, 0, 12 * n, s));
   scatter_kernel<<<cdiv(n, 256), 256, 0, s>>>(texel_index, count, rgb, texture);
-  for (int l = 0; l < levels; ++l) {   // pull: level l + 1 of the pyramid (N >> (l + 1) texels a side)
+  for (int l = 0; l < S.levels; ++l) {   // pull: level l + 1 of the pyramid (N >> (l + 1) texels a side)
     int m = N >> (l + 1);
-    pull_kernel<<<cdiv((int64_t)m * m, 256), 256, 0, s>>>(l ? lvl[l - 1] : nullptr, texture, owner, m, lvl[l]);
+    pull_kernel<<<cdiv((int64_t)m * m, 256), 256, 0, s>>>(l ? S.lvl[l - 1] : nullptr, texture, owner, m, S.lvl[l]);
   }
-  for (int l = levels - 2; l >= -1; --l) {   // push: coarse to fine, the texture last
+  for (int l = S.levels - 2; l >= -1; --l) {   // push: coarse to fine, the texture last
     int m = N >> (l + 1);
-    push_kernel<<<cdiv((int64_t)m * m, 256), 256, 0, s>>>(l >= 0 ? lvl[l] : nullptr, texture, owner, m, lvl[l + 1]);
+    push_kernel<<<cdiv((int64_t)m * m, 256), 256, 0, s>>>(l >= 0 ? S.lvl[l] : nullptr, texture, owner, m, S.lvl[l + 1]);
   }
   O2345_LAUNCH_CHECK();
   return O2345_OK;

@@ -256,12 +256,13 @@ def test_raster_refuses_bad_arguments_without_a_device():
     assert need > 8 * 64 and lib.o2345_raster_scratch_bytes(-1, 1, 1, 8, 8) == -1
     f = C.c_void_p(fake)
 
-    def call(mesh=good, V=1, W=8, H=8, near=0.1, shading=0, scratch_bytes=need):
-        return lib.o2345_raster(C.byref(mesh) if mesh is not None else None, V, f, f, W, H, near, shading, f, scratch_bytes,
-                                f, f, f, f, f, None)
+    def call(mesh=good, V=1, W=8, H=8, near=0.1, shading=0, scratch=f, scratch_bytes=need):
+        return lib.o2345_raster(C.byref(mesh) if mesh is not None else None, V, f, f, W, H, near, shading, scratch,
+                                scratch_bytes, f, f, f, f, f, None)
     cases = [dict(mesh=None), dict(mesh=_lib.RasterMesh(verts=fake, nv=3, nf=1)), dict(mesh=_lib.RasterMesh(verts=fake, faces=fake, nv=0, nf=1)),
              dict(V=0), dict(W=0), dict(H=20000), dict(near=0.0), dict(shading=2), dict(scratch_bytes=need - 1),
-             dict(mesh=_lib.RasterMesh(verts=fake, faces=fake, face_tex=fake, nv=3, nf=1))]
+             dict(mesh=_lib.RasterMesh(verts=fake, faces=fake, face_tex=fake, nv=3, nf=1)),
+             dict(scratch=C.c_void_p(fake + 4))]
     for i, kw in enumerate(cases):
         assert call(**kw) == -1, (i, _lib.last_error())
         assert "o2345_raster" in _lib.last_error()
