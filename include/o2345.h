@@ -422,7 +422,8 @@ int o2345_layernorm_rows(const void* x, int64_t M, int C, float eps, const float
 int o2345_softmax_rows(const void* s, int64_t rows, int n, void* p, o2345_stream_t stream);
 /* Fused multi-head self-attention (ldm/modules/attention.py:170-193): out[b, n, h*d + j] = softmax(q k^T * scale) v.
  * q, k, v: fp16 [B*N, >= H*d] views with a common row stride ld (e.g. column blocks of a fused qkv projection);
- * d in {40, 64, 80, 160} (64: CLIP ViT-L/14); scores stay on chip (mma.sync m16n8k16, fp32 online softmax). */
+ * d in {40, 64, 80, 160} (64: CLIP ViT-L/14); scores stay on chip (mma.sync m16n8k16, fp32 online softmax).
+ * scale must be positive and finite (O2345_EINVAL otherwise). */
 int o2345_attention_f16(const void* q, const void* k, const void* v, int B, int N, int H, int d, int ld, void* out,
                         int ldo, float scale, o2345_stream_t stream);
 /* y[M,I] = x[:, :I] * gelu(x[:, I:2I]) */

@@ -11,6 +11,8 @@
 // (N^2 exps per head), not tensor-bound, at these sizes.
 #include <cuda_fp16.h>
 
+#include <cmath>
+
 #include "common.cuh"
 #include "mma_sync.cuh"
 
@@ -183,6 +185,8 @@ extern "C" int o2345_attention_f16(const void* q, const void* k, const void* v, 
   O2345_CHECK_ARG(B > 0 && N > 0 && H > 0 && (ld % 8) == 0 && (ldo % 2) == 0, "bad sizes");
   O2345_CHECK_ARG(d == 40 || d == 64 || d == 80 || d == 160, "head dim must be 40, 64, 80 or 160");
   O2345_CHECK_ARG(((uintptr_t)q % 16) == 0 && ((uintptr_t)k % 16) == 0 && ((uintptr_t)v % 16) == 0, "q/k/v must be 16-byte aligned");
+  // the running maximum is taken on the raw scores, with the scale folded into the exponent: right only for scale > 0
+  O2345_CHECK_ARG(scale > 0.f && std::isfinite(scale), "scale must be positive and finite");
   const int nw = N >= 512 ? 8 : 4;               // 128 queries per CTA on long sequences
   dim3 grid(cdiv(N, 16 * nw), B * H);
   float sl2 = scale * 1.4426950408889634f;

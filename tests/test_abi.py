@@ -73,6 +73,14 @@ def test_argument_checks_return_einval_without_touching_the_gpu():
         lambda: lib.o2345_conv3x3_f16(fake, 1, 8, 24, 16, fake, 16, fake, 16, None, None, 0, None),
         # attention head sizes
         lambda: lib.o2345_attention_f16(fake, fake, fake, 1, 16, 2, 48, 96, fake, 96, 1.0, None),
+        # attention scale: the kernel's running maximum is only right for a positive, finite scale
+        lambda: lib.o2345_attention_f16(fake, fake, fake, 1, 16, 2, 40, 240, fake, 80, 0.0, None),
+        lambda: lib.o2345_attention_f16(fake, fake, fake, 1, 16, 2, 40, 240, fake, 80, -1.0, None),
+        lambda: lib.o2345_attention_f16(fake, fake, fake, 1, 16, 2, 40, 240, fake, 80, float("nan"), None),
+        lambda: lib.o2345_attention_f16(fake, fake, fake, 1, 16, 2, 40, 240, fake, 80, float("inf"), None),
+        # softmax rows are at most 1024 long; timestep embeddings have an even width
+        lambda: lib.o2345_softmax_rows(fake, 8, 1025, fake, None),
+        lambda: lib.o2345_timestep_embedding(fake, 2, 321, fake, None),
         # group norm: channels not a multiple of the group count
         lambda: lib.o2345_groupnorm_stats(fake, 1, 16, 40, 32, 1e-5, None, None, fake, fake, fake, None),
         # blend precision

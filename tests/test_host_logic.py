@@ -150,6 +150,29 @@ def test_ddim_iteration_counts():
     assert ddim_iterations(75) == 76 and ddim_iterations(50) == 49 and ddim_iterations(5) == 4
 
 
+def test_ddim_direction_coefficient_stays_positive():
+    """The DDIM update takes sqrt(1 - a_prev - sigma^2) of fp32 schedule values (o2345_cfg_ddim_update).  For the Zero123
+    schedules (5, 50 and 75 steps, eta 0 and 1, the fp32 alphas_cumprod and its fp16 rounding of a `.half()` model) that
+    difference stays positive at every iteration, in fp32 arithmetic and with room for its rounding.  Its smallest value,
+    at the last step with eta = 1, is 6.5e-6 for 5 steps and above 1e-4 for 50 and 75 steps: far above a few fp32 ulps of 1."""
+    from types import SimpleNamespace
+
+    from o2345.ddim import DDIMSampler
+    from oracle import ldm_oracle as LO
+    ac = torch.from_numpy(LO.linear_beta_alphas_cumprod())
+    for a in (ac, ac.half()):
+        for S in (5, 50, 75):
+            for eta in (0.0, 1.0):
+                smp = DDIMSampler(SimpleNamespace(num_timesteps=1000, device=torch.device("cpu"), alphas_cumprod=a))
+                smp.make_schedule(S, ddim_eta=eta, verbose=False)
+                steps = len(smp.ddim_timesteps) - 1
+                ap, sig = smp.ddim_alphas_prev[:steps].numpy(), smp.ddim_sigmas[:steps].numpy()
+                term32 = np.float32(1.0) - ap - sig * sig
+                exact = 1.0 - ap.astype(np.float64) - sig.astype(np.float64) ** 2
+                assert term32.dtype == np.float32 and (term32 > 0).all(), (a.dtype, S, eta, term32.min())
+                assert exact.min() > 64 * 2.0 ** -24, (a.dtype, S, eta, exact.min())
+
+
 def test_upsample_conv_weight_decomposition_is_exact_algebra():
     """nearest 2x + 3x3 conv (pad 1) == four 2x2 convolutions of the low-resolution map with the collapsed kernel rows / columns
     summed (o2345.unet._Packed.conv_up, consumed by o2345_conv_up2x_f16): checked in fp64 on the CPU with torch's own conv2d,
