@@ -373,7 +373,9 @@ void o2345_debug_gemm_model(const float* seven);
 
 /* Diagnostic hook (not part of the data path): when device_buf16 != NULL, CTA (0,0,0) of every following GEMM
  * launch stores clock64() stamps of its phases into device_buf16[0..8] (entry, prologue done, first TMA issued, last TMA
- * issued, first operands landed, last MMA issued, accumulator ready, epilogue done, exit).  NULL switches it off. */
+ * issued, first operands landed, last MMA issued, epilogue start, epilogue done, exit) of its last tile; in a persistent
+ * launch device_buf16[9] also receives the previous tile's "last MMA issued" stamp, so [4] - [9] is the gap between two
+ * tiles' MMAs.  NULL switches it off. */
 void o2345_debug_gemm_trace(long long* device_buf16);
 
 /* Implicit-GEMM 3x3 convolution, stride 1, zero padding 1 (nn.Conv2d(C, N, 3, padding=1) of the UNet ResBlocks and the

@@ -11,13 +11,16 @@
 //   warpgroup 0   one thread is the TMA producer: cp.async.bulk.tensor (SWIZZLE_128B) into a STAGES-deep shared-memory ring
 //                 guarded by full / empty mbarriers;
 //   warpgroups 1-2  each issues wgmma.mma_async m64nBNk16 on its 64 rows of the tile, four per stage, one stage in flight
-//                 while the previous one is released; once the K loop is done the (now idle) operand ring receives the fp32
-//                 accumulator tile, and the same EIGHT warps run the epilogue: warp w owns 32 rows and one of two column
-//                 ranges of the tile; alpha / bias / activation / GEGLU gate -> fp16 -> a shared-memory transpose ->
-//                 coalesced row stores with the residual added.
+//                 while the previous one is released, then runs the epilogue of its 64 rows.
 // MODE selects the epilogue at compile time:
 //   0 staged, no activation   1 staged, GEGLU gate   2 staged, SiLU / GELU / QuickGELU (runtime switch per tile)
-//   3 generic (fp32 output, batched, unaligned N) and SPLIT-K.
+//      Each consumer warpgroup applies alpha / bias / row-group bias / activation / GEGLU gate to its own wgmma fragment
+//      registers, rounds to fp16 and writes them into its private 64-row output half tile in shared memory, where TMA has
+//      already put the residual (loaded during the main loop) -- the residual is added in place -- and one thread stores
+//      the half tile with an asynchronous TMA store.  The operand ring is handed back at the last MMA, so the producer
+//      fills the next tile's first stages while the epilogue runs, and the two warpgroups never wait for each other.
+//   3 generic (fp32 output, batched, unaligned N) and SPLIT-K: the fp32 accumulator tile goes through the (idle) operand
+//      ring and the eight consumer warps store it from there.
 // Split-K (tiles alone cannot fill 132 SMs): the `splits` CTAs of a tile are launched as ONE thread-block cluster
 // (1, 1, splits), so the hardware co-schedules them.  Each stores its partial accumulator into its own fp32 plane of the
 // workspace, a cluster barrier (release / acquire) publishes the planes, and every split then sums the planes and applies
@@ -40,9 +43,8 @@ constexpr int EPI_THREADS = 32 * EPI_WARPS;
 constexpr int GEMM_THREADS = 128 + EPI_THREADS;
 constexpr uint64_t WAIT_LIMIT_NS = 4000000000ull;   // bounded waits: a protocol bug traps (with a record) instead of hanging the GPU
 constexpr int MAX_CLUSTER = 8;                      // splits: one cluster per tile (8 = the portable cluster size)
-constexpr int RES_PREFETCH = 8;                     // 16-byte residual pieces per lane fetched before the accumulator is read
 
-enum { WAIT_EMPTY = 1, WAIT_FULL = 2 };   // which wait timed out (o2345_last_trap)
+enum { WAIT_EMPTY = 1, WAIT_FULL = 2, WAIT_RESIDUAL = 3 };   // which wait timed out (o2345_last_trap)
 
 struct TrapRecord {
   unsigned long long magic;
@@ -89,6 +91,20 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const CUtensorMap* map, u
       ::"r"(smem_u32(dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+// asynchronous TMA stores of a shared-memory box (bulk async-group of the issuing thread)
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
+               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
+}
+__device__ __forceinline__ void tma_store_5d(const CUtensorMap* map, const void* src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
+               ::"l"(map), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// this thread's stores have finished reading shared memory / have completed
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
   asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
@@ -98,6 +114,7 @@ __device__ __forceinline__ void cluster_sync_all() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
 __device__ __forceinline__ void epi_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }   // the eight MMA / epilogue warps only
+__device__ __forceinline__ void wg_bar(int wg) { asm volatile("bar.sync %0, 128;" ::"r"(2 + wg) : "memory"); }   // one consumer warpgroup
 
 // the accumulator tile in shared memory: fp32 [128][BN + 4] (the pad spreads the row-per-thread reads over the banks)
 __host__ __device__ constexpr int acc_ld(int bn) { return bn + 4; }
@@ -380,27 +397,51 @@ __device__ __forceinline__ void splitk_finalize(const GemmParams& p, int m0, int
   }
 }
 
-constexpr int EPI_RB_GROUPS = 8;                 // row-bias groups (images) one 128-row tile may span when staged in smem
-__host__ __device__ constexpr int epi_smem_bytes(int bn) { return bn * 4 + EPI_RB_GROUPS * bn * 2; }
-// the two column ranges of the eight epilogue warps split the tile at a multiple of 32 (a GEGLU chunk never straddles them)
+constexpr int EPI_RB_GROUPS = 8;                 // row-bias groups (images) one warpgroup's 64 rows may span when staged in smem
+__host__ __device__ constexpr int epi_smem_bytes(int bn) { return bn * 4 + EPI_RB_GROUPS * bn * 2; }   // per consumer warpgroup
+// the two column ranges of the eight MODE 3 epilogue warps split the tile at a multiple of 32
 __host__ __device__ constexpr int col_split(int bn) { return ((bn / 2 + 31) / 32) * 32; }
 
-// Called by the eight epilogue warps while the main loop runs: the tile's bias and row-group-bias slices go to shared
-// memory, so that the epilogue proper never waits on a first-touch global load.
+// Staged modes: the fp16 output columns of a tile (GEGLU halves them), and the TMA box width the output half tile of a
+// warpgroup is cut into -- the widest of 64 / 32 / 16 columns that divides it, with the 128 / 64 / 32-byte swizzle of that
+// row length.
+__host__ __device__ constexpr int out_cols(int bn, int mode) { return mode == 1 ? bn / 2 : bn; }
+__host__ __device__ constexpr int out_box(int ow) { return ow % 64 == 0 ? 64 : (ow % 32 == 0 ? 32 : 16); }
+__host__ __device__ constexpr int out_half_bytes(int ow) { return 64 * ow * 2; }
+
+// Byte offset of (row r, output column c) in a warpgroup's half tile: boxes of BOX columns x 64 rows, 2 BOX bytes per row,
+// laid out as TMA's swizzle for that row length places them (16-byte chunk index ^= offset bits 7..).  The eight rows one
+// fragment store of a warp touches then fall into eight different bank groups.
+template <int BOX>
+__device__ __forceinline__ uint32_t out_off(int r, int c) {
+  const uint32_t o = (uint32_t)(r * (2 * BOX) + (c % BOX) * 2);
+  return (uint32_t)(c / BOX) * (128 * BOX) + (o ^ (((o >> 7) & (BOX / 8 - 1)) << 4));
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t a) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(a) : "memory");
+  return v;
+}
+__device__ __forceinline__ void st_shared_u32(uint32_t a, uint32_t v) { asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(v) : "memory"); }
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<uint32_t*>(&h); }
+__device__ __forceinline__ __half2 bits_h2(uint32_t v) { return *reinterpret_cast<__half2*>(&v); }
+
+// Called by a consumer warpgroup while its first k-block's MMAs run: the tile's bias slice and the row-group-bias slices
+// of the warpgroup's rows [rm0, rm0 + 64) go to its shared-memory copy, so that the epilogue never waits on a first-touch
+// global load.
 template <int BN>
-__device__ __forceinline__ void epilogue_preload(const GemmParams& p, int m0, int n0, float* sbias, __half* srb, int te) {
-  for (int i = te; i < BN; i += EPI_THREADS) sbias[i] = (p.bias && n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.f;
-  if (p.rowbias) {
-    const int g0 = m0 / p.rows_per_group;
-    const int last = (m0 + BM - 1 < p.M ? m0 + BM - 1 : p.M - 1) / p.rows_per_group;
+__device__ __forceinline__ void epilogue_preload(const GemmParams& p, int rm0, int n0, float* sbias, __half* srb, int tw) {
+  for (int i = tw; i < BN; i += 128) sbias[i] = (p.bias && n0 + i < p.N) ? __ldg(p.bias + n0 + i) : 0.f;
+  if (p.rowbias && rm0 < p.M) {
+    const int g0 = rm0 / p.rows_per_group;
+    const int last = (rm0 + 63 < p.M ? rm0 + 63 : p.M - 1) / p.rows_per_group;
     const int ng = last - g0 + 1;
-    if (ng >= 1 && ng <= EPI_RB_GROUPS)
-      for (int i = te; i < ng * BN; i += EPI_THREADS) {
+    if (ng <= EPI_RB_GROUPS)
+      for (int i = tw; i < ng * BN; i += 128) {
         const int gi = i / BN, c = i - gi * BN;
         srb[i] = (n0 + c < p.N) ? p.rowbias[(int64_t)(g0 + gi) * p.rowbias_ld + n0 + c] : __float2half(0.f);
       }
   }
-  epi_bar();
 }
 
 template <int ACT>
@@ -411,173 +452,80 @@ __device__ __forceinline__ float act_fn(float x) {
   return x;
 }
 
-// Phase 1 of the staged epilogue for one thread (= one accumulator row) over tile columns [c_lo, c_hi): accumulator tile ->
-// alpha / bias / row-group bias / activation (ACT 3: GEGLU gate) -> fp16 -> this row of the warp's shared-memory slab.
-// rb: this row's row-group bias indexed by TILE column (nullptr: none); rb_smem: it is the shared-memory copy (no N tail).
-template <int ACT>
-__device__ __forceinline__ void stage_rows(const GemmParams& p, const float* acc_row, uint8_t* mine, int n0, int c_lo, int c_hi,
-                                           const float* sbias, const __half* rb, bool rb_smem) {
-#pragma unroll 1
-  for (int c0 = c_lo; c0 < c_hi; c0 += 32) {
-    if (n0 + c0 >= p.N) break;                     // warp-uniform
-    uint32_t r[32];
-    acc_ld32(acc_row + c0, r);
-    if (ACT == 3) {
-      __half2 h[8];
+// Staged epilogue of one consumer thread (tw = its index in the warpgroup) on its m64nBN fragment d, whose element
+// d[4 j + 2 h + e] is row 16 (tw / 32) + (tw % 32) / 4 + 8 h, tile column 8 j + 2 (tw % 4) + e of the warpgroup's rows:
+// alpha / bias / row-group bias / activation (ACT 3: GEGLU gate) in fp32, rounded to fp16 (where autocast rounds the layer
+// output), then the residual -- already in the half tile -- added in fp32 and rounded again.  rb[h]: row-group bias of the
+// thread's row h indexed by tile column, nullptr for none; rb_global: it points to global memory (mind the N tail).
+template <int BN, int MODE, int ACT>
+__device__ __forceinline__ void epilogue_regs(const GemmParams& p, const float (&d)[BN / 2], uint32_t tile, int tw, int n0,
+                                              const float* sbias, const __half* const (&rb)[2], bool rb_global) {
+  constexpr int BOX = out_box(out_cols(BN, MODE));
+  const int q = tw & 3, r = 16 * (tw >> 5) + ((tw & 31) >> 2);
+  if constexpr (MODE == 1) {   // chunk k of 32 columns = 16 values + their 16 gates: a value and its gate sit in the same thread
 #pragma unroll
-      for (int e = 0; e < 16; e += 2) {
-        float a0 = fmaf(__uint_as_float(r[e]), p.alpha, sbias[c0 + e]), a1 = fmaf(__uint_as_float(r[e + 1]), p.alpha, sbias[c0 + e + 1]);
-        float g0 = fmaf(__uint_as_float(r[16 + e]), p.alpha, sbias[c0 + 16 + e]);
-        float g1 = fmaf(__uint_as_float(r[17 + e]), p.alpha, sbias[c0 + 17 + e]);
-        h[e >> 1] = __floats2half2_rn(a0 * gelu_erf_fast(g0), a1 * gelu_erf_fast(g1));
-      }
-      uint4* d = reinterpret_cast<uint4*>(mine + (c0 - c_lo));   // (c0 - c_lo) / 2 output columns x 2 bytes
-      d[0] = reinterpret_cast<uint4*>(h)[0], d[1] = reinterpret_cast<uint4*>(h)[1];
-    } else {
+    for (int k = 0; k < BN / 32; ++k)
 #pragma unroll
-      for (int j = 0; j < 32; j += 8) {
-        float v[8];
-        const float4 b0 = *reinterpret_cast<const float4*>(sbias + c0 + j), b1 = *reinterpret_cast<const float4*>(sbias + c0 + j + 4);
-        v[0] = b0.x, v[1] = b0.y, v[2] = b0.z, v[3] = b0.w, v[4] = b1.x, v[5] = b1.y, v[6] = b1.z, v[7] = b1.w;
-        if (rb && (rb_smem || n0 + c0 + j + 8 <= p.N)) {
-          uint4 q = *reinterpret_cast<const uint4*>(rb + c0 + j);
-          const __half* hq = reinterpret_cast<const __half*>(&q);
+      for (int jj = 0; jj < 2; ++jj) {
+        const int j = 4 * k + jj, c = 8 * j + 2 * q;
+        const float2 bv = *reinterpret_cast<const float2*>(sbias + c), bg = *reinterpret_cast<const float2*>(sbias + c + 16);
 #pragma unroll
-          for (int e = 0; e < 8; ++e) v[e] += __half2float(hq[e]);
+        for (int h = 0; h < 2; ++h) {
+          const float a0 = fmaf(d[4 * j + 2 * h], p.alpha, bv.x), a1 = fmaf(d[4 * j + 2 * h + 1], p.alpha, bv.y);
+          const float g0 = fmaf(d[4 * (j + 2) + 2 * h], p.alpha, bg.x), g1 = fmaf(d[4 * (j + 2) + 2 * h + 1], p.alpha, bg.y);
+          st_shared_u32(tile + out_off<BOX>(r + 8 * h, 16 * k + 8 * jj + 2 * q),
+                        h2_bits(__floats2half2_rn(a0 * gelu_erf_fast(g0), a1 * gelu_erf_fast(g1))));
         }
-        __half2 h[4];
-#pragma unroll
-        for (int e = 0; e < 8; e += 2) {
-          float x0 = fmaf(__uint_as_float(r[j + e]), p.alpha, v[e]), x1 = fmaf(__uint_as_float(r[j + e + 1]), p.alpha, v[e + 1]);
-          h[e >> 1] = __floats2half2_rn(act_fn<ACT>(x0), act_fn<ACT>(x1));
-        }
-        *reinterpret_cast<uint4*>(mine + (c0 - c_lo + j) * 2) = *reinterpret_cast<uint4*>(h);
       }
-    }
-  }
-}
-
-// Output geometry of one epilogue warp in the staged modes: 32 rows x tile columns [c_lo, c_hi) become `outc` fp16 columns
-// (GEGLU halves them) = `ppr` 16-byte pieces per row, `total` pieces per warp, lane l owns pieces l, l + 32, ...
-struct WarpOut {
-  int outc, stride, ppr, total, ocol0, nout;
-};
-template <int MODE>
-__device__ __forceinline__ WarpOut warp_out(const GemmParams& p, int n0, int c_lo, int c_hi) {
-  constexpr bool geglu = MODE == 1;
-  WarpOut g;
-  g.outc = geglu ? (c_hi - c_lo) >> 1 : (c_hi - c_lo);
-  g.stride = g.outc * 2 + 16;                      // +16: 16-byte pieces of consecutive rows rotate banks
-  g.ppr = g.outc >> 3;
-  g.total = 32 * g.ppr;
-  g.ocol0 = geglu ? (n0 + c_lo) >> 1 : n0 + c_lo;  // first column of C this warp writes
-  g.nout = geglu ? p.N >> 1 : p.N;
-  return g;
-}
-
-// The first RES_PREFETCH residual pieces of this lane, fetched while the main loop runs.
-__device__ __forceinline__ void prefetch_residual(const GemmParams& p, const WarpOut& g, int lane, int row0,
-                                                  uint4 (&resq)[RES_PREFETCH]) {
+  } else {
 #pragma unroll
-  for (int u = 0; u < RES_PREFETCH; ++u) {
-    resq[u] = make_uint4(0u, 0u, 0u, 0u);
-    const int pp = lane + 32 * u;
-    if (p.residual && pp < g.total) {
-      const int rl = pp / g.ppr, ci = pp - rl * g.ppr;
-      const int grow = row0 + rl, col = g.ocol0 + ci * 8;
-      if (grow < p.M && col < g.nout) resq[u] = *reinterpret_cast<const uint4*>(p.residual + out_row(p, grow) * p.ldc + col);
-    }
-  }
-}
-
-__device__ __forceinline__ uint4 add_h8(uint4 v, uint4 q) {
-  __half2* a = reinterpret_cast<__half2*>(&v);
-  const __half2* b = reinterpret_cast<const __half2*>(&q);
+  for (int j = 0; j < BN / 8; ++j) {
+    const int c = 8 * j + 2 * q;
+    const float2 b = *reinterpret_cast<const float2*>(sbias + c);
 #pragma unroll
-  for (int e = 0; e < 4; ++e) {
-    float2 fa = __half22float2(a[e]), fb = __half22float2(b[e]);
-    a[e] = __floats2half2_rn(fa.x + fb.x, fa.y + fb.y);
-  }
-  return v;
-}
-
-// Staged epilogue of ONE warp: 32 accumulator rows x tile columns [c_lo, c_hi), fp16 output.
-//   phase 1   thread = row of the accumulator tile: alpha / bias / row-group bias / activation / GEGLU gate, rounded to
-//             fp16 (where autocast rounds the layer output) into this warp's slab;
-//   phase 2   the warp walks the slab in 16-byte pieces along rows, adds the residual (prefetched for the first
-//             RES_PREFETCH pieces of a lane) and writes whole rows: every global access is a run of full 32-byte sectors.
-// (r1 trace: with one 16-byte store per lane to 32 different rows the epilogue took 46 000 cycles per tile.)
-template <int BN, int MODE>
-__device__ __forceinline__ void epilogue_staged(const GemmParams& p, const WarpOut& g, const float* acc_row, uint8_t* slab, int lane,
-                                                int m0, int row0, int n0, int c_lo, int c_hi, const float* sbias, const __half* srb,
-                                                const uint4 (&resq)[RES_PREFETCH]) {
-  const int row = row0 + lane;
-  // row-group bias of this thread's row: from the smem copy when the tile spans few groups, else straight from global
-  const __half* rb = nullptr;
-  bool rb_smem = false;
-  if (MODE != 1 && p.rowbias) {
-    const int rr = row < p.M ? row : p.M - 1;
-    const int g0 = m0 / p.rows_per_group, last = (m0 + BM - 1 < p.M ? m0 + BM - 1 : p.M - 1) / p.rows_per_group;
-    rb_smem = last - g0 + 1 <= EPI_RB_GROUPS;
-    rb = rb_smem ? srb + (rr / p.rows_per_group - g0) * BN : p.rowbias + (int64_t)(rr / p.rows_per_group) * p.rowbias_ld + n0;
-  }
-  uint8_t* mine = slab + lane * g.stride;
-  if (MODE == 0) {
-    stage_rows<0>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem);
-  } else if (MODE == 1) {
-    stage_rows<3>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem);
-  } else {   // the activation switch is hoisted out of the element loops: one branch per tile
-    switch (p.act) {
-      case 1: stage_rows<1>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
-      case 2: stage_rows<2>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
-      default: stage_rows<4>(p, acc_row, mine, n0, c_lo, c_hi, sbias, rb, rb_smem); break;
-    }
-  }
-  __syncwarp();
-  __half* C = reinterpret_cast<__half*>(p.C);
-  // N is a multiple of 8 on this path (host check): no partial pieces
-#pragma unroll
-  for (int u = 0; u < RES_PREFETCH; ++u) {
-    const int pp = lane + 32 * u;
-    if (pp < g.total) {
-      const int rl = pp / g.ppr, ci = pp - rl * g.ppr;
-      const int grow = row0 + rl, col = g.ocol0 + ci * 8;
-      if (grow < p.M && col < g.nout) {
-        uint4 v = *reinterpret_cast<const uint4*>(slab + rl * g.stride + ci * 16);
-        if (p.residual) v = add_h8(v, resq[u]);
-        *reinterpret_cast<uint4*>(C + out_row(p, grow) * p.ldc + col) = v;
+    for (int h = 0; h < 2; ++h) {
+      float v0 = b.x, v1 = b.y;
+      if (rb[h] && (!rb_global || n0 + c < p.N)) {
+        const float2 f = __half22float2(*reinterpret_cast<const __half2*>(rb[h] + c));
+        v0 += f.x, v1 += f.y;
       }
+      const float x0 = fmaf(d[4 * j + 2 * h], p.alpha, v0), x1 = fmaf(d[4 * j + 2 * h + 1], p.alpha, v1);
+      __half2 o = __floats2half2_rn(act_fn<ACT>(x0), act_fn<ACT>(x1));
+      const uint32_t a = tile + out_off<BOX>(r + 8 * h, c);
+      if (p.residual) {
+        const float2 fa = __half22float2(o), fb = __half22float2(bits_h2(ld_shared_u32(a)));
+        o = __floats2half2_rn(fa.x + fb.x, fa.y + fb.y);
+      }
+      st_shared_u32(a, h2_bits(o));
     }
   }
-  constexpr int UN = 4;
-  for (int base = lane + 32 * RES_PREFETCH; base < g.total; base += 32 * UN) {
-    uint4 v[UN], q[UN];
-    int64_t o[UN];
-    bool ok[UN];
-#pragma unroll
-    for (int u = 0; u < UN; ++u) {
-      const int pp = base + 32 * u;
-      const int rl = pp / g.ppr, ci = pp - rl * g.ppr;
-      const int grow = row0 + rl, col = g.ocol0 + ci * 8;
-      ok[u] = pp < g.total && grow < p.M && col < g.nout;
-      o[u] = out_row(p, grow) * p.ldc + col;
-      if (ok[u]) {
-        v[u] = *reinterpret_cast<const uint4*>(slab + rl * g.stride + ci * 16);
-        if (p.residual) q[u] = *reinterpret_cast<const uint4*>(p.residual + o[u]);
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < UN; ++u) {
-      if (!ok[u]) continue;
-      if (p.residual) v[u] = add_h8(v[u], q[u]);
-      *reinterpret_cast<uint4*>(C + o[u]) = v[u];
-    }
   }
 }
 
-__host__ __device__ constexpr int epi_slab_bytes(int bn) { return EPI_WARPS * 32 * (col_split(bn) * 2 + 16); }
-constexpr int smem_bytes(int bn, int stages) {
-  return stages * (BM * BK * 2 + bn * BK * 2) + epi_slab_bytes(bn) + 2 * stages * 8 + 16 + epi_smem_bytes(bn) + 1024;
+// One thread of a consumer warpgroup moves its half tile (rows [rm0, rm0 + 64), output columns from ocol0) between shared
+// memory and the output / residual tensor map, one TMA box of BOX columns at a time; boxes wholly past the last column are
+// skipped, the map clips the rest.  A load first announces on `bar` exactly the bytes of the boxes it issues.  The
+// up-sampling conv writes its phase (upa, upb) through the 5-D map [B H][2][W][2][N]: the half tile's 64 low-resolution
+// pixels are one box of (W_tile, rows) (make_out_map).
+template <int BOX, int NBOX, bool STORE>
+__device__ __forceinline__ void out_tile_tma(const GemmParams& p, const CUtensorMap* map, uint8_t* tile, int rm0, int ocol0, int nout,
+                                             uint64_t* bar) {
+  const int nb = min(NBOX, (nout - ocol0 + BOX - 1) / BOX);
+  if (!STORE) mbar_expect_tx(bar, (uint32_t)nb * (128 * BOX));
+#pragma unroll
+  for (int b = 0; b < NBOX; ++b) {
+    if (b >= nb) break;
+    const int c = ocol0 + b * BOX;
+    uint8_t* s = tile + b * (128 * BOX);
+    if (!STORE) tma_load_2d(s, map, bar, c, rm0);
+    else if (p.up) tma_store_5d(map, s, c, p.upb, rm0 % p.cW, p.upa, rm0 / p.cW);
+    else tma_store_2d(map, s, c, rm0);
+  }
+}
+
+constexpr int smem_bytes(int bn, int stages, int mode) {
+  return stages * (BM * BK * 2 + bn * BK * 2) + (mode == 3 ? 0 : 2 * out_half_bytes(out_cols(bn, mode))) + (2 * stages + 2) * 8 + 16 +
+         2 * epi_smem_bytes(bn) + 1024;
 }
 
 // Where the producer's next k-block comes from.  The producer is one thread that waits for a free stage and then issues its
@@ -627,7 +575,7 @@ __device__ __forceinline__ void produce_stage(const GemmParams& p, const CUtenso
   }
 }
 
-// A warpgroup's m64nBN accumulator fragment -> rows [row0, row0 + 64) of the shared-memory accumulator tile
+// MODE 3: a warpgroup's m64nBN accumulator fragment -> rows [row0, row0 + 64) of the shared-memory accumulator tile
 template <int BN>
 __device__ __forceinline__ void acc_store(float* acc, const float (&d)[BN / 2], int row0, int t) {
   const int r = row0 + 16 * (t >> 5) + ((t & 31) >> 2), c = 2 * (t & 3);
@@ -639,9 +587,11 @@ __device__ __forceinline__ void acc_store(float* acc, const float (&d)[BN / 2], 
 }
 
 // ------------------------------------------------------------------------------------------------ the kernel
+// tmC / tmR (staged modes): the fp16 output and the residual seen in boxes of one warpgroup's half tile (make_out_map)
 template <int BN, int STAGES, int MODE>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ GemmParams p) {
+gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmC,
+               const __grid_constant__ CUtensorMap tmR, const __grid_constant__ GemmParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment is required by SWIZZLE_128B
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
@@ -650,14 +600,16 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   static_assert(BN % 32 == 0 && BN >= 64 && BN <= 256, "tile width: a multiple of 32 (GEGLU chunks, 32-column epilogue reads)");
   static_assert(BM * acc_ld(BN) * 4 <= STAGES * (A_BYTES + B_BYTES), "the accumulator tile must fit in the operand ring");
   constexpr int CSPLIT = col_split(BN);
+  constexpr int OW = out_cols(BN, MODE), BOX = out_box(OW), OUT_HALF = out_half_bytes(OW);
   uint8_t* sA = smem;
   uint8_t* sB = smem + STAGES * A_BYTES;
-  uint8_t* slabs = sB + STAGES * B_BYTES;
-  uint64_t* full = reinterpret_cast<uint64_t*>(slabs + epi_slab_bytes(BN));
+  uint8_t* sOut = sB + STAGES * B_BYTES;                      // staged modes: one fp16 half tile per consumer warpgroup
+  uint64_t* full = reinterpret_cast<uint64_t*>(sOut + (MODE == 3 ? 0 : 2 * OUT_HALF));
   uint64_t* empty = full + STAGES;
-  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(empty + STAGES) + 15) & ~(uintptr_t)15);
-  __half* srb = reinterpret_cast<__half*>(sbias + BN);
-  float* acc = reinterpret_cast<float*>(smem);                // the operand ring, once the K loop is done
+  uint64_t* resbar = empty + STAGES;                          // per consumer warpgroup: its residual half tile has landed
+  float* sbias = reinterpret_cast<float*>((reinterpret_cast<uintptr_t>(resbar + 2) + 15) & ~(uintptr_t)15);   // [2][BN]
+  __half* srb = reinterpret_cast<__half*>(sbias + 2 * BN);                                                     // [2][8 BN]
+  float* acc = reinterpret_cast<float*>(smem);                // MODE 3: the operand ring, once the K loop is done
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) stamp(p, 0), stamp_ns(p, 16);
@@ -674,9 +626,11 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   if (threadIdx.x == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
+    if (MODE != 3) asm volatile("prefetch.tensormap [%0];" ::"l"(&tmC) : "memory");
     for (int s = 0; s < STAGES; ++s) mbar_init(full + s, 1), mbar_init(empty + s, 2);   // empty: one arrival per MMA warpgroup
+    mbar_init(resbar, 1), mbar_init(resbar + 1, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    fence_proxy_async();
   }
   __syncthreads();
   pdl_wait();      // everything above touched no global memory: it overlaps the tail of the previous kernel
@@ -685,15 +639,15 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
 
   // Tiles of this CTA: one (blockIdx.x, blockIdx.y), or -- persistent launch (p.persist, staged epilogues only) -- tiles
   // blockIdx.x, blockIdx.x + gridDim.x, ... of the column-major tile order.  The ring's stage / phase counters run on across
-  // tiles, so the producer fills the next tile's first stages as soon as the epilogue has handed the ring back.
+  // tiles, so the producer fills the next tile's first stages as soon as the last MMA of a tile has released its stage.
   const int tiles_m = (p.M + BM - 1) / BM, tiles = tiles_m * ((p.N + BN - 1) / BN);
   const bool persist = MODE != 3 && p.persist;
-  uint32_t cnt = 0;   // k-blocks consumed so far by this CTA
+  uint32_t cnt = 0;       // k-blocks consumed so far by this CTA
+  uint32_t rphase = 0;    // residual half tiles this warpgroup has loaded so far (parity of resbar)
   for (int t = persist ? blockIdx.x : blockIdx.y * tiles_m + blockIdx.x; t < tiles; t += persist ? gridDim.x : tiles) {
   const int m0 = (t % tiles_m) * BM, n0 = (t / tiles_m) * BN;
   if (warp < 4) {
     if (threadIdx.x == 0) {  // ---------------- TMA producer
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // the epilogue's generic accesses to the ring come first
       ProducerPos q = producer_start(p, m0, bz, kb0);
       for (int kb = kb0; kb < kb1; ++kb) {
         const uint32_t c = cnt + (kb - kb0);
@@ -708,10 +662,13 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     }
     __syncwarp();
   } else {  // ------------------------ warpgroups 1 and 2: MMAs on rows [64 wg, 64 wg + 64), then the epilogue
-    const int wg = (warp >> 2) - 1, e = warp - 4, quarter = e & 3, te = threadIdx.x - 128;
-    const int c_lo = e < 4 ? 0 : CSPLIT, c_hi = e < 4 ? CSPLIT : BN;   // this warp's tile columns
-    const int row0 = m0 + quarter * 32;
-    if (MODE != 3) epilogue_preload<BN>(p, m0, n0, sbias, srb, te);
+    const int wg = (warp >> 2) - 1, e = warp - 4, quarter = e & 3, te = threadIdx.x - 128, tw = threadIdx.x & 127;
+    // staged modes: this warpgroup's rows, output columns, half tile and bias slices
+    const int rm0 = m0 + 64 * wg, ocol0 = MODE == 1 ? n0 / 2 : n0, nout = MODE == 1 ? p.N / 2 : p.N;
+    const bool rows = rm0 < p.M;
+    uint8_t* tile = sOut + wg * OUT_HALF;
+    float* wbias = sbias + wg * BN;
+    __half* wrb = srb + wg * EPI_RB_GROUPS * BN;
     {
       float d[BN / 2];
 #pragma unroll
@@ -721,32 +678,79 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int s = c % STAGES;
         const uint32_t ph = (c / STAGES) & 1;
         mbar_wait(full + s, ph, p, WAIT_FULL, s);
-        if (kb == kb0 && te == 0) stamp(p, 4);
+        if (kb == kb0 && te == 0) {
+          if (p.trace && t != (int)blockIdx.x && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) p.trace[9] = p.trace[5];
+          stamp(p, 4);
+        }
         const uint32_t a0 = smem_u32(sA + s * A_BYTES) + wg * (64 * 128), b0 = smem_u32(sB + s * B_BYTES);
         wg::fence();
 #pragma unroll
         for (int k = 0; k < BK / 16; ++k)   // advancing 16 fp16 along K inside the 128-byte swizzle atom = +32 bytes on the start address
           wg::mma_f16<BN>(d, wg::desc_sw128(a0 + k * 32), wg::desc_sw128(b0 + k * 32), 1);
         wg::commit();
+        if (MODE != 3 && kb == kb0) {
+          // under the first k-block's MMAs: once the previous tile's store has read the half tile, the residual is loaded
+          // into it; the bias slices are refreshed (the previous epilogue is done with them: it ended at a wg_bar)
+          if (tw == 0) {
+            bulk_wait_read();
+            if (p.residual && rows) out_tile_tma<BOX, OW / BOX, false>(p, &tmR, tile, rm0, ocol0, nout, resbar + wg);
+          }
+          epilogue_preload<BN>(p, rm0, n0, wbias, wrb, tw);
+          wg_bar(wg);
+        }
         wg::wait<1>();                      // the previous stage's MMAs are done: hand that stage back to the producer
-        if (kb > kb0 && (threadIdx.x & 127) == 0) mbar_arrive(empty + (c - 1) % STAGES);
+        if (kb > kb0 && tw == 0) mbar_arrive(empty + (c - 1) % STAGES);
       }
       wg::wait<0>();
-      if ((threadIdx.x & 127) == 0) mbar_arrive(empty + (cnt + kb1 - kb0 - 1) % STAGES);
+      if (tw == 0) mbar_arrive(empty + (cnt + kb1 - kb0 - 1) % STAGES);   // the ring is the producer's again
       if (te == 0) stamp(p, 5);
-      epi_bar();                            // both warpgroups are done reading the ring: it becomes the accumulator tile
-      acc_store<BN>(acc, d, 64 * wg, threadIdx.x & 127);
+      if (MODE != 3) {
+        if (rows) {
+          if (p.residual) mbar_wait(resbar + wg, rphase & 1, p, WAIT_RESIDUAL, wg);
+          if (te == 0) stamp(p, 6);
+          // row-group bias of the thread's two rows: from the smem copy when the warpgroup's rows span few groups
+          const __half* rb[2] = {nullptr, nullptr};
+          bool rb_global = false;
+          if (MODE != 1 && p.rowbias) {
+            const int g0 = rm0 / p.rows_per_group, last = (rm0 + 63 < p.M ? rm0 + 63 : p.M - 1) / p.rows_per_group;
+            rb_global = last - g0 + 1 > EPI_RB_GROUPS;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              const int row = rm0 + 16 * (tw >> 5) + ((tw & 31) >> 2) + 8 * h, g = (row < p.M ? row : p.M - 1) / p.rows_per_group;
+              rb[h] = rb_global ? p.rowbias + (int64_t)g * p.rowbias_ld + n0 : wrb + (g - g0) * BN;
+            }
+          }
+          const uint32_t ts = smem_u32(tile);
+          if constexpr (MODE == 0) {
+            epilogue_regs<BN, 0, 0>(p, d, ts, tw, n0, wbias, rb, rb_global);
+          } else if constexpr (MODE == 1) {
+            epilogue_regs<BN, 1, 3>(p, d, ts, tw, n0, wbias, rb, rb_global);
+          } else {   // the activation switch is hoisted out of the element loops: one branch per tile
+            switch (p.act) {
+              case 1: epilogue_regs<BN, 2, 1>(p, d, ts, tw, n0, wbias, rb, rb_global); break;
+              case 2: epilogue_regs<BN, 2, 2>(p, d, ts, tw, n0, wbias, rb, rb_global); break;
+              default: epilogue_regs<BN, 2, 4>(p, d, ts, tw, n0, wbias, rb, rb_global); break;
+            }
+          }
+          fence_proxy_async();              // the half tile's generic writes, before the TMA store reads it
+          wg_bar(wg);
+          if (tw == 0) {
+            out_tile_tma<BOX, OW / BOX, true>(p, &tmC, tile, rm0, ocol0, nout, nullptr);
+            bulk_commit();
+          }
+          if (p.residual) ++rphase;
+        }
+      } else {
+        epi_bar();                          // both warpgroups are done reading the ring: it becomes the accumulator tile
+        acc_store<BN>(acc, d, 64 * wg, tw);
+      }
     }
-    epi_bar();
-    if (te == 0) stamp(p, 6);
-    const float* acc_row = acc + (quarter * 32 + lane) * acc_ld(BN);
-    if (MODE != 3) {
-      const WarpOut g = warp_out<MODE>(p, n0, c_lo, c_hi);
-      uint4 resq[RES_PREFETCH];
-      prefetch_residual(p, g, lane, row0, resq);
-      epilogue_staged<BN, MODE>(p, g, acc_row, slabs + e * 32 * (CSPLIT * 2 + 16), lane, m0, row0, n0, c_lo, c_hi, sbias, srb, resq);
-    } else {
-      const int row = row0 + lane;
+    if (MODE == 3) {
+      epi_bar();
+      if (te == 0) stamp(p, 6);
+      const float* acc_row = acc + (quarter * 32 + lane) * acc_ld(BN);
+      const int c_lo = e < 4 ? 0 : CSPLIT, c_hi = e < 4 ? CSPLIT : BN;   // this warp's tile columns
+      const int row = m0 + quarter * 32 + lane;
       if (split) {
         if (te == 0) stamp_ns(p, 17);
 #pragma unroll 1
@@ -770,8 +774,9 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     if (te == 0) stamp(p, 7);
   }
   cnt += kb1 - kb0;
-  __syncthreads();   // the epilogue is done with the accumulator tile, slabs and bias slices: the ring is free for the next tile
+  if (MODE == 3) __syncthreads();   // one tile per CTA: the accumulator tile is done with before the split-K exchange
   }
+  if (MODE != 3 && warp >= 4 && (threadIdx.x & 127) == 0) bulk_wait();   // the last half tile is in global memory
   if (split) {
     // the `splits` CTAs of a tile form ONE cluster (co-scheduled by the hardware): this barrier -- release / acquire at
     // cluster scope -- publishes every split's partial plane to its siblings
@@ -818,6 +823,39 @@ int make_map(CUtensorMap* m, const void* ptr, int64_t rows, int64_t K, int64_t l
   return O2345_OK;
 }
 
+// Staged modes: the fp16 output (or residual) [M rows, nout columns, row stride ldc] in boxes of `box` columns x 64 rows, one
+// consumer warpgroup's half tile, with the swizzle out_off() lays the half tile out in.  Rows past M and columns past nout
+// are clipped by the map (stores) or zero-filled (loads).  The up-sampling conv's phase (upa, upb) scatters low-resolution
+// pixel (b, y, x) to output row (2 (b H + y) + upa) 2 W + 2 x + upb: a 5-D view [B H][2][W][2][nout] whose box is
+// (box, 1, W_tile, 1, 64 / W_tile) with W_tile = min(W, 64) -- the half tile's 64 consecutive pixels.
+int make_out_map(CUtensorMap* m, const void* ptr, const GemmParams& p, int nout, int box) {
+  EncodeTiledFn fn = encode_fn();
+  if (!fn) { set_error("cuTensorMapEncodeTiled entry point not available"); return O2345_ECUDA; }
+  const CUtensorMapSwizzle sw = box == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : (box == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
+  const cuuint64_t row = (cuuint64_t)p.ldc * 2;
+  cuuint32_t estr[5] = {1, 1, 1, 1, 1};
+  CUresult r;
+  if (p.up) {
+    // a half tile's 64 consecutive pixels are whole rows of W_tile pixels only when W divides 64 or is a multiple of it
+    // (conv_tiles() admits W that divide 128 or are multiples of 128); any other W would scatter wrong rows
+    O2345_CHECK_ARG(64 % p.cW == 0 || p.cW % 64 == 0, "up-sampling conv output map: W must divide 64 or be a multiple of 64");
+    const int wt = p.cW < 64 ? p.cW : 64;
+    cuuint64_t dims[5] = {(cuuint64_t)nout, 2, (cuuint64_t)p.cW, 2, (cuuint64_t)(p.M / p.cW)};
+    cuuint64_t strides[4] = {row, 2 * row, 2 * (cuuint64_t)p.cW * row, 4 * (cuuint64_t)p.cW * row};
+    cuuint32_t boxd[5] = {(cuuint32_t)box, 1, (cuuint32_t)wt, 1, (cuuint32_t)(64 / wt)};
+    r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 5, const_cast<void*>(ptr), dims, strides, boxd, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  } else {
+    cuuint64_t dims[2] = {(cuuint64_t)nout, (cuuint64_t)p.M};
+    cuuint64_t strides[1] = {row};
+    cuuint32_t boxd[2] = {(cuuint32_t)box, 64};
+    r = fn(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(ptr), dims, strides, boxd, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
+           CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  }
+  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (GEMM output) failed with %d (M=%d nout=%d ldc=%lld)", (int)r, p.M, nout, (long long)p.ldc); return O2345_ECUDA; }
+  return O2345_OK;
+}
+
 // Host-mapped trap record (one per process): allocated on the first launch that is not inside a stream capture.
 TrapRecord* g_diag = nullptr;
 bool g_diag_tried = false;
@@ -858,9 +896,11 @@ void read_force_env() {
 }
 
 // Tile width and k-splits for a problem of M x N with nk k-blocks of 64: the candidate with the lowest predicted time under a
-// small cost model (its constants are starting values, not yet fitted on an H100 with tools/gemm_sweep.py):
+// small cost model.  A batch-64 tools/gemm_sweep.py on an H100 (DESIGN section 6) found no other constants that pick faster
+// configurations without changing a split count, and a split count that changes regroups the fp32 partial sums, i.e. the
+// layer's rounding:
 //   * a launch costs ~5 us of fixed latency (launch, prologue, first TMA round trip, tear-down) + ~3 us of epilogue per
-//     160 columns of tile and wave of CTAs;
+//     160 columns of tile and wave of CTAs; the main loop's cycles are converted at 1 750 cycles per us;
 //   * the main loop is bound by operand delivery or by the tensor pipe (a 128 x BN x 64 k-block is 4 BN cycles of wgmma at
 //     ~2 048 fp16 FMA per clock and SM): an SM ingests ~40 B/clk, the whole L2 -> SM fabric ~6 300 B/clk -- so few fat tiles
 //     starve (few SMs pull), many thin tiles re-read A (fabric), and long-K problems with few tiles want split-K;
@@ -918,9 +958,10 @@ Config pick_config(const GemmParams& p, int nk, bool can_split, int64_t ws_float
     c.bn = (g_force[1] == 64 || g_force[1] == 128 || g_force[1] == 160 || g_force[1] == 256) ? g_force[1] : 128;
     c.splits = 1;
   }
-  // Many waves of tiles: one CTA per SM walks them, so that launch, prologue and the wave tail are paid once per SM
+  // Two or more waves of tiles: one CTA per SM walks them, so that launch, prologue and the wave tail are paid once per SM
+  // and the next tile's loads run under the previous tile's epilogue (tools/gemm_persist_ab.py, DESIGN section 6)
   const int tiles = cdiv(M, BM) * cdiv(N, c.bn);
-  const int min_tiles = g_persist_min_tiles > 0 ? g_persist_min_tiles : 4 * sm_count();
+  const int min_tiles = g_persist_min_tiles > 0 ? g_persist_min_tiles : 2 * sm_count();
   c.persist = c.splits == 1 && (g_persist == 1 || (g_persist == 0 && tiles >= min_tiles));
   return c;
 }
@@ -938,7 +979,7 @@ long long* g_trace = nullptr;
 
 template <int BN, int STAGES, int MODE>
 int launch(const CUtensorMap& a, const CUtensorMap& b, GemmParams p, int batch, int persist, cudaStream_t st) {
-  constexpr int SMEM = smem_bytes(BN, STAGES);
+  constexpr int SMEM = smem_bytes(BN, STAGES, MODE);
   static_assert(SMEM <= 227 * 1024, "one CTA per SM");
   static PerDeviceOnce attr;
   if (attr.need())
@@ -953,7 +994,14 @@ int launch(const CUtensorMap& a, const CUtensorMap& b, GemmParams p, int batch, 
     const int tiles = (int)grid.x * (int)grid.y;
     grid = dim3(tiles < sm_count() ? tiles : sm_count(), 1, 1);
   }
-  O2345_CUDA(launch_pdl_cluster(gemm_tc_kernel<BN, STAGES, MODE>, grid, dim3(GEMM_THREADS), (size_t)SMEM, st, 1, splits, a, b, p));
+  CUtensorMap mc, mr;
+  memset(&mc, 0, sizeof(mc)), memset(&mr, 0, sizeof(mr));
+  if (MODE != 3) {
+    constexpr int OW = out_cols(BN, MODE);
+    O2345_TRY(make_out_map(&mc, p.C, p, p.act == 3 ? p.N / 2 : p.N, out_box(OW)));
+    if (p.residual) O2345_TRY(make_out_map(&mr, p.residual, p, p.N, out_box(OW)));
+  }
+  O2345_CUDA(launch_pdl_cluster(gemm_tc_kernel<BN, STAGES, MODE>, grid, dim3(GEMM_THREADS), (size_t)SMEM, st, 1, splits, a, b, mc, mr, p));
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }
@@ -968,7 +1016,7 @@ int launch_mode(int mode, const CUtensorMap& a, const CUtensorMap& b, const Gemm
   }
 }
 
-// ring depth per tile width: as many stages as fit next to the epilogue slabs in 227 KB (one CTA per SM)
+// ring depth per tile width: as many stages as fit next to the two output half tiles in 227 KB (one CTA per SM)
 int dispatch(const Config& c, int mode, const CUtensorMap& a, const CUtensorMap& b, const GemmParams& p, int batch, cudaStream_t st) {
   if (c.bn == 64) return launch_mode<64, 6>(mode, a, b, p, batch, c.persist, st);
   if (c.bn == 128) return launch_mode<128, 5>(mode, a, b, p, batch, c.persist, st);
@@ -1019,12 +1067,12 @@ extern "C" int o2345_last_trap(char* buf, size_t n) {
   const TrapRecord* d = g_diag;
   if (!d || d->magic != TRAP_MAGIC) return 0;
   static const char* names[] = {"?", "empty (producer waiting for the MMA to free a stage)", "full (MMA issuer waiting for TMA bytes)",
-                                };
+                                "residual (epilogue waiting for the TMA load of its residual half tile)"};
   snprintf(buf, n,
            "gemm_tc_kernel<BN=%d, MODE=%d> M=%d N=%d K=%d conv=%d splits=%d: CTA (%d,%d,%d) rank %d gave up after 4 s "
            "on barrier '%s' stage %d",
            d->bn, d->mode, d->M, d->N, d->K, d->conv, d->splits, d->bx, d->by, d->bz, d->rank,
-           names[d->tag >= 1 && d->tag <= 2 ? d->tag : 0], d->stage);
+           names[d->tag >= 1 && d->tag <= 3 ? d->tag : 0], d->stage);
   return 1;
 }
 
