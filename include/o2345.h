@@ -12,9 +12,10 @@
  *   - every pointer is a DEVICE pointer unless the name ends in _host;
  *   - all floating point data is fp32, dense and contiguous in the stated layout;
  *   - the caller allocates every buffer (outputs and scratch); nothing is allocated or
- *     freed behind the ABI and no call synchronises the device (except the four that say so:
+ *     freed behind the ABI and no call synchronises the device (except the five that say so:
  *     o2345_lod_children and o2345_surface_sample read a device-side check, o2345_simplify reads
- *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial);
+ *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial,
+ *     o2345_vertex_normals reads its checks once);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -34,7 +35,7 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 11 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 12 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
@@ -45,7 +46,9 @@ extern "C" {
                                  9: mesh scoring: o2345_surface_sample(_scratch_bytes), o2345_nearest, o2345_nn_scratch_bytes
                                 10: mesh simplification: o2345_simplify, o2345_simplify_scratch_bytes
                                 11: texture baking: o2345_texture_atlas, o2345_texel_points, o2345_texture_fill,
-                                    o2345_transfer_colors and their scratch-size functions */
+                                    o2345_transfer_colors and their scratch-size functions
+                                12: normal maps: o2345_tangent_normals, o2345_normal_quantise, o2345_vertex_normals(_scratch_bytes);
+                                    o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info) */
 
 typedef void* o2345_stream_t;
 
@@ -475,6 +478,9 @@ typedef struct o2345_raster_mesh {
   const int32_t* face_tex; /* [nf] texture of each face (-1 or >= n_tex: none), or NULL                            */
   const uint8_t* texels;   /* RGBA8 texels of every texture, row-major, packed one after another                    */
   const int32_t* tex_info; /* [n_tex,5]: first texel, width, height, wrap s, wrap t (O2345_WRAP_*)                  */
+  const float* normals;    /* [nv,3] vertex normals, or NULL (used only with tangents and face_ntex)                */
+  const float* tangents;   /* [nv,4] tangent xyz and handedness w (glTF TANGENT), or NULL                          */
+  const int32_t* face_ntex;/* [nf] tangent-space normal texture of each face (-1 or >= n_tex: none), or NULL       */
   int64_t nv, nf;
   int n_tex;
 } o2345_raster_mesh;
@@ -491,7 +497,14 @@ int64_t o2345_raster_scratch_bytes(int64_t nv, int64_t nf, int V, int W, int H);
  * index (v * H + j) * W + i: color [.,3] (perspective-correct vertex colour times the bilinear texture sample of the
  * face's texture, then the shading term), alpha (1 covered, 0 background), depth (camera z, 0 background), normal [.,3]
  * (unit world-space face normal turned toward the camera centre), tri (face index, -1 background).  Background pixels
- * are all zero. */
+ * are all zero.
+ * Normal maps: for a face with a valid face_ntex when normals and tangents are given, with the perspective-correct weights
+ * of colour and uv (fp32, rounded to nearest, no contraction):
+ *   N = normalize(interpolated normal), T = normalize(interpolated tangent xyz), w = -1 if the interpolated tangent w < 0
+ *   else 1, B = (N x T) * w, t = 2 * bilinear sample of texture face_ntex - 1, n = normalize((t.x T + t.y B) + t.z N),
+ * and s * n replaces the face normal in `normal` and in the shading term, s = +1 or -1 the sign that turns the face's
+ * normal in its own corner order toward the camera (as the face normal output is turned).
+ * A face whose N, T or n has zero or non-finite length keeps its face normal; so does every other face. */
 int o2345_raster(const o2345_raster_mesh* mesh, int V, const float* w2c, const float* intr, int W, int H, float near,
                  int shading, void* scratch, int64_t scratch_bytes, float* color, float* alpha, float* depth,
                  float* normal, int32_t* tri, o2345_stream_t stream);
@@ -613,6 +626,32 @@ int o2345_texture_fill(const int32_t* texel_index, const int32_t* count, const f
 int o2345_transfer_colors(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* colors,
                           const float* points, int64_t n, const int32_t* nn_index, const int32_t* sample_face,
                           int64_t n_samples, float* rgb, o2345_stream_t stream);
+
+/* Normal maps (o2345/mesh_texture.py, run.py / simplify_mesh.py --normal_map; mesh_io's writers and o2345_raster read the
+ * same frame).  For a face with corners P0, P1, P2 (in face order) and uv rows (u_k, v_k) (glTF: v down the image), in fp64
+ * from the fp32 inputs, every operation rounded to nearest in the order of csrc/texture.cu:
+ *   e1 = P1 - P0, e2 = P2 - P0, (du1, dv1) = uv1 - uv0, (du2, dv2) = uv2 - uv0, det = du1 dv2 - du2 dv1,
+ *   dp/du = (dv2 e1 - dv1 e2) / det, dp/dv = (du1 e2 - du2 e1) / det (per component),
+ *   T = dp/du / |dp/du|, B = -dp/dv / |dp/dv| (+Y up the image), N = (e1 x e2) / |e1 x e2|, |a| = sqrt((ax ax + ay ay) + az az);
+ *   a world normal n is coded as (n.T, n.B, n.N) / |n|, rounded to fp32.
+ * The atlas's charts are isometric, so T, B, N are orthonormal and t.x T + t.y B + t.z N decodes exactly.  A face with
+ * det = 0 (or not finite) or no area, and a normal that is zero or not finite, give (0, 0, 1).  The texel's byte code is
+ * round_half_even((c + 1) * 127.5) per component of v / |v| in fp32 (|v| as above in fp32); a vector of zero or non-finite
+ * length is (0, 0, 1), i.e. (128, 128, 255).
+ * out [n,3] fp32 := the code of normals [n,3] in the frame of face texel_face[i] with the atlas uv [nf,3,2] (a face index
+ * out of range gives NaN). */
+int o2345_tangent_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
+                          const int32_t* texel_face, const float* normals, int64_t n, float* out, o2345_stream_t stream);
+/* out [n,3] uint8 := the byte codes of texture [n,3] fp32 (after o2345_texture_fill), as above; n <= 8192^2. */
+int o2345_normal_quantise(const float* texture, int64_t n, uint8_t* out, o2345_stream_t stream);
+/* Bytes of scratch o2345_vertex_normals needs (-1 for sizes out of range). */
+int64_t o2345_vertex_normals_scratch_bytes(int64_t nv, int64_t nf);
+/* normals [nv,3] fp32: per vertex the sum of (B - A) x (C - A) (fp64) over its faces in ascending face order, divided by
+ * its length and rounded once to fp32; (0, 0, 0) for a vertex without faces or with a zero sum.  Returns O2345_EINVAL for
+ * a face index outside [0, nv) or a non-finite coordinate: this call synchronises the stream once to read that check.
+ * scratch: 16-byte aligned. */
+int o2345_vertex_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, void* scratch,
+                         int64_t scratch_bytes, float* normals, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

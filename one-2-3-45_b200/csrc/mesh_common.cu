@@ -1,4 +1,4 @@
-// The input check of the mesh calls (simplify.cu, texture.cu); see mesh_common.cuh.
+// The input check and the vertex -> face adjacency of the mesh calls (simplify.cu, texture.cu); see mesh_common.cuh.
 #include "mesh_common.cuh"
 
 namespace o2345 {
@@ -19,7 +19,47 @@ __global__ void check_kernel(const float* __restrict__ V, int64_t nv, const int3
   }
 }
 
+__global__ void degree_kernel(const int32_t* __restrict__ F, int64_t n3, int32_t* __restrict__ deg) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n3) atomicAdd(deg + F[i], 1);
+}
+
+__global__ void fill_kernel(const int32_t* __restrict__ F, int64_t n3, const int32_t* __restrict__ off,
+                            int32_t* __restrict__ cursor, int32_t* __restrict__ adj) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n3) return;
+  int v = F[i];
+  adj[off[v] + atomicAdd(cursor + v, 1)] = (int32_t)(i / 3);
+}
+
+// one thread per vertex: insertion sort of its faces by index
+__global__ void sort_kernel(const int32_t* __restrict__ off, int64_t nv, int32_t* __restrict__ adj) {
+  int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= nv) return;
+  int32_t* L = adj + off[u];
+  int d = off[u + 1] - off[u];
+  for (int i = 1; i < d; ++i) {
+    int f = L[i], j = i - 1;
+    while (j >= 0 && L[j] > f) L[j + 1] = L[j], --j;
+    L[j + 1] = f;
+  }
+}
+
 }  // namespace
+
+int vertex_faces(const int32_t* faces, int64_t nf, int64_t nv, int32_t* off, int32_t* sums, int32_t* cursor, int32_t* adj,
+                 cudaStream_t stream) {
+  const int64_t n3 = 3 * nf;
+  O2345_CUDA(cudaMemsetAsync(off, 0, 4 * (nv + 1), stream));
+  O2345_CUDA(cudaMemsetAsync(cursor, 0, 4 * nv, stream));
+  if (n3 > 0) degree_kernel<<<cdiv(n3, 256), 256, 0, stream>>>(faces, n3, off);
+  O2345_LAUNCH_CHECK();
+  O2345_TRY(scan_i32(off, nv + 1, sums, nullptr, stream));
+  if (n3 > 0) fill_kernel<<<cdiv(n3, 256), 256, 0, stream>>>(faces, n3, off, cursor, adj);
+  sort_kernel<<<cdiv(nv, 128), 128, 0, stream>>>(off, nv, adj);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
 
 int mesh_check(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, uint8_t* flags, int32_t* err,
                cudaStream_t stream) {

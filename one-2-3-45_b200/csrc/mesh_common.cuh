@@ -1,5 +1,6 @@
 // Shared pieces of the mesh kernels (metrics.cu, simplify.cu, texture.cu): fp64 vectors from the fp32 vertices with
-// explicit round-to-nearest operations in the order the numpy oracles repeat (no FMA contraction), and the input check.
+// explicit round-to-nearest operations in the order the numpy oracles repeat (no FMA contraction), the input check and
+// the vertex -> face adjacency.
 #pragma once
 #include "common.cuh"
 
@@ -37,5 +38,12 @@ __device__ __forceinline__ bool face_ok(const int c[3], int64_t nv) {
 int mesh_check(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, uint8_t* flags, int32_t* err,
                cudaStream_t stream);
 int mesh_check_status(int32_t err, const char* func);
+
+// mesh_common.cu.  Vertex -> face adjacency of faces [nf,3] whose indices all lie in [0, nv): off [nv + 1] the exclusive
+// offsets (off[nv] = 3 nf), adj [3 nf] the faces of vertex u at adj[off[u] .. off[u + 1]), ascending (a face that holds u
+// twice is listed twice).  Scratch: sums [scan_blocks(nv + 1)], cursor [nv].  Degree count, scan_i32, scatter, then one
+// thread per vertex sorts its list (the scatter's order depends on scheduling).
+int vertex_faces(const int32_t* faces, int64_t nf, int64_t nv, int32_t* off, int32_t* sums, int32_t* cursor, int32_t* adj,
+                 cudaStream_t stream);
 
 }  // namespace o2345

@@ -5,7 +5,7 @@
 //              64-bit atomicMin of (float bits of the perspective-correct camera z) << 32 | triangle id.  A triangle whose
 //              clipped bounding box holds more than `split` pixels is queued and walked by a warp instead;
 //   resolve    one thread per (view, pixel): the winner's perspective-correct barycentrics -> colour, alpha, depth,
-//              camera-facing world normal, triangle id.
+//              camera-facing world normal (the face's, or its normal map's in the interpolated tangent frame), triangle id.
 //
 // Every float operation of the vertex, depth and resolve stages is an explicit round-to-nearest intrinsic in the order
 // oracle/raster_oracle.py repeats with numpy float32 (no FMA contraction), so the triangle ids are bit-identical to the
@@ -214,6 +214,39 @@ __device__ __forceinline__ float interp(const float p[3], float a, float b, floa
   return __fadd_rn(__fadd_rn(__fmul_rn(p[0], a), __fmul_rn(p[1], b)), __fmul_rn(p[2], c));
 }
 
+// v := v / |v| in fp32; false (v unchanged) when |v| is not a positive finite number
+__device__ __forceinline__ bool normalize3(float v[3]) {
+  float l = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2])));
+  if (!(l > 0.f && l < INFINITY)) return false;
+#pragma unroll
+  for (int c = 0; c < 3; ++c) v[c] = __fdiv_rn(v[c], l);
+  return true;
+}
+
+// The normal-mapped normal at perspective-correct weights p: N = normalize(interpolated normal), T = normalize(interpolated
+// tangent xyz), B = (N x T) * w (w the sign of the interpolated tangent w), t = 2 * texel - 1, n = normalize((t.x T +
+// t.y B) + t.z N).  False when N, T or n has no direction (the face normal is kept).
+__device__ bool mapped_normal(const o2345_raster_mesh& m, const float p[3], int i0, int i1, int i2, int ntex, float u,
+                              float v, float n[3]) {
+  float N[3], T[3], t[3];
+#pragma unroll
+  for (int c = 0; c < 3; ++c) {
+    N[c] = interp(p, m.normals[3 * i0 + c], m.normals[3 * i1 + c], m.normals[3 * i2 + c]);
+    T[c] = interp(p, m.tangents[4 * i0 + c], m.tangents[4 * i1 + c], m.tangents[4 * i2 + c]);
+  }
+  if (!normalize3(N) || !normalize3(T)) return false;
+  float w = interp(p, m.tangents[4 * i0 + 3], m.tangents[4 * i1 + 3], m.tangents[4 * i2 + 3]) < 0.f ? -1.f : 1.f;
+  float B[3] = {__fmul_rn(__fsub_rn(__fmul_rn(N[1], T[2]), __fmul_rn(N[2], T[1])), w),
+                __fmul_rn(__fsub_rn(__fmul_rn(N[2], T[0]), __fmul_rn(N[0], T[2])), w),
+                __fmul_rn(__fsub_rn(__fmul_rn(N[0], T[1]), __fmul_rn(N[1], T[0])), w)};
+  sample_texture(m.texels, m.tex_info + 5 * ntex, u, v, t);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) t[c] = __fsub_rn(__fmul_rn(2.0f, t[c]), 1.0f);
+#pragma unroll
+  for (int c = 0; c < 3; ++c) n[c] = __fadd_rn(__fadd_rn(__fmul_rn(t[0], T[c]), __fmul_rn(t[1], B[c])), __fmul_rn(t[2], N[c]));
+  return normalize3(n);
+}
+
 __global__ void raster_resolve_kernel(o2345_raster_mesh m, int V, const float* __restrict__ w2c, int W, int H,
                                       const int2* __restrict__ xy, const float* __restrict__ zc, int shading,
                                       const unsigned long long* __restrict__ zbuf, float* __restrict__ color,
@@ -247,9 +280,13 @@ __global__ void raster_resolve_kernel(o2345_raster_mesh m, int V, const float* _
       rgb[0] = rgb[1] = rgb[2] = 1.f;
     }
     int tex = m.face_tex ? m.face_tex[id] : -1;
+    int ntex = m.face_ntex && m.normals && m.tangents ? m.face_ntex[id] : -1;
+    float u = 0.f, vv = 0.f;
+    if ((tex >= 0 && tex < m.n_tex) || (ntex >= 0 && ntex < m.n_tex)) {
+      u = interp(p, m.uvs[2 * i0], m.uvs[2 * i1], m.uvs[2 * i2]);
+      vv = interp(p, m.uvs[2 * i0 + 1], m.uvs[2 * i1 + 1], m.uvs[2 * i2 + 1]);
+    }
     if (tex >= 0 && tex < m.n_tex) {
-      float u = interp(p, m.uvs[2 * i0], m.uvs[2 * i1], m.uvs[2 * i2]);
-      float vv = interp(p, m.uvs[2 * i0 + 1], m.uvs[2 * i1 + 1], m.uvs[2 * i2 + 1]);
       float t[3];
       sample_texture(m.texels, m.tex_info + 5 * tex, u, vv, t);
 #pragma unroll
@@ -274,8 +311,16 @@ __global__ void raster_resolve_kernel(o2345_raster_mesh m, int V, const float* _
       face = __fadd_rn(face, __fmul_rn(n[c], __fsub_rn(cc, P0[c])));
     }
     float s = len > 0.f ? (face < 0.f ? -1.f : 1.f) : 0.f;
+    float nm[3];
+    if (len > 0.f && ntex >= 0 && ntex < m.n_tex && mapped_normal(m, p, i0, i1, i2, ntex, u, vv, nm)) {
+      // s turns the slot-ordered normal toward the camera; the map's normal takes the sign of the face's own winding
+      float sf = i1 == m.faces[3 * (int64_t)id + 1] ? s : -s;
 #pragma unroll
-    for (int c = 0; c < 3; ++c) nrm[c] = len > 0.f ? __fdiv_rn(__fmul_rn(s, n[c]), len) : 0.f;
+      for (int c = 0; c < 3; ++c) nrm[c] = __fmul_rn(sf, nm[c]);
+    } else {
+#pragma unroll
+      for (int c = 0; c < 3; ++c) nrm[c] = len > 0.f ? __fdiv_rn(__fmul_rn(s, n[c]), len) : 0.f;
+    }
     if (shading == O2345_SHADE_LAMBERT) {
       float l = __fadd_rn(0.4f, __fmul_rn(0.6f, fmaxf(nrm[2], 0.f)));
 #pragma unroll
@@ -326,6 +371,7 @@ extern "C" int o2345_raster(const o2345_raster_mesh* mesh, int V, const float* w
   O2345_CHECK_ARG(near > 0.f, "near must be > 0");
   O2345_CHECK_ARG(shading == O2345_SHADE_UNLIT || shading == O2345_SHADE_LAMBERT, "unknown shading mode");
   O2345_CHECK_ARG(!m.face_tex || (m.uvs && m.texels && m.tex_info && m.n_tex >= 1), "face_tex needs uvs, texels and tex_info");
+  O2345_CHECK_ARG(!m.face_ntex || (m.uvs && m.texels && m.tex_info && m.n_tex >= 1), "face_ntex needs uvs, texels and tex_info");
   O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_raster_scratch_bytes(m.nv, m.nf, V, W, H),
                   "scratch smaller than o2345_raster_scratch_bytes");
   O2345_CHECK_ARG(((uintptr_t)scratch & 7) == 0, "scratch must be 8-byte aligned");   // 64-bit atomics, int2 stores

@@ -2,7 +2,7 @@
 //
 //   input      one thread per face / vertex: index and finiteness checks, faces with a repeated index dropped (ordered
 //              compaction, o2345_compact);
-//   per round  vertex -> face adjacency (degree count, scan_i32, scatter, per-vertex sort by face index), then one thread per
+//   per round  vertex -> face adjacency (vertex_faces, mesh_common.cu: sorted by face index), then one thread per
 //              vertex: locks and valence; the vertex quadrics (first round only, summed in ascending face order); the
 //              proposal of every unlocked vertex (its legal neighbour with the least (cost, index)) and its claim, an
 //              atomicMin of the 64-bit key over the closed 1-rings of both ends; acceptance where the key holds every
@@ -45,33 +45,15 @@ __global__ void gather_faces_kernel(const int32_t* __restrict__ src, const int32
   dst[3 * i] = src[3 * r], dst[3 * i + 1] = src[3 * r + 1], dst[3 * i + 2] = src[3 * r + 2];
 }
 
-// ----------------------------------------------------------------------------- adjacency
-__global__ void degree_kernel(const int32_t* __restrict__ F, int64_t n3, int32_t* __restrict__ deg) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n3) atomicAdd(deg + F[i], 1);
-}
-
-__global__ void fill_kernel(const int32_t* __restrict__ F, int64_t n3, const int32_t* __restrict__ off,
-                            int32_t* __restrict__ cursor, int32_t* __restrict__ adj) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n3) return;
-  int v = F[i];
-  adj[off[v] + atomicAdd(cursor + v, 1)] = (int32_t)(i / 3);
-}
-
-// One thread per vertex: sorts its faces by index (the scatter's order depends on scheduling), counts its distinct
-// neighbours and locks it unless every edge at it has exactly two faces and its faces form one closed fan.
-__global__ void vertex_kernel(const int32_t* __restrict__ F, const int32_t* __restrict__ off, int32_t* __restrict__ adj,
+// ----------------------------------------------------------------------------- adjacency (vertex_faces, mesh_common.cu)
+// One thread per vertex: counts its distinct neighbours and locks it unless every edge at it has exactly two faces and
+// its faces form one closed fan.
+__global__ void vertex_kernel(const int32_t* __restrict__ F, const int32_t* __restrict__ off, const int32_t* __restrict__ adj,
                               int nv, uint8_t* __restrict__ locked, int32_t* __restrict__ val) {
   int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= nv) return;
-  int32_t* L = adj + off[u];
+  const int32_t* L = adj + off[u];
   int d = off[u + 1] - off[u];
-  for (int i = 1; i < d; ++i) {
-    int f = L[i], j = i - 1;
-    while (j >= 0 && L[j] > f) L[j + 1] = L[j], --j;
-    L[j + 1] = f;
-  }
   int nval = 0;
   bool ok = d > 0;
   for (int j = 0; j < d; ++j) {
@@ -379,13 +361,7 @@ extern "C" int o2345_simplify(const float* verts, int64_t nv, const int32_t* fac
   int rounds = 0;
   const int vb = cdiv(nv, 128);
   while (F > target_faces) {
-    const int64_t n3 = 3 * F;
-    O2345_CUDA(cudaMemsetAsync(S.off, 0, 4 * (nv + 1), s));
-    O2345_CUDA(cudaMemsetAsync(S.cursor, 0, 4 * nv, s));
-    degree_kernel<<<cdiv(n3, 256), 256, 0, s>>>(cur, n3, S.off);
-    O2345_LAUNCH_CHECK();
-    O2345_TRY(scan_i32(S.off, nv + 1, S.sums, nullptr, s));
-    fill_kernel<<<cdiv(n3, 256), 256, 0, s>>>(cur, n3, S.off, S.cursor, S.adj);
+    O2345_TRY(vertex_faces(cur, F, nv, S.off, S.sums, S.cursor, S.adj, s));
     vertex_kernel<<<vb, 128, 0, s>>>(cur, S.off, S.adj, (int)nv, S.locked, S.val);
     if (rounds == 0) quadric_kernel<<<vb, 128, 0, s>>>(verts, cur, S.off, S.adj, (int)nv, S.Q);
     O2345_CUDA(cudaMemsetAsync(S.claim, 0xff, 8 * nv, s));

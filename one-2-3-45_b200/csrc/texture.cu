@@ -1,6 +1,7 @@
-// Texture baking (ops.texture_atlas / texel_points / texture_fill / transfer_colors, o2345/mesh_texture.py): one isometric
-// chart per face, packed on shelves into an N x N atlas, the surface point behind every texel of a chart, push-pull fill
-// of the texels no chart owns, and the colour of a point taken from the nearest face of a source mesh.
+// Texture baking (ops.texture_atlas / texel_points / texture_fill / transfer_colors / tangent_normals / normal_quantise /
+// vertex_normals, o2345/mesh_texture.py): one isometric chart per face, packed on shelves into an N x N atlas, the surface
+// point behind every texel of a chart, push-pull fill of the texels no chart owns, the colour of a point taken from the
+// nearest face of a source mesh, and normal maps: world normals in each face's tangent frame, quantised to uint8.
 //
 //   atlas         one thread per face: the chart (base = the longest edge by fp32 squared length, first on ties; L, d, h in
 //                 fp64 rounded once to fp32) and L * h in fp64; the sum of L * h in a fixed order (cumsum_f64_chunked, scan.cu:
@@ -14,7 +15,11 @@
 //   fill          the owned texels' colours scattered into the texture, a pull pyramid of weighted 2 x 2 means and a push
 //                 pass that hands every empty texel its parent's value;
 //   transfer      one thread per point: the closest point of the source face behind the point's nearest surface sample
-//                 and the face's vertex colours interpolated there.
+//                 and the face's vertex colours interpolated there;
+//   tangent       one thread per owned texel: the face's frame (T, B, N) from its corners and uv in fp64 and the world
+//                 normal's coordinates in it; quantise: one thread per texel, renormalised in fp32 and coded to uint8;
+//   vertex normal vertex -> face adjacency (vertex_faces, mesh_common.cu), then one thread per vertex: the sum of its
+//                 faces' (B - A) x (C - A) in ascending face order in fp64, normalised, rounded once to fp32.
 //
 // Every floating-point operation is an explicit round-to-nearest intrinsic in the order oracle/texture_oracle.py repeats
 // with numpy (no FMA contraction), so every output is bit-identical to the oracle and independent of thread scheduling.
@@ -367,6 +372,99 @@ __global__ void transfer_kernel(const float* __restrict__ V, int64_t nv, const i
   blend3(l, colors + 3 * (int64_t)c[0], colors + 3 * (int64_t)c[1], colors + 3 * (int64_t)c[2], rgb + 3 * i);
 }
 
+// ----------------------------------------------------------------------------- normal maps
+__device__ __forceinline__ D3 scale3(D3 a, double s) { return {__dmul_rn(a.x, s), __dmul_rn(a.y, s), __dmul_rn(a.z, s)}; }
+
+// a / |a| in fp64; false when |a| is not a positive finite number
+__device__ __forceinline__ bool unit3(D3 a, D3& out) {
+  double l = __dsqrt_rn(dot3(a, a));
+  if (!(l > 0.0 && l < INFINITY)) return false;
+  out = {__ddiv_rn(a.x, l), __ddiv_rn(a.y, l), __ddiv_rn(a.z, l)};
+  return true;
+}
+
+// One thread per texel: the tangent-space coordinates of world normal nw[i] in the frame of face texel_face[i] (rule in
+// include/o2345.h): T = dp/du, B = -dp/dv, N = e1 x e2, each normalised; (0, 0, 1) for a degenerate face or a zero or
+// non-finite normal, NaN for a face index out of range.
+__global__ void tangent_kernel(const float* __restrict__ V, int64_t nv, const int32_t* __restrict__ F, int64_t nf,
+                               const float* __restrict__ uv, const int32_t* __restrict__ texel_face,
+                               const float* __restrict__ nw, int64_t n, float* __restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  int64_t f = texel_face[i];
+  int c[3] = {-1, -1, -1};
+  if (f >= 0 && f < nf) c[0] = F[3 * f], c[1] = F[3 * f + 1], c[2] = F[3 * f + 2];
+  if (!face_ok(c, nv)) {
+    out[3 * i] = out[3 * i + 1] = out[3 * i + 2] = __int_as_float(0x7fc00000);
+    return;
+  }
+  float t[3] = {0.f, 0.f, 1.f};
+  D3 P0 = vert(V, c[0]), P1 = vert(V, c[1]), P2 = vert(V, c[2]), e1 = sub3(P1, P0), e2 = sub3(P2, P0);
+  const float* q = uv + 6 * f;
+  double du1 = __dsub_rn((double)q[2], (double)q[0]), dv1 = __dsub_rn((double)q[3], (double)q[1]);
+  double du2 = __dsub_rn((double)q[4], (double)q[0]), dv2 = __dsub_rn((double)q[5], (double)q[1]);
+  double det = __dsub_rn(__dmul_rn(du1, dv2), __dmul_rn(du2, dv1));
+  D3 w = {(double)nw[3 * i], (double)nw[3 * i + 1], (double)nw[3 * i + 2]};
+  double ln = __dsqrt_rn(dot3(w, w));
+  D3 T, B, N;
+  if (fabs(det) > 0.0 && ln > 0.0 && ln < INFINITY) {
+    D3 dpdu = sub3(scale3(e1, dv2), scale3(e2, dv1)), dpdv = sub3(scale3(e2, du1), scale3(e1, du2));
+    dpdu = {__ddiv_rn(dpdu.x, det), __ddiv_rn(dpdu.y, det), __ddiv_rn(dpdu.z, det)};
+    dpdv = {__ddiv_rn(-dpdv.x, det), __ddiv_rn(-dpdv.y, det), __ddiv_rn(-dpdv.z, det)};
+    if (unit3(dpdu, T) && unit3(dpdv, B) && unit3(cross3(P0, P1, P2), N)) {
+      t[0] = __double2float_rn(__ddiv_rn(dot3(w, T), ln));
+      t[1] = __double2float_rn(__ddiv_rn(dot3(w, B), ln));
+      t[2] = __double2float_rn(__ddiv_rn(dot3(w, N), ln));
+    }
+  }
+  out[3 * i] = t[0], out[3 * i + 1] = t[1], out[3 * i + 2] = t[2];
+}
+
+// One thread per texel: v / |v| in fp32 ((0, 0, 1) when |v| is zero or not finite), each component coded as
+// round_half_even((c + 1) * 127.5).
+__global__ void quantise_kernel(const float* __restrict__ tex, int64_t n, uint8_t* __restrict__ out) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float v[3] = {tex[3 * i], tex[3 * i + 1], tex[3 * i + 2]};
+  float l = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(v[0], v[0]), __fmul_rn(v[1], v[1])), __fmul_rn(v[2], v[2])));
+  bool ok = l > 0.f && l < INFINITY;
+#pragma unroll
+  for (int k = 0; k < 3; ++k) {
+    float c = ok ? __fdiv_rn(v[k], l) : (k == 2 ? 1.f : 0.f);
+    int b = __float2int_rn(__fmul_rn(__fadd_rn(c, 1.f), 127.5f));
+    out[3 * i + k] = (uint8_t)min(max(b, 0), 255);
+  }
+}
+
+// One thread per vertex: the sum of its faces' (B - A) x (C - A) in ascending face order (fp64), normalised, rounded to
+// fp32; (0, 0, 0) for a zero sum.
+__global__ void vertex_normal_kernel(const float* __restrict__ V, const int32_t* __restrict__ F,
+                                     const int32_t* __restrict__ off, const int32_t* __restrict__ adj, int64_t nv,
+                                     float* __restrict__ out) {
+  int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (u >= nv) return;
+  D3 s = {0.0, 0.0, 0.0};
+  for (int j = off[u]; j < off[u + 1]; ++j) {
+    int64_t f = adj[j];
+    D3 n = cross3(vert(V, F[3 * f]), vert(V, F[3 * f + 1]), vert(V, F[3 * f + 2]));
+    s = {__dadd_rn(s.x, n.x), __dadd_rn(s.y, n.y), __dadd_rn(s.z, n.z)};
+  }
+  D3 r = {0.0, 0.0, 0.0};
+  unit3(s, r);
+  out[3 * u] = __double2float_rn(r.x), out[3 * u + 1] = __double2float_rn(r.y), out[3 * u + 2] = __double2float_rn(r.z);
+}
+
+// The scratch of o2345_vertex_normals, carved in this order (a Carver without a base only measures it).
+struct NormalScratch {
+  int64_t nv, nf;
+  Carver c;
+  int32_t* off = c.take<int32_t>(nv + 1);
+  int32_t* sums = c.take<int32_t>(scan_blocks(nv + 1));
+  int32_t* cursor = c.take<int32_t>(nv);
+  int32_t* adj = c.take<int32_t>(3 * nf);
+  int32_t* err = c.take<int32_t>(1);
+};
+
 }  // namespace
 }  // namespace o2345
 
@@ -500,6 +598,53 @@ extern "C" int o2345_transfer_colors(const float* verts, int64_t nv, const int32
   O2345_CHECK_ARG(n >= 1 && n <= INT32_MAX && n_samples >= 1 && n_samples <= INT32_MAX, "need 1 <= n, n_samples <= 2^31-1");
   cudaStream_t s = (cudaStream_t)stream;
   transfer_kernel<<<cdiv(n, 128), 128, 0, s>>>(verts, nv, faces, nf, colors, points, n, nn_index, sample_face, n_samples, rgb);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+extern "C" int o2345_tangent_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
+                                     const int32_t* texel_face, const float* normals, int64_t n, float* out,
+                                     o2345_stream_t stream) {
+  O2345_CHECK_ARG(verts && faces && uv && texel_face && normals && out, "verts, faces, uv, texel_face, normals and out are required");
+  O2345_CHECK_ARG(nv >= 1 && nv <= INT32_MAX && nf >= 1 && nf <= INT32_MAX / 3, "need 1 <= nv <= 2^31-1 and 1 <= nf <= (2^31-1)/3");
+  O2345_CHECK_ARG(n >= 1 && n <= INT32_MAX, "need 1 <= n <= 2^31-1");
+  cudaStream_t s = (cudaStream_t)stream;
+  tangent_kernel<<<cdiv(n, 128), 128, 0, s>>>(verts, nv, faces, nf, uv, texel_face, normals, n, out);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+extern "C" int o2345_normal_quantise(const float* texture, int64_t n, uint8_t* out, o2345_stream_t stream) {
+  O2345_CHECK_ARG(texture && out, "texture and out are required");
+  O2345_CHECK_ARG(n >= 1 && n <= (int64_t)kMaxN * kMaxN, "need 1 <= n <= 8192^2");
+  cudaStream_t s = (cudaStream_t)stream;
+  quantise_kernel<<<cdiv(n, 256), 256, 0, s>>>(texture, n, out);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+extern "C" int64_t o2345_vertex_normals_scratch_bytes(int64_t nv, int64_t nf) {
+  if (nv < 1 || nv > INT32_MAX - 1 || nf < 1 || nf > INT32_MAX / 3) return -1;
+  return NormalScratch{nv, nf, {}}.c.bytes;
+}
+
+extern "C" int o2345_vertex_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, void* scratch,
+                                    int64_t scratch_bytes, float* normals, o2345_stream_t stream) {
+  O2345_CHECK_ARG(verts && faces && normals, "verts, faces and normals are required");
+  O2345_CHECK_ARG(nv >= 1 && nv <= INT32_MAX - 1 && nf >= 1 && nf <= INT32_MAX / 3, "need 1 <= nv < 2^31-1 and 1 <= nf <= (2^31-1)/3");
+  O2345_CHECK_ARG(scratch && scratch_bytes >= o2345_vertex_normals_scratch_bytes(nv, nf),
+                  "scratch smaller than o2345_vertex_normals_scratch_bytes");
+  O2345_CHECK_ARG(((uintptr_t)scratch & 15) == 0, "scratch must be 16-byte aligned");
+  cudaStream_t s = (cudaStream_t)stream;
+  NormalScratch S{nv, nf, {(char*)scratch}};
+  O2345_CUDA(cudaMemsetAsync(S.err, 0, 4, s));
+  O2345_TRY(mesh_check(verts, nv, faces, nf, nullptr, S.err, s));
+  int32_t err = 0;   // the adjacency scatters through the face indices: they are checked on the host first
+  O2345_CUDA(cudaMemcpyAsync(&err, S.err, 4, cudaMemcpyDeviceToHost, s));
+  O2345_CUDA(cudaStreamSynchronize(s));
+  O2345_TRY(mesh_check_status(err, __func__));
+  O2345_TRY(vertex_faces(faces, nf, nv, S.off, S.sums, S.cursor, S.adj, s));
+  vertex_normal_kernel<<<cdiv(nv, 128), 128, 0, s>>>(verts, faces, S.off, S.adj, nv, normals);
   O2345_LAUNCH_CHECK();
   return O2345_OK;
 }

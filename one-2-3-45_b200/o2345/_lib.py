@@ -37,7 +37,8 @@ class Epilogue(C.Structure):
 
 class RasterMesh(C.Structure):
     _fields_ = [("verts", c_fp), ("colors", c_fp), ("uvs", c_fp), ("faces", c_fp), ("face_tex", c_fp), ("texels", c_fp),
-                ("tex_info", c_fp), ("nv", c_i64), ("nf", c_i64), ("n_tex", C.c_int)]
+                ("tex_info", c_fp), ("normals", c_fp), ("tangents", c_fp), ("face_ntex", c_fp), ("nv", c_i64), ("nf", c_i64),
+                ("n_tex", C.c_int)]
 
 
 PTS_EXPLICIT, PTS_LATTICE, PTS_RAYS = 0, 1, 2
@@ -148,12 +149,16 @@ _SIGS = {
     "o2345_texture_fill_scratch_bytes": (c_i64, [C.c_int]),
     "o2345_texture_fill": (C.c_int, [c_fp, c_fp, c_fp, c_fp, C.c_int, c_fp, c_i64, c_fp, c_fp]),
     "o2345_transfer_colors": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, c_fp]),
+    "o2345_tangent_normals": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp, c_i64, c_fp, c_fp]),
+    "o2345_normal_quantise": (C.c_int, [c_fp, c_i64, c_fp, c_fp]),
+    "o2345_vertex_normals_scratch_bytes": (c_i64, [c_i64, c_i64]),
+    "o2345_vertex_normals": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 11         # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 12         # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 
@@ -192,7 +197,7 @@ def last_error() -> str:
 
 
 # kernels launched per successful entry-point call (memsets are not counted)
-_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4, "o2345_surface_sample": 5, "o2345_nearest": 7, "o2345_texel_points": 5}
+_KERNELS_PER_CALL = {"o2345_compact": 3, "o2345_prune_by_sdf": 3, "o2345_sp_coarsen": 3, "o2345_mc_tri_offsets": 4, "o2345_conv_up2x_f16": 4, "o2345_raster": 4, "o2345_surface_sample": 5, "o2345_nearest": 7, "o2345_texel_points": 5, "o2345_vertex_normals": 8}
 _launches = 0
 
 

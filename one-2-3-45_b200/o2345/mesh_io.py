@@ -13,7 +13,8 @@ Restates, on plain numpy arrays:
                             faces -- then `.obj` with `v x y z r g b` lines (trimesh's include_color=True) or a binary glTF.
   * `write_textured_glb` / `write_textured_obj`
                             a mesh with per-corner uv and a colour texture (o2345/mesh_texture.py; not in the reference):
-                            glTF with an embedded PNG as baseColorTexture, or OBJ + MTL (map_Kd) + PNG.
+                            glTF with an embedded PNG as baseColorTexture, or OBJ + MTL (map_Kd) + PNG; optionally a
+                            tangent-space normal map in the frame of `tangent_frames` (normalTexture, or `norm` in the MTL).
 """
 from __future__ import annotations
 
@@ -165,11 +166,37 @@ def _png_bytes(texture):
     return buf.getvalue()
 
 
-def write_textured_glb(path, vertices, triangles, uv, texture):
+def tangent_frames(vertices, triangles, uv):
+    """The tangent frame of every face (include/o2345.h, the rule the normal-map baker codes with): in fp64 from the fp32
+    corners and uv rows (glTF: v down the image), T = dp/du, B = -dp/dv (+Y up the image), N = e1 x e2 (the winding as
+    given), each normalised -> T, B, N float64 [m,3].  A degenerate face gets N = (0, 0, 1) where e1 x e2 = 0 and
+    T = (1, 0, 0), B = N x T where its uv have no area."""
+    v = np.asarray(vertices, np.float32).astype(np.float64)
+    f = np.asarray(triangles, np.int64).reshape(-1, 3)
+    q = np.asarray(uv, np.float32).reshape(-1, 3, 2).astype(np.float64)
+    e1, e2 = v[f[:, 1]] - v[f[:, 0]], v[f[:, 2]] - v[f[:, 0]]
+    d1, d2 = q[:, 1] - q[:, 0], q[:, 2] - q[:, 0]
+    det = d1[:, 0] * d2[:, 1] - d2[:, 0] * d1[:, 1]
+
+    def unit(a, fallback):
+        ln = np.linalg.norm(a, axis=1, keepdims=True)
+        ok = (ln > 0) & np.isfinite(ln)
+        return np.where(ok, a / np.where(ok, ln, 1.0), fallback)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        s = np.where(det != 0, 1.0 / np.where(det != 0, det, 1.0), 0.0)[:, None]
+    N = unit(np.cross(e1, e2), np.array([0.0, 0.0, 1.0]))
+    T = unit((d2[:, 1:2] * e1 - d1[:, 1:2] * e2) * s, np.array([1.0, 0.0, 0.0]))
+    B = unit(-(d1[:, 0:1] * e2 - d2[:, 0:1] * e1) * s, np.cross(N, T))
+    return T, B, N
+
+
+def write_textured_glb(path, vertices, triangles, uv, texture, normal_texture=None):
     """Binary glTF 2.0 of a textured mesh: vertices [n,3], triangles [m,3], uv [m,3,2] (row k for corner k, glTF's
     convention), texture uint8 [N,N,3].  Vertices are split per corner (3m of them: POSITION float32, TEXCOORD_0 float32,
     uint32 indices 0 .. 3m-1) and the material is unlit-friendly PBR: the texture as an embedded PNG baseColorTexture
-    (CLAMP_TO_EDGE, LINEAR), metallic 0, roughness 1.  No COLOR_0."""
+    (CLAMP_TO_EDGE, LINEAR), metallic 0, roughness 1.  No COLOR_0.  With normal_texture uint8 [N,N,3] (tangent space, in
+    the frame of tangent_frames) the corners also get NORMAL (the face normal of the written winding) and TANGENT (T, w)
+    with w = sign((N x T) . B) in this frame, and the material a normalTexture (a second PNG)."""
     f = np.asarray(triangles, np.int64).reshape(-1, 3)
     v = np.ascontiguousarray(np.asarray(vertices, np.float32)[f.reshape(-1)])
     t = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 2))
@@ -177,6 +204,12 @@ def write_textured_glb(path, vertices, triangles, uv, texture):
         raise ValueError(f"uv has {len(t) // 3} faces, triangles {len(f)}")
     idx = np.arange(len(v), dtype=np.uint32)
     blobs = [v.tobytes(), t.tobytes(), idx.tobytes(), _png_bytes(texture)]
+    if normal_texture is not None:
+        T, B, N = tangent_frames(vertices, f, uv)
+        w = np.where(np.einsum("ij,ij->i", np.cross(N, T), B) < 0, -1.0, 1.0)
+        nrm = np.ascontiguousarray(np.repeat(N, 3, 0).astype(np.float32))
+        tan = np.ascontiguousarray(np.repeat(np.concatenate([T, w[:, None]], 1), 3, 0).astype(np.float32))
+        blobs += [_png_bytes(normal_texture), nrm.tobytes(), tan.tobytes()]
     offs, total = [], 0
     for b in blobs:
         offs.append(total)
@@ -202,6 +235,16 @@ def write_textured_glb(path, vertices, triangles, uv, texture):
                       {"bufferView": 1, "componentType": 5126, "count": int(len(t)), "type": "VEC2"},
                       {"bufferView": 2, "componentType": 5125, "count": int(len(idx)), "type": "SCALAR"}],
     }
+    if normal_texture is not None:
+        doc["meshes"][0]["primitives"][0]["attributes"].update(NORMAL=3, TANGENT=4)
+        doc["materials"][0]["normalTexture"] = {"index": 1}
+        doc["textures"].append({"sampler": 0, "source": 1})
+        doc["images"].append({"bufferView": 4, "mimeType": "image/png"})
+        doc["bufferViews"] += [{"buffer": 0, "byteOffset": offs[4], "byteLength": len(blobs[4])},
+                               {"buffer": 0, "byteOffset": offs[5], "byteLength": len(blobs[5]), "target": 34962},
+                               {"buffer": 0, "byteOffset": offs[6], "byteLength": len(blobs[6]), "target": 34962}]
+        doc["accessors"] += [{"bufferView": 5, "componentType": 5126, "count": int(len(v)), "type": "VEC3"},
+                             {"bufferView": 6, "componentType": 5126, "count": int(len(v)), "type": "VEC4"}]
     js = json.dumps(doc, separators=(",", ":")).encode("utf-8")
     js += b" " * ((4 - len(js) % 4) % 4)
     with open(path, "wb") as fh:
@@ -212,9 +255,11 @@ def write_textured_glb(path, vertices, triangles, uv, texture):
         fh.write(bytes(bin_chunk))
 
 
-def write_textured_obj(path, vertices, triangles, uv, texture):
+def write_textured_obj(path, vertices, triangles, uv, texture, normal_texture=None):
     """Wavefront OBJ of a textured mesh beside its material: `v x y z`, then one `vt u (1 - v)` per face corner (OBJ's v
-    points up the image), then `f a/t b/t c/t`; <stem>.mtl (`map_Kd <stem>_albedo.png`) and the PNG next to it."""
+    points up the image), then `f a/t b/t c/t`; <stem>.mtl (`map_Kd <stem>_albedo.png`) and the PNG next to it.  With
+    normal_texture uint8 [N,N,3] (tangent space, the frame of tangent_frames) also one `vn` per face (its normal),
+    `f a/t/n ...`, <stem>_normal.png and `norm <stem>_normal.png` in the MTL."""
     import os
     stem = os.path.splitext(os.path.basename(path))[0]
     folder = os.path.dirname(os.path.abspath(path))
@@ -223,25 +268,36 @@ def write_textured_obj(path, vertices, triangles, uv, texture):
     t = np.asarray(uv, np.float64).reshape(-1, 2)
     with open(os.path.join(folder, stem + "_albedo.png"), "wb") as fh:
         fh.write(_png_bytes(texture))
+    mtl = "# o2345-b200\nnewmtl albedo\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd %s_albedo.png\n" % stem
+    if normal_texture is not None:
+        with open(os.path.join(folder, stem + "_normal.png"), "wb") as fh:
+            fh.write(_png_bytes(normal_texture))
+        mtl += "norm %s_normal.png\n" % stem
     with open(os.path.join(folder, stem + ".mtl"), "w") as fh:
-        fh.write("# o2345-b200\nnewmtl albedo\nKa 1 1 1\nKd 1 1 1\nKs 0 0 0\nillum 1\nmap_Kd %s_albedo.png\n" % stem)
+        fh.write(mtl)
     with open(path, "w") as fh:
         fh.write("# o2345-b200\nmtllib %s.mtl\n" % stem)
         for p in v:
             fh.write("v %.8f %.8f %.8f\n" % (p[0], p[1], p[2]))
         for q in t:
             fh.write("vt %.8f %.8f\n" % (q[0], 1.0 - q[1]))
+        if normal_texture is not None:
+            for n in tangent_frames(v, f, uv)[2]:
+                fh.write("vn %.8f %.8f %.8f\n" % (n[0], n[1], n[2]))
         fh.write("usemtl albedo\n")
         for i, q in enumerate(f + 1):
-            fh.write("f %d/%d %d/%d %d/%d\n" % (q[0], 3 * i + 1, q[1], 3 * i + 2, q[2], 3 * i + 3))
+            if normal_texture is None:
+                fh.write("f %d/%d %d/%d %d/%d\n" % (q[0], 3 * i + 1, q[1], 3 * i + 2, q[2], 3 * i + 3))
+            else:
+                fh.write("f %d/%d/%d %d/%d/%d %d/%d/%d\n" % (q[0], 3 * i + 1, i + 1, q[1], 3 * i + 2, i + 1, q[2], 3 * i + 3, i + 1))
 
 
-def write_textured(path, vertices, triangles, uv, texture):
+def write_textured(path, vertices, triangles, uv, texture, normal_texture=None):
     """write_textured_glb or write_textured_obj by the extension of path."""
     if path.lower().endswith(".glb"):
-        return write_textured_glb(path, vertices, triangles, uv, texture)
+        return write_textured_glb(path, vertices, triangles, uv, texture, normal_texture)
     if path.lower().endswith(".obj"):
-        return write_textured_obj(path, vertices, triangles, uv, texture)
+        return write_textured_obj(path, vertices, triangles, uv, texture, normal_texture)
     raise ValueError(f"{path}: a textured mesh is written as .glb or .obj")
 
 
@@ -336,11 +392,14 @@ def read_glb(path):
       roots     [4x4] world matrix of every root node of the default scene that has a mesh below it;
       meshes    one entry per node with a mesh: verts [n,3], faces [m,3] (every indexed or non-indexed triangle primitive of
                 the mesh, joined), colors [n,3] (COLOR_0 times the material's baseColorFactor, white without either), uvs
-                [n,2] (TEXCOORD_0, or None), face_tex [m] (texture of the material's baseColorTexture, -1 without), root
-                (index into roots), local_to_root [4x4] (product of the node matrices below the root's own);
+                [n,2] (TEXCOORD_0, or None), face_tex [m] (texture of the material's baseColorTexture, -1 without), normals
+                [n,3] (NORMAL, zeros for a primitive without, or None), tangents [n,4] (TANGENT alike), face_ntex [m]
+                (texture of the material's normalTexture where the primitive has TEXCOORD_0, NORMAL and TANGENT, -1
+                without), root (index into roots), local_to_root [4x4] (product of the node matrices below the root's
+                own);
       textures  [(RGBA uint8 [h,w,4], wrap s, wrap t)] decoded with PIL.
-    All in glTF's own (Y-up) axes.  Primitives that are not triangle lists, alpha modes, normal / occlusion /
-    metallic-roughness textures and texture transforms are ignored; a texture is sampled at TEXCOORD_0."""
+    All in glTF's own (Y-up) axes.  Primitives that are not triangle lists, alpha modes, occlusion / metallic-roughness
+    textures, the normal map's scale and texture transforms are ignored; a texture is sampled at TEXCOORD_0."""
     import io
     raw = open(path, "rb").read()
     magic, version, _ = struct.unpack_from("<III", raw, 0)
@@ -379,7 +438,7 @@ def read_glb(path):
         return tex_of_image[key]
 
     def mesh(mi):
-        vs, fs, cs, us, ts, n = [], [], [], [], [], 0
+        vs, fs, cs, us, ts, ns, gs, nts, n = [], [], [], [], [], [], [], [], 0
         for prim in doc["meshes"][mi]["primitives"]:
             if prim.get("mode", 4) != 4:
                 continue
@@ -394,6 +453,10 @@ def read_glb(path):
                 c = _glb_accessor(doc, binary, att["COLOR_0"])[:, :3].astype(np.float64)
             c = c * np.asarray(pbr.get("baseColorFactor", [1.0, 1.0, 1.0, 1.0])[:3], np.float64)
             tex = texture(pbr["baseColorTexture"]["index"]) if "baseColorTexture" in pbr and "TEXCOORD_0" in att else -1
+            mapped = "normalTexture" in mat and all(k in att for k in ("TEXCOORD_0", "NORMAL", "TANGENT"))
+            nts.append(np.full(len(f), texture(mat["normalTexture"]["index"]) if mapped else -1, np.int64))
+            ns.append(_glb_accessor(doc, binary, att["NORMAL"])[:, :3] if "NORMAL" in att else np.zeros((len(v), 3)))
+            gs.append(_glb_accessor(doc, binary, att["TANGENT"])[:, :4] if "TANGENT" in att else np.zeros((len(v), 4)))
             vs.append(v[:, :3])
             fs.append(f + n)
             cs.append(c)
@@ -402,9 +465,11 @@ def read_glb(path):
             n += len(v)
         if not vs:
             return None
-        has_uv = any("TEXCOORD_0" in p["attributes"] for p in doc["meshes"][mi]["primitives"])
+        has = lambda key: any(key in p["attributes"] for p in doc["meshes"][mi]["primitives"])
         return {"verts": np.concatenate(vs), "faces": np.concatenate(fs), "colors": np.concatenate(cs),
-                "uvs": np.concatenate(us) if has_uv else None, "face_tex": np.concatenate(ts)}
+                "uvs": np.concatenate(us) if has("TEXCOORD_0") else None, "face_tex": np.concatenate(ts),
+                "normals": np.concatenate(ns) if has("NORMAL") else None,
+                "tangents": np.concatenate(gs) if has("TANGENT") else None, "face_ntex": np.concatenate(nts)}
 
     roots, meshes = [], []
 

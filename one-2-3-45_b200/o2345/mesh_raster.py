@@ -17,7 +17,9 @@ render/launch_render_eval.py under Blender 3.6 + BlenderProc), restated from the
 Parity unpinned: neither Blender nor BlenderProc is available, so the rig is restated from the script's code, not pinned
 against renders.  Geometry, silhouette and depth follow the rig; colour is a defined model (unlit base colour, or the
 Lambert stand-in of O2345_SHADE_LAMBERT for the rig's overhead area light), not Cycles' lighting or the Filmic view
-transform.  glTF alpha modes, normal maps and metallic-roughness are ignored: the base colour is opaque."""
+transform.  A glTF normal map (normalTexture with NORMAL and TANGENT) replaces the face normal in the normal output and
+the Lambert term; a NORMAL without a normal map does not (faces stay flat).  Alpha modes and metallic-roughness are
+ignored: the base colour is opaque."""
 from __future__ import annotations
 
 import math
@@ -40,7 +42,8 @@ def _h(R):
 
 def load_scene(path, y_up=None):
     """-> scene dict in Blender's axes: roots [4x4 world matrices], meshes (verts local, faces, colors or None, uvs or None,
-    face_tex or None, root, local_to_root) and textures [(RGBA [h,w,4], wrap s, wrap t)].  y_up overrides the format's axis
+    face_tex or None, normals / tangents / face_ntex or None (GLB only), root, local_to_root) and textures
+    [(RGBA [h,w,4], wrap s, wrap t)].  y_up overrides the format's axis
     convention (True: apply the Y-up -> Z-up change, False: none)."""
     ext = os.path.splitext(path)[1].lower()
     if ext == ".glb":
@@ -68,6 +71,10 @@ def load_scene(path, y_up=None):
         for m in meshes:
             m["verts"] = m["verts"] @ Y_UP_TO_Z_UP.T
             m["local_to_root"] = C @ m["local_to_root"] @ C.T
+            if m.get("normals") is not None:       # a rotation: normals and tangents turn like positions
+                m["normals"] = m["normals"] @ Y_UP_TO_Z_UP.T
+            if m.get("tangents") is not None:
+                m["tangents"] = np.concatenate([m["tangents"][:, :3] @ Y_UP_TO_Z_UP.T, m["tangents"][:, 3:]], 1)
     return {"roots": [np.asarray(R, np.float64) for R in roots], "meshes": meshes, "textures": textures}
 
 
@@ -100,23 +107,39 @@ def normalize_scene(scene):
 def flatten(scene):
     """World-space arrays of ops.raster / oracle.raster_oracle.render: verts float32 [nv,3], faces int32 [nf,3], colors
     float32 [nv,3] (or None when no object has any), uvs float32 [nv,2] + face_tex int32 [nf] + texels uint8 + tex_info
-    int32 [n_tex,5] (or None when no face is textured)."""
-    vs, fs, cs, us, ts, n = [], [], [], [], [], 0
+    int32 [n_tex,5] (or None when no face is textured), normals float32 [nv,3] + tangents float32 [nv,4] + face_ntex int32
+    [nf] (or None when no face has a normal map).  Tangents go through each object's linear part A, normals through
+    A^-T, and the tangent w is multiplied by sign(det A)."""
+    vs, fs, cs, us, ts, ns, gs, nts, n = [], [], [], [], [], [], [], [], 0
     any_col = any(m["colors"] is not None for m in scene["meshes"])
     for m in scene["meshes"]:
         M = scene["roots"][m["root"]] @ m["local_to_root"]
-        v = m["verts"] @ M[:3, :3].T + M[:3, 3]
+        A = M[:3, :3]
+        v = m["verts"] @ A.T + M[:3, 3]
         vs.append(v)
         fs.append(m["faces"] + n)
         cs.append(m["colors"] if m["colors"] is not None else np.ones((len(v), 3)))
         us.append(m["uvs"] if m["uvs"] is not None else np.zeros((len(v), 2)))
         ts.append(m["face_tex"] if m["face_tex"] is not None else np.full(len(m["faces"]), -1))
+        nts.append(m["face_ntex"] if m.get("face_ntex") is not None else np.full(len(m["faces"]), -1))
+        if (nts[-1] >= 0).any():
+            ns.append(m["normals"] @ np.linalg.inv(A))
+            g = m["tangents"]
+            gs.append(np.concatenate([g[:, :3] @ A.T, g[:, 3:] * np.sign(np.linalg.det(A))], 1))
+        else:
+            ns.append(np.zeros((len(v), 3)))
+            gs.append(np.zeros((len(v), 4)))
         n += len(v)
     out = {"verts": np.concatenate(vs).astype(np.float32), "faces": np.concatenate(fs).astype(np.int32),
            "colors": np.concatenate(cs).astype(np.float32) if any_col else None,
-           "uvs": None, "face_tex": None, "texels": None, "tex_info": None}
+           "uvs": None, "face_tex": None, "texels": None, "tex_info": None, "normals": None, "tangents": None,
+           "face_ntex": None}
     face_tex = np.concatenate(ts).astype(np.int32)
-    if scene["textures"] and (face_tex >= 0).any():
+    face_ntex = np.concatenate(nts).astype(np.int32)
+    if scene["textures"] and (face_ntex >= 0).any():
+        out.update(normals=np.concatenate(ns).astype(np.float32), tangents=np.concatenate(gs).astype(np.float32),
+                   face_ntex=face_ntex)
+    if scene["textures"] and ((face_tex >= 0).any() or (face_ntex >= 0).any()):
         info, first = [], 0
         for rgba, ws, wt in scene["textures"]:
             info.append([first, rgba.shape[1], rgba.shape[0], ws, wt])
@@ -156,8 +179,8 @@ def camera_arrays(c2w, K):
 
 def render(flat, c2w, K, W, H, shading="unlit", near=NEAR, device="cuda"):
     """Renders flatten()'s arrays from cameras c2w [V,4,4] (OpenCV) with intrinsics K -> device tensors color [V,H,W,3],
-    alpha [V,H,W], depth [V,H,W] (camera z, 0 on the background), normal [V,H,W,3] (unit world face normal toward the
-    camera), tri [V,H,W] int32 (face index into flat['faces'], -1 on the background)."""
+    alpha [V,H,W], depth [V,H,W] (camera z, 0 on the background), normal [V,H,W,3] (unit world face normal, or the normal
+    map's, toward the camera), tri [V,H,W] int32 (face index into flat['faces'], -1 on the background)."""
     import torch
     from . import ops
     if shading not in SHADINGS:
@@ -168,7 +191,8 @@ def render(flat, c2w, K, W, H, shading="unlit", near=NEAR, device="cuda"):
     with torch.cuda.device(dev):
         return ops.raster(t(flat["verts"]), t(flat["faces"]), t(w2c), t(intr), int(W), int(H), near=near,
                           shading=SHADINGS[shading], colors=t(flat["colors"]), uvs=t(flat["uvs"]),
-                          face_tex=t(flat["face_tex"]), texels=t(flat["texels"]), tex_info=t(flat["tex_info"]))
+                          face_tex=t(flat["face_tex"]), texels=t(flat["texels"]), tex_info=t(flat["tex_info"]),
+                          normals=t(flat.get("normals")), tangents=t(flat.get("tangents")), face_ntex=t(flat.get("face_ntex")))
 
 
 def render_rig(path, camera_dist=1.5, resolution=512, shading="unlit", device="cuda"):

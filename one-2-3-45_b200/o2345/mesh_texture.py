@@ -2,7 +2,12 @@
 gets its own chart in an N x N atlas (ops.texture_atlas), the surface point behind every texel a chart owns is evaluated
 by a colour function (ops.texel_points), and the texels no chart owns are filled by push-pull (ops.texture_fill), all in
 csrc/texture.cu.  The colour function is the reconstruction's (SparseNeuSRenderer.blend_points, the one that colours the
-vertices) or, for a mesh without a reconstruction, the colours of a source mesh (transfer_fn)."""
+vertices) or, for a mesh without a reconstruction, the colours of a source mesh (transfer_fn).
+
+A normal map shares the atlas and the texel points: a normal function gives the world normal at every texel's point (the
+SDF gradient, or a source mesh's interpolated vertex normals: normal_transfer_fn), ops.tangent_normals codes it in the
+face's tangent frame (the rule of include/o2345.h, which mesh_io's writers and the rasterizer decode), the same push-pull
+fills the rest and ops.normal_quantise codes it to uint8."""
 from __future__ import annotations
 
 import numpy as np
@@ -32,12 +37,13 @@ def quantise(rgb):
     return (rgb.cpu() * 255).numpy().astype(np.uint8)
 
 
-def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False):
+def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False, normal_fn=None):
     """vertices [n,3], faces [m,3] (numpy) -> (uv float32 [m,3,2], texture uint8 [N,N,3]); uv row k belongs to corner
     faces[f, k], in glTF's convention (v down the image, texel i's centre at (i + 0.5) / N).  colour_fn(points [T,3] fp32
     device tensor) -> rgb [T,3] in [0, 1] on the device, for the surface point behind every owned texel.  A texel whose
-    point is a vertex gets that vertex's position exactly.  return_atlas: also the device tensors of the atlas and the
-    texels (dict)."""
+    point is a vertex gets that vertex's position exactly.  normal_fn(points) -> world normals [T,3] (any length) adds a
+    tangent-space normal map uint8 [N,N,3] in the same uv as a third result.  return_atlas: also the device tensors of the
+    atlas and the texels (dict; with normal_fn also their tangent-space normals and the fp32 filled map)."""
     N = check_size(texture_size)
     dev = _device(device)
     vt = torch.from_numpy(np.ascontiguousarray(vertices, np.float32).reshape(-1, 3)).to(dev)
@@ -47,10 +53,16 @@ def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=Fal
         index, points, face = ops.texel_points(vt, ft, at["uv"], at["owner"], N)
         rgb = colour_fn(points).float().contiguous()
         tex = ops.texture_fill(index, rgb, at["owner"], N)
+        extra = {}
+        if normal_fn is not None:
+            tn = ops.tangent_normals(vt, ft, at["uv"], face, normal_fn(points).float().contiguous())
+            nfill = ops.texture_fill(index, tn, at["owner"], N)
+            extra = {"tangent_normals": tn, "normal_fill": nfill, "normal_map": ops.normal_quantise(nfill)}
     uv, texture = at["uv"].cpu().numpy(), quantise(tex)
+    res = (uv, texture) if normal_fn is None else (uv, texture, extra["normal_map"].cpu().numpy())
     if return_atlas:
-        return uv, texture, dict(at, texel_index=index, points=points, texel_face=face, rgb=rgb)
-    return uv, texture
+        return (*res, dict(at, texel_index=index, points=points, texel_face=face, rgb=rgb, **extra))
+    return res
 
 
 def transfer_fn(src_v, src_f, src_c, texture_size=None, device=None, seed=TRANSFER_SEED):
@@ -64,11 +76,26 @@ def transfer_fn(src_v, src_f, src_c, texture_size=None, device=None, seed=TRANSF
     c = c[:, :3].astype(np.float32) / np.float32(255) if c.dtype == np.uint8 else c[:, :3].astype(np.float32)
     sv = torch.from_numpy(np.ascontiguousarray(src_v, np.float32).reshape(-1, 3)).to(dev)
     sf = torch.from_numpy(np.ascontiguousarray(src_f, np.int32).reshape(-1, 3)).to(dev)
-    sc = torch.from_numpy(np.ascontiguousarray(c)).to(dev)
+    return _transfer(sv, sf, torch.from_numpy(np.ascontiguousarray(c)).to(dev), texture_size, seed)
 
-    def colour(points):
+
+def normal_transfer_fn(src_v, src_f, texture_size=None, device=None, seed=TRANSFER_SEED):
+    """A normal_fn for bake that takes normals from a source mesh src_v [n,3], src_f [m,3]: its vertex normals
+    (ops.vertex_normals), interpolated at each point's closest point on the face of its nearest source sample, with the
+    same seeded samples and search as transfer_fn."""
+    dev = _device(device)
+    sv = torch.from_numpy(np.ascontiguousarray(src_v, np.float32).reshape(-1, 3)).to(dev)
+    sf = torch.from_numpy(np.ascontiguousarray(src_f, np.int32).reshape(-1, 3)).to(dev)
+    with torch.cuda.device(dev):
+        return _transfer(sv, sf, ops.vertex_normals(sv, sf), texture_size, seed)
+
+
+def _transfer(sv, sf, values, texture_size, seed):
+    """The function of points that interpolates values [n,3] (one row per source vertex) on the face of each point's
+    nearest source sample."""
+    def fn(points):
         n = TRANSFER_SAMPLES * (check_size(texture_size) ** 2 if texture_size is not None else len(points))
         samples, sample_face = ops.surface_sample(sv, sf, n, seed)
         _, nn = ops.nearest(points, samples)
-        return ops.transfer_colors(sv, sf, sc, points, nn, sample_face)
-    return colour
+        return ops.transfer_colors(sv, sf, values, points, nn, sample_face)
+    return fn

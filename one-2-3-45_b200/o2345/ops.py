@@ -417,11 +417,12 @@ def ray_composite(rays_d, mid, dists, sdf, grad, color, active, nvalid, inv_s, r
 
 # ----------------------------------------------------------------------------- mesh rasterizer
 def raster(verts, faces, w2c, intr, W, H, near=0.1, shading=L.SHADE_UNLIT, colors=None, uvs=None, face_tex=None, texels=None,
-           tex_info=None):
+           tex_info=None, normals=None, tangents=None, face_ntex=None):
     """V views of one triangle mesh (csrc/raster.cu): verts [nv,3] world, faces [nf,3] int32, w2c [V,3,4] OpenCV, intr
     [V,4] = (fx, fy, cx, cy); optional colors [nv,3], uvs [nv,2] with face_tex [nf] int32, texels RGBA8 uint8 and tex_info
-    [n_tex,5] int32.  Returns device tensors color [V,H,W,3], alpha [V,H,W], depth [V,H,W], normal [V,H,W,3], tri [V,H,W]
-    int32 (-1 background)."""
+    [n_tex,5] int32; optional normal maps: normals [nv,3], tangents [nv,4] and face_ntex [nf] int32 (textures of the same
+    pool).  Returns device tensors color [V,H,W,3], alpha [V,H,W], depth [V,H,W], normal [V,H,W,3], tri [V,H,W] int32 (-1
+    background)."""
     verts, w2c, intr = cf32(verts).view(-1, 3), cf32(w2c).view(-1, 3, 4), cf32(intr).view(-1, 4)
     faces = faces.contiguous().view(-1, 3)
     V, nv, nf, dev = w2c.shape[0], verts.shape[0], faces.shape[0], verts.device
@@ -429,7 +430,10 @@ def raster(verts, faces, w2c, intr, W, H, near=0.1, shading=L.SHADE_UNLIT, color
         raise ValueError(f"{V} w2c matrices but {intr.shape[0]} intrinsics")
     colors = None if colors is None else cf32(colors).view(-1, 3)
     uvs = None if uvs is None else cf32(uvs).view(-1, 2)
-    for name, t, rows in (("colors", colors, nv), ("uvs", uvs, nv), ("face_tex", face_tex, nf)):
+    normals = None if normals is None else cf32(normals).view(-1, 3)
+    tangents = None if tangents is None else cf32(tangents).view(-1, 4)
+    for name, t, rows in (("colors", colors, nv), ("uvs", uvs, nv), ("face_tex", face_tex, nf), ("normals", normals, nv),
+                          ("tangents", tangents, nv), ("face_ntex", face_ntex, nf)):
         if t is not None and t.shape[0] != rows:
             raise ValueError(f"{name} has {t.shape[0]} rows, expected {rows}")
     mesh = L.RasterMesh(verts=_f(verts).value, colors=_f(colors).value if colors is not None else None,
@@ -437,6 +441,9 @@ def raster(verts, faces, w2c, intr, W, H, near=0.1, shading=L.SHADE_UNLIT, color
                         face_tex=_p(face_tex, _i32).value if face_tex is not None else None,
                         texels=_p(texels, _u8).value if texels is not None else None,
                         tex_info=_p(tex_info, _i32).value if tex_info is not None else None,
+                        normals=_f(normals).value if normals is not None else None,
+                        tangents=_f(tangents).value if tangents is not None else None,
+                        face_ntex=_p(face_ntex, _i32).value if face_ntex is not None else None,
                         nv=nv, nf=nf, n_tex=0 if tex_info is None else tex_info.shape[0])
     nbytes = L.load().o2345_raster_scratch_bytes(nv, nf, V, W, H)
     scratch = torch.empty(nbytes, dtype=_u8, device=dev)
@@ -561,3 +568,43 @@ def transfer_colors(verts, faces, colors, points, nn_index, sample_face):
     L.call("o2345_transfer_colors", _f(verts), verts.shape[0], _p(faces, _i32), faces.shape[0], _f(colors), _f(points), n,
            _p(nn_index.contiguous(), _i32), _p(sample_face.contiguous(), _i32), sample_face.shape[0], _f(rgb), _stream())
     return rgb
+
+
+# ----------------------------------------------------------------------------- normal maps
+def tangent_normals(verts, faces, uv, texel_face, normals):
+    """World normals [T,3] at texels of faces texel_face [T] int32 -> their tangent-space unit vectors [T,3] fp32 in each
+    face's frame from its corners and atlas uv [nf,3,2] (csrc/texture.cu; the rule is in include/o2345.h).  Degenerate
+    faces and zero or non-finite normals give (0, 0, 1)."""
+    verts, faces, uv = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3), cf32(uv).view(-1, 3, 2)
+    normals = cf32(normals).view(-1, 3)
+    n, dev = normals.shape[0], normals.device
+    if texel_face.shape[0] != n:
+        raise ValueError(f"{n} normals for {texel_face.shape[0]} texels")
+    out = torch.empty(n, 3, dtype=_f32, device=dev)
+    if n == 0:
+        return out
+    L.call("o2345_tangent_normals", _f(verts), verts.shape[0], _p(faces, _i32), faces.shape[0], _f(uv),
+           _p(texel_face.contiguous(), _i32), _f(normals), n, _f(out), _stream())
+    return out
+
+
+def normal_quantise(texture):
+    """Tangent-space texture [N,N,3] fp32 (texture_fill) -> uint8 [N,N,3]: renormalised in fp32, each component coded as
+    round_half_even((c + 1) * 127.5); an empty vector becomes (128, 128, 255)."""
+    texture = cf32(texture)
+    out = torch.empty(texture.shape, dtype=_u8, device=texture.device)
+    L.call("o2345_normal_quantise", _f(texture), texture.numel() // 3, _p(out, _u8), _stream())
+    return out
+
+
+def vertex_normals(verts, faces):
+    """Unit vertex normals [nv,3] fp32 of verts [nv,3], faces [nf,3] int32: each vertex's sum of its faces'
+    (B - A) x (C - A) in ascending face order in fp64, normalised and rounded once ((0, 0, 0) for a zero sum).
+    Synchronises once; raises O2345Error for an index outside [0, nv) or a non-finite coordinate."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    nbytes = L.load().o2345_vertex_normals_scratch_bytes(nv, nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    out = torch.empty(nv, 3, dtype=_f32, device=dev)
+    L.call("o2345_vertex_normals", _f(verts), nv, _p(faces, _i32), nf, _p(scratch), nbytes, _f(out), _stream())
+    return out

@@ -1,5 +1,5 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--target_faces N] [--texture_size N] [--output_format .ply]`
+[--mesh_resolution R] [--target_faces N] [--texture_size N [--normal_map]] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -15,7 +15,8 @@ follow reference utils/utils.py:31-45 (o2345/mesh_io.py).  `--target_faces N` (n
 mesh to N faces on the GPU before mesh.ply is written (o2345/mesh_simplify.py); .obj / .glb are converted from that mesh.
 `--texture_size N` (not in the reference; .obj or .glb only) bakes the reconstruction's colours into an N x N texture on
 the GPU (o2345/mesh_texture.py) and writes mesh.glb, or mesh.obj + mesh.mtl + mesh_albedo.png, textured; mesh.ply is
-written as without it.
+written as without it.  `--normal_map` (with `--texture_size`) also bakes the SDF's gradient into a tangent-space normal
+map in the same uv: the GLB gains NORMAL, TANGENT and a normalTexture, the OBJ `vn` and mesh_normal.png (`norm`).
 
 Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
 calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
@@ -56,6 +57,8 @@ def parse_args(argv=None):
                     help='simplify the mesh to this many faces (quadric edge collapse; default: the full marching-cubes mesh)')
     ap.add_argument('--texture_size', type=int, default=None,
                     help='bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output only)')
+    ap.add_argument('--normal_map', action='store_true',
+                    help='also bake a tangent-space normal map from the SDF gradient (needs --texture_size; .obj or .glb output)')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -72,6 +75,8 @@ def parse_args(argv=None):
             ap.error("--texture_size must be a power of two in [64, 8192]")
         if args.output_format not in (".obj", ".glb"):
             ap.error("--texture_size needs --output_format .obj or .glb")
+    if args.normal_map and args.texture_size is None:
+        ap.error("--normal_map needs --texture_size")
     return args
 
 
@@ -93,7 +98,7 @@ def _write_format(shape_dir, output_format, mesh=None):
         from o2345.mesh_io import to_viewer_frame, write_textured
         v, f, uv = to_viewer_frame(mesh["vertices"], mesh["triangles"], mesh["uv"])
         mesh_path = os.path.join(shape_dir, f"mesh{output_format}")
-        write_textured(mesh_path, v, f, uv, mesh["texture"])
+        write_textured(mesh_path, v, f, uv, mesh["texture"], mesh.get("normal_texture"))
         return mesh_path
     mesh_path = os.path.join(shape_dir, "mesh.ply")
     if output_format == ".ply":          # reference run.py:113-118
@@ -107,7 +112,8 @@ def _write_format(shape_dir, output_format, mesh=None):
 
 
 def _texture_kw(args):
-    return {} if args.texture_size is None else {"texture_size": args.texture_size}
+    kw = {} if args.texture_size is None else {"texture_size": args.texture_size}
+    return dict(kw, normal_map=True) if args.normal_map else kw
 
 
 def main(argv=None):

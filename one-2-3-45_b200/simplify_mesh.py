@@ -12,7 +12,13 @@ vertex counts before and after and the number of rounds.
 
 --texture_size N (.glb or .obj output) also bakes the welded input's vertex colours into an N x N texture of the
 simplified mesh (o2345/mesh_texture.py: each texel takes the colour of the input surface at its nearest point) and
-writes it textured: .glb with the texture embedded, .obj beside <stem>.mtl and <stem>_albedo.png."""
+writes it textured: .glb with the texture embedded, .obj beside <stem>.mtl and <stem>_albedo.png.
+
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out small.glb --target_faces 5000 --texture_size 2048 --normal_map
+
+--normal_map (with --texture_size) also bakes the welded input's vertex normals, taken at the same nearest points, into a
+tangent-space normal map, so the simplified mesh shades like the full one: the .glb gains NORMAL, TANGENT and a
+normalTexture, the .obj `vn` lines and <stem>_normal.png (`norm` in the MTL)."""
 from __future__ import annotations
 
 import argparse
@@ -35,6 +41,8 @@ def parse_args(argv=None):
     ap.add_argument("--target_faces", type=int, required=True, help="number of faces to reduce to")
     ap.add_argument("--texture_size", type=int, default=None,
                     help="bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output)")
+    ap.add_argument("--normal_map", action="store_true",
+                    help="also bake the input's normals into a tangent-space normal map (needs --texture_size)")
     args = ap.parse_args(argv)
     if os.path.splitext(args.inp)[1].lower() not in INPUTS:
         ap.error(f"{args.inp}: unsupported input format (only {', '.join(INPUTS)})")
@@ -48,6 +56,8 @@ def parse_args(argv=None):
             ap.error("--texture_size must be a power of two in [64, 8192]")
         if os.path.splitext(args.out)[1].lower() not in TEXTURED:
             ap.error(f"--texture_size needs a {' or '.join(TEXTURED)} output")
+    if args.normal_map and args.texture_size is None:
+        ap.error("--normal_map needs --texture_size")
     return args
 
 
@@ -82,12 +92,13 @@ def main(argv=None):
     print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     if args.texture_size is not None:
-        from o2345.mesh_texture import bake, transfer_fn
-        uv, tex = bake(v, f, args.texture_size, transfer_fn(*src, texture_size=args.texture_size))
-        print(f"baked a {args.texture_size} x {args.texture_size} texture")
-        mesh_io.write_textured(args.out, v, f, uv, tex)
+        from o2345.mesh_texture import bake, normal_transfer_fn, transfer_fn
+        nfn = normal_transfer_fn(*src[:2], texture_size=args.texture_size) if args.normal_map else None
+        baked = bake(v, f, args.texture_size, transfer_fn(*src, texture_size=args.texture_size), normal_fn=nfn)
+        print(f"baked a {args.texture_size} x {args.texture_size} texture" + (" and normal map" if args.normal_map else ""))
+        mesh_io.write_textured(args.out, v, f, *baked)
         print("wrote", args.out)
-        return v, f, c, rounds, uv, tex
+        return (v, f, c, rounds, *baked)
     write_mesh(args.out, v, f, c)
     print("wrote", args.out)
     return v, f, c, rounds
