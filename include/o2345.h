@@ -15,7 +15,8 @@
  *     freed behind the ABI and no call synchronises the device (except the five that say so:
  *     o2345_lod_children and o2345_surface_sample read a device-side check, o2345_simplify reads
  *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial,
- *     o2345_vertex_normals reads its checks once);
+ *     o2345_vertex_normals reads its checks once, o2345_chart_atlas reads its checks, a flag per component pass,
+ *     two values per chart round and a fit flag per trial);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -35,7 +36,7 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 12 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 13 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
@@ -48,7 +49,8 @@ extern "C" {
                                 11: texture baking: o2345_texture_atlas, o2345_texel_points, o2345_texture_fill,
                                     o2345_transfer_colors and their scratch-size functions
                                 12: normal maps: o2345_tangent_normals, o2345_normal_quantise, o2345_vertex_normals(_scratch_bytes);
-                                    o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info) */
+                                    o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info)
+                                13: multi-face charts: o2345_chart_atlas(_scratch_bytes), o2345_tangent_normals_decoded */
 
 typedef void* o2345_stream_t;
 
@@ -599,6 +601,43 @@ int64_t o2345_texture_atlas_scratch_bytes(int64_t nf);
 int o2345_texture_atlas(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int N, void* scratch,
                         int64_t scratch_bytes, float* uv, int32_t* boxes, int32_t* owner, int32_t* rung_host,
                         double* rho_host, o2345_stream_t stream);
+/* Bytes of scratch o2345_chart_atlas needs (-1 for sizes out of range); it includes 8 N^2 bytes for the owner keys. */
+int64_t o2345_chart_atlas_scratch_bytes(int64_t nv, int64_t nf, int N);
+/* A second atlas of the same triangles, with multi-face charts (--atlas charts).  Its uv and owner follow the contract of
+ * o2345_texture_atlas, so o2345_texel_points, o2345_texture_fill and the writers take it unchanged.  In fp64 from the fp32
+ * vertices, every operation rounded to nearest in the order of csrc/texture.cu:
+ *   label    n = (P1 - P0) x (P2 - P0); axis a = the largest |n_a| (the lower axis on ties); label = 2a + (n_a < 0);
+ *            a zero or non-finite n gives label 6, a chart of the face's own;
+ *   project  (u, v) = (p[(a+1) % 3], p[(a+2) % 3]) in fp32, u negated when n_a < 0 (so every face of a label has positive
+ *            uv area and |n . axis| >= |n| / sqrt(3): no face flips, stretch <= sqrt(3)); label 6 projects along z;
+ *   charts   connected components of the faces that share an edge with exactly two (face, edge) uses, on two faces, and
+ *            the same key (round 0: the label); boundary, non-manifold and degenerate edges cut; a chart's id is its
+ *            least face index;
+ *   overlap  faces f, g of a chart overlap when their projected triangles share an interior point: with
+ *            orient(a, b, p) = (bx - ax)(py - ay) - (by - ay)(px - ax), a triangle of orient 0 has no interior; for each
+ *            edge (t_k, t_k+1) of either triangle, s = orient(t_k, t_k+1, t_k+2) and o_j = the other triangle's three
+ *            orients; they are separated when max o_j <= min(0, s) or min o_j >= max(0, s);
+ *   cut      a chart with an overlap ranks its m faces by (x0 + x1) + x2 of their corners along its longer extent (u on
+ *            ties), ties by face index; the first m / 2 take side 0, the rest side 1; the next round's key is
+ *            2 id + side (side 0 for charts without overlap); rounds repeat until no chart overlaps;
+ *   extent   per chart, min and max of its corners' u and v; e = max - min in fp64 rounded up to fp32;
+ *   packing  box = ceil(e_u rho) + 4 by ceil(e_v rho) + 4, the shelves and the rung search of o2345_texture_atlas over the
+ *            charts in id order, with S = the sum of e_u e_v (fp64, the same chunked order);
+ *   uv       (box origin + 2 + (p - chart min) rho) / N per coordinate in fp64, rounded to fp32;
+ *   owner    a texel of a chart's box is a candidate of each face of the chart whose uv bounding box (uv * N in fp32) grown
+ *            by 2 holds its centre; key = (fp32 of the squared distance of the centre to the face's uv triangle, f), the
+ *            least key wins.  The distance is 0 when the three edge orients (b, c), (c, a), (a, b) of the centre are all
+ *            >= 0 or all <= 0 on a triangle of non-zero orient, else |q - ((la a + lb b) + lc c)|^2 with the barycentrics
+ *            of the 7-region test of o2345_texel_points (corners in face order).  A texel without candidate is -1.
+ * Outputs: uv [nf,3,2], boxes [nf,4] int32 (the box of the face's chart), owner [N*N], labels [nf] int32, chart [nf] int32
+ * (its chart's id), *rung_host, *rho_host, *rounds_host (the cut rounds) and *charts_host (the chart count); any of the
+ * host pointers may be NULL.  Returns O2345_EINVAL for a face index outside [0, nv), a non-finite coordinate, charts
+ * without area or charts that do not fit at j = 1.  Synchronises to read the checks, one flag per component pass, the
+ * chart count and the overlap flag per round, the sum and a fit flag per trial.  scratch: 16-byte aligned. */
+int o2345_chart_atlas(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, int N, void* scratch,
+                      int64_t scratch_bytes, float* uv, int32_t* boxes, int32_t* owner, int32_t* labels, int32_t* chart,
+                      int32_t* rung_host, double* rho_host, int32_t* rounds_host, int32_t* charts_host,
+                      o2345_stream_t stream);
 /* Bytes of scratch o2345_texel_points needs (-1 for an invalid N). */
 int64_t o2345_texel_points_scratch_bytes(int N);
 /* For the faces and the uv / owner of o2345_texture_atlas: texel_index [N*N] (capacity; the first *count entries are the
@@ -642,6 +681,12 @@ int o2345_transfer_colors(const float* verts, int64_t nv, const int32_t* faces, 
  * out of range gives NaN). */
 int o2345_tangent_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
                           const int32_t* texel_face, const float* normals, int64_t n, float* out, o2345_stream_t stream);
+/* As o2345_tangent_normals, in the frame a decoder builds from NORMAL and TANGENT (T, w): B = w (N x T) with
+ * w = sign((N x T) . (-dp/dv)) (+1 on 0), N x T in the operation order of (b - a) x (c - a) with a = 0.  For the charts
+ * of o2345_chart_atlas, where dp/du and dp/dv are not orthogonal; on an isometric chart it is the frame above. */
+int o2345_tangent_normals_decoded(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* uv,
+                                  const int32_t* texel_face, const float* normals, int64_t n, float* out,
+                                  o2345_stream_t stream);
 /* out [n,3] uint8 := the byte codes of texture [n,3] fp32 (after o2345_texture_fill), as above; n <= 8192^2. */
 int o2345_normal_quantise(const float* texture, int64_t n, uint8_t* out, o2345_stream_t stream);
 /* Bytes of scratch o2345_vertex_normals needs (-1 for sizes out of range). */

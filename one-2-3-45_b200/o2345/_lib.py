@@ -144,12 +144,17 @@ _SIGS = {
     "o2345_texture_atlas_scratch_bytes": (c_i64, [c_i64]),
     "o2345_texture_atlas": (C.c_int, [c_fp, c_i64, c_fp, c_i64, C.c_int, c_fp, c_i64, c_fp, c_fp, c_fp,
                                       C.POINTER(C.c_int32), C.POINTER(C.c_double), c_fp]),
+    "o2345_chart_atlas_scratch_bytes": (c_i64, [c_i64, c_i64, C.c_int]),
+    "o2345_chart_atlas": (C.c_int, [c_fp, c_i64, c_fp, c_i64, C.c_int, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp, c_fp,
+                                    C.POINTER(C.c_int32), C.POINTER(C.c_double), C.POINTER(C.c_int32),
+                                    C.POINTER(C.c_int32), c_fp]),
     "o2345_texel_points_scratch_bytes": (c_i64, [C.c_int]),
     "o2345_texel_points": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, C.c_int, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp, c_fp]),
     "o2345_texture_fill_scratch_bytes": (c_i64, [C.c_int]),
     "o2345_texture_fill": (C.c_int, [c_fp, c_fp, c_fp, c_fp, C.c_int, c_fp, c_i64, c_fp, c_fp]),
     "o2345_transfer_colors": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, c_fp]),
     "o2345_tangent_normals": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp, c_i64, c_fp, c_fp]),
+    "o2345_tangent_normals_decoded": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp, c_i64, c_fp, c_fp]),
     "o2345_normal_quantise": (C.c_int, [c_fp, c_i64, c_fp, c_fp]),
     "o2345_vertex_normals_scratch_bytes": (c_i64, [c_i64, c_i64]),
     "o2345_vertex_normals": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp]),
@@ -158,7 +163,7 @@ _SIGS = {
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 12         # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 13         # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 

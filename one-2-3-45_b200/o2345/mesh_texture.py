@@ -1,5 +1,6 @@
 """Texture baking on host arrays (run.py / simplify_mesh.py --texture_size, GenericTrainer.export_mesh_step): every face
-gets its own chart in an N x N atlas (ops.texture_atlas), the surface point behind every texel a chart owns is evaluated
+gets its own chart in an N x N atlas (ops.texture_atlas; or, with atlas="charts", faces share projected multi-face charts:
+ops.chart_atlas), the surface point behind every texel a chart owns is evaluated
 by a colour function (ops.texel_points), and the texels no chart owns are filled by push-pull (ops.texture_fill), all in
 csrc/texture.cu.  The colour function is the reconstruction's (SparseNeuSRenderer.blend_points, the one that colours the
 vertices) or, for a mesh without a reconstruction, the colours of a source mesh (transfer_fn).
@@ -16,6 +17,7 @@ import torch
 from . import ops
 
 MIN_SIZE, MAX_SIZE = 64, 8192
+ATLASES = ("faces", "charts")  # ops.texture_atlas (the default) and ops.chart_atlas
 TRANSFER_SEED = 0          # seed of the source surface samples of transfer_fn
 TRANSFER_SAMPLES = 4       # source samples per texel of the atlas
 
@@ -37,25 +39,36 @@ def quantise(rgb):
     return (rgb.cpu() * 255).numpy().astype(np.uint8)
 
 
-def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False, normal_fn=None):
+def check_atlas(atlas):
+    """Raises ValueError unless atlas is one of ATLASES."""
+    if atlas not in ATLASES:
+        raise ValueError(f"atlas must be one of {', '.join(ATLASES)}, got {atlas!r}")
+    return atlas
+
+
+def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False, normal_fn=None, atlas="faces"):
     """vertices [n,3], faces [m,3] (numpy) -> (uv float32 [m,3,2], texture uint8 [N,N,3]); uv row k belongs to corner
     faces[f, k], in glTF's convention (v down the image, texel i's centre at (i + 0.5) / N).  colour_fn(points [T,3] fp32
     device tensor) -> rgb [T,3] in [0, 1] on the device, for the surface point behind every owned texel.  A texel whose
     point is a vertex gets that vertex's position exactly.  normal_fn(points) -> world normals [T,3] (any length) adds a
     tangent-space normal map uint8 [N,N,3] in the same uv as a third result.  return_atlas: also the device tensors of the
-    atlas and the texels (dict; with normal_fn also their tangent-space normals and the fp32 filled map)."""
+    atlas and the texels (dict; with normal_fn also their tangent-space normals and the fp32 filled map).  atlas: "faces"
+    (ops.texture_atlas, one isometric chart per face) or "charts" (ops.chart_atlas, multi-face projected charts: denser
+    and far fewer seams, stretch up to sqrt(3); its normal map is coded in the decoders' frame)."""
     N = check_size(texture_size)
+    check_atlas(atlas)
     dev = _device(device)
     vt = torch.from_numpy(np.ascontiguousarray(vertices, np.float32).reshape(-1, 3)).to(dev)
     ft = torch.from_numpy(np.ascontiguousarray(faces, np.int32).reshape(-1, 3)).to(dev)
     with torch.cuda.device(dev):
-        at = ops.texture_atlas(vt, ft, N)
+        at = (ops.texture_atlas if atlas == "faces" else ops.chart_atlas)(vt, ft, N)
         index, points, face = ops.texel_points(vt, ft, at["uv"], at["owner"], N)
         rgb = colour_fn(points).float().contiguous()
         tex = ops.texture_fill(index, rgb, at["owner"], N)
         extra = {}
         if normal_fn is not None:
-            tn = ops.tangent_normals(vt, ft, at["uv"], face, normal_fn(points).float().contiguous())
+            code = ops.tangent_normals if atlas == "faces" else ops.tangent_normals_decoded
+            tn = code(vt, ft, at["uv"], face, normal_fn(points).float().contiguous())
             nfill = ops.texture_fill(index, tn, at["owner"], N)
             extra = {"tangent_normals": tn, "normal_fill": nfill, "normal_map": ops.normal_quantise(nfill)}
     uv, texture = at["uv"].cpu().numpy(), quantise(tex)

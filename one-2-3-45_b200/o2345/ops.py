@@ -524,6 +524,29 @@ def texture_atlas(verts, faces, N):
     return {"uv": uv[:nf], "boxes": boxes[:nf], "owner": owner, "j": j.value, "rho": rho.value}
 
 
+def chart_atlas(verts, faces, N):
+    """Multi-face charts packed into an N x N atlas (csrc/texture.cu; the rules are in include/o2345.h): faces with the
+    same dominant normal axis and sign, joined across edges of two faces, projected along that axis and cut at their
+    median until no chart overlaps itself.  -> the dict of texture_atlas (boxes: each face's chart box) plus label [nf]
+    int32, chart [nf] int32 (the chart's least face), rounds (cut rounds) and charts (chart count).  Synchronises per
+    component pass, per round and per trial; raises O2345Error for bad input or charts that do not fit."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    nbytes = L.load().o2345_chart_atlas_scratch_bytes(nv, nf, int(N))
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    uv = torch.empty(max(nf, 1), 3, 2, dtype=_f32, device=dev)
+    boxes = torch.empty(max(nf, 1), 4, dtype=_i32, device=dev)
+    owner = torch.empty(int(N) * int(N), dtype=_i32, device=dev)
+    label = torch.empty(max(nf, 1), dtype=_i32, device=dev)
+    chart = torch.empty(max(nf, 1), dtype=_i32, device=dev)
+    j, rho, rounds, charts = C.c_int32(0), C.c_double(0.0), C.c_int32(0), C.c_int32(0)
+    L.call("o2345_chart_atlas", _f(verts), nv, _p(faces, _i32), nf, int(N), _p(scratch), nbytes, _f(uv), _p(boxes, _i32),
+           _p(owner, _i32), _p(label, _i32), _p(chart, _i32), C.byref(j), C.byref(rho), C.byref(rounds), C.byref(charts),
+           _stream())
+    return {"uv": uv[:nf], "boxes": boxes[:nf], "owner": owner, "j": j.value, "rho": rho.value, "label": label[:nf],
+            "chart": chart[:nf], "rounds": rounds.value, "charts": charts.value}
+
+
 def texel_points(verts, faces, uv, owner, N):
     """The owned texels of an atlas (texture_atlas) and the surface points behind them: -> texel_index [T] int32
     (ascending), points [T,3] fp32, texel_face [T] int32.  Reads T on the host."""
@@ -584,6 +607,22 @@ def tangent_normals(verts, faces, uv, texel_face, normals):
     if n == 0:
         return out
     L.call("o2345_tangent_normals", _f(verts), verts.shape[0], _p(faces, _i32), faces.shape[0], _f(uv),
+           _p(texel_face.contiguous(), _i32), _f(normals), n, _f(out), _stream())
+    return out
+
+
+def tangent_normals_decoded(verts, faces, uv, texel_face, normals):
+    """As tangent_normals, in the frame decoders build from NORMAL and TANGENT: B = w (N x T), w = sign((N x T) . -dp/dv)
+    (for chart_atlas, whose dp/du and dp/dv are not orthogonal)."""
+    verts, faces, uv = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3), cf32(uv).view(-1, 3, 2)
+    normals = cf32(normals).view(-1, 3)
+    n, dev = normals.shape[0], normals.device
+    if texel_face.shape[0] != n:
+        raise ValueError(f"{n} normals for {texel_face.shape[0]} texels")
+    out = torch.empty(n, 3, dtype=_f32, device=dev)
+    if n == 0:
+        return out
+    L.call("o2345_tangent_normals_decoded", _f(verts), verts.shape[0], _p(faces, _i32), faces.shape[0], _f(uv),
            _p(texel_face.contiguous(), _i32), _f(normals), n, _f(out), _stream())
     return out
 

@@ -68,14 +68,15 @@ class GenericTrainer(nn.Module):
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
                 alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None,
-                texture_size=None, normal_map=False):
+                texture_size=None, normal_map=False, atlas="faces"):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
                                  iter_step=iter_step, save_vis=save_vis)
         if mode == 'export_mesh':
             return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution,
-                                         target_faces=target_faces, texture_size=texture_size, normal_map=normal_map)
+                                         target_faces=target_faces, texture_size=texture_size, normal_map=normal_map,
+                                         atlas=atlas)
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -199,12 +200,13 @@ class GenericTrainer(nn.Module):
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None,
-                         texture_size=None, normal_map=False):
+                         texture_size=None, normal_map=False, atlas="faces"):
         """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
         after the vertex merge and before mesh.ply is written.  With texture_size N the final mesh's colours are also baked
         into an N x N texture (o2345/mesh_texture.py): the result gains uv [F,3,2] and texture uint8 [N,N,3]; mesh.ply is
         written as without it.  normal_map (needs texture_size) also bakes the SDF gradient into a tangent-space normal
-        map in the same uv: the result gains normal_texture uint8 [N,N,3]."""
+        map in the same uv: the result gains normal_texture uint8 [N,N,3].  atlas selects mesh_texture.bake's atlas
+        ("faces" or "charts")."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
         if self.num_lods > 1:
             # the lod-1 mesh is coloured with the lod-0 feature maps, as in the reference (:959-978)
@@ -217,7 +219,7 @@ class GenericTrainer(nn.Module):
                 w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
                 rendering_network=self.rendering_network_lod1, lod=1, threshold=0, query_c2w=sample['query_c2w'],
                 scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces,
-                texture_size=texture_size, normal_map=normal_map)
+                texture_size=texture_size, normal_map=normal_map, atlas=atlas)
         return self.validate_colored_mesh(
             density_or_sdf_network=self.sdf_network_lod0,
             func_extract_geometry=self.sdf_renderer_lod0.extract_geometry, resolution=resolution,
@@ -226,7 +228,7 @@ class GenericTrainer(nn.Module):
             w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
             rendering_network=self.rendering_network_lod0, lod=0, threshold=0, query_c2w=sample['query_c2w'],
             scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces,
-            texture_size=texture_size, normal_map=normal_map)
+            texture_size=texture_size, normal_map=normal_map, atlas=atlas)
 
     @torch.no_grad()
     def validate_colored_mesh(self, density_or_sdf_network, func_extract_geometry, world_space=True, resolution=360,
@@ -235,7 +237,7 @@ class GenericTrainer(nn.Module):
                               intrinsics=None, rendering_network=None, rendering_projector=None, query_c2w=None,
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
                               iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None,
-                              texture_size=None, colour_chunk=1 << 20, normal_map=False):
+                              texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces"):
         if normal_map and texture_size is None:
             raise ValueError("normal_map needs texture_size")
         bmin = torch.tensor(bound_min, dtype=torch.float32)
@@ -282,7 +284,7 @@ class GenericTrainer(nn.Module):
             gradient = lambda p: (torch.cat([density_or_sdf_network.gradient(c, conditional_volume, lod)[:, 0]
                                              for c in p.split(colour_chunk)]) if len(p) else p)
             baked = bake(normalised[kept], triangles, texture_size, chunked, conditional_volume.device,
-                         **({"normal_fn": gradient} if normal_map else {}))
+                         **({"normal_fn": gradient} if normal_map else {}), **({} if atlas == "faces" else {"atlas": atlas}))
             out["uv"], out["texture"] = baked[:2]
             if normal_map:
                 out["normal_texture"] = baked[2]

@@ -1,5 +1,5 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--target_faces N] [--texture_size N [--normal_map]] [--output_format .ply]`
+[--mesh_resolution R] [--target_faces N] [--texture_size N [--normal_map] [--atlas charts]] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -17,6 +17,8 @@ mesh to N faces on the GPU before mesh.ply is written (o2345/mesh_simplify.py); 
 the GPU (o2345/mesh_texture.py) and writes mesh.glb, or mesh.obj + mesh.mtl + mesh_albedo.png, textured; mesh.ply is
 written as without it.  `--normal_map` (with `--texture_size`) also bakes the SDF's gradient into a tangent-space normal
 map in the same uv: the GLB gains NORMAL, TANGENT and a normalTexture, the OBJ `vn` and mesh_normal.png (`norm`).
+`--atlas charts` (with `--texture_size`) packs multi-face projected charts instead of one chart per face (the default
+`faces`): the full marching-cubes mesh then fits textures of practical size, and only chart borders are seams.
 
 Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
 calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
@@ -59,6 +61,8 @@ def parse_args(argv=None):
                     help='bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output only)')
     ap.add_argument('--normal_map', action='store_true',
                     help='also bake a tangent-space normal map from the SDF gradient (needs --texture_size; .obj or .glb output)')
+    ap.add_argument('--atlas', choices=("faces", "charts"), default="faces",
+                    help='texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -77,6 +81,8 @@ def parse_args(argv=None):
             ap.error("--texture_size needs --output_format .obj or .glb")
     if args.normal_map and args.texture_size is None:
         ap.error("--normal_map needs --texture_size")
+    if args.atlas != "faces" and args.texture_size is None:
+        ap.error("--atlas needs --texture_size")
     return args
 
 
@@ -113,6 +119,7 @@ def _write_format(shape_dir, output_format, mesh=None):
 
 def _texture_kw(args):
     kw = {} if args.texture_size is None else {"texture_size": args.texture_size}
+    kw = kw if args.atlas == "faces" else dict(kw, atlas=args.atlas)
     return dict(kw, normal_map=True) if args.normal_map else kw
 
 

@@ -18,7 +18,12 @@ writes it textured: .glb with the texture embedded, .obj beside <stem>.mtl and <
 
 --normal_map (with --texture_size) also bakes the welded input's vertex normals, taken at the same nearest points, into a
 tangent-space normal map, so the simplified mesh shades like the full one: the .glb gains NORMAL, TANGENT and a
-normalTexture, the .obj `vn` lines and <stem>_normal.png (`norm` in the MTL)."""
+normalTexture, the .obj `vn` lines and <stem>_normal.png (`norm` in the MTL).
+
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out full.glb --target_faces 1000000 --texture_size 1024 --atlas charts
+
+--atlas charts (with --texture_size) bakes into multi-face projected charts instead of one chart per face: meshes with
+far more faces fit the texture, and only chart borders are seams."""
 from __future__ import annotations
 
 import argparse
@@ -43,6 +48,8 @@ def parse_args(argv=None):
                     help="bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output)")
     ap.add_argument("--normal_map", action="store_true",
                     help="also bake the input's normals into a tangent-space normal map (needs --texture_size)")
+    ap.add_argument("--atlas", choices=("faces", "charts"), default="faces",
+                    help="texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)")
     args = ap.parse_args(argv)
     if os.path.splitext(args.inp)[1].lower() not in INPUTS:
         ap.error(f"{args.inp}: unsupported input format (only {', '.join(INPUTS)})")
@@ -58,6 +65,8 @@ def parse_args(argv=None):
             ap.error(f"--texture_size needs a {' or '.join(TEXTURED)} output")
     if args.normal_map and args.texture_size is None:
         ap.error("--normal_map needs --texture_size")
+    if args.atlas != "faces" and args.texture_size is None:
+        ap.error("--atlas needs --texture_size")
     return args
 
 
@@ -94,7 +103,8 @@ def main(argv=None):
     if args.texture_size is not None:
         from o2345.mesh_texture import bake, normal_transfer_fn, transfer_fn
         nfn = normal_transfer_fn(*src[:2], texture_size=args.texture_size) if args.normal_map else None
-        baked = bake(v, f, args.texture_size, transfer_fn(*src, texture_size=args.texture_size), normal_fn=nfn)
+        baked = bake(v, f, args.texture_size, transfer_fn(*src, texture_size=args.texture_size), normal_fn=nfn,
+                     atlas=args.atlas)
         print(f"baked a {args.texture_size} x {args.texture_size} texture" + (" and normal map" if args.normal_map else ""))
         mesh_io.write_textured(args.out, v, f, *baked)
         print("wrote", args.out)
