@@ -36,7 +36,7 @@ extern "C" {
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
 
-#define O2345_ABI_VERSION 13 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
+#define O2345_ABI_VERSION 14 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
                                  4: the lod-1 refinement group (o2345_sdf_voxels, o2345_prune_*, o2345_lod_children, ...)
                                  5: render_blend precision 2 (the wgmma kernel, O2345_BLEND_TC5) is gone
@@ -50,7 +50,8 @@ extern "C" {
                                     o2345_transfer_colors and their scratch-size functions
                                 12: normal maps: o2345_tangent_normals, o2345_normal_quantise, o2345_vertex_normals(_scratch_bytes);
                                     o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info)
-                                13: multi-face charts: o2345_chart_atlas(_scratch_bytes), o2345_tangent_normals_decoded */
+                                13: multi-face charts: o2345_chart_atlas(_scratch_bytes), o2345_tangent_normals_decoded
+                                14: input-view projection: o2345_project_view, o2345_face_normals */
 
 typedef void* o2345_stream_t;
 
@@ -697,6 +698,36 @@ int64_t o2345_vertex_normals_scratch_bytes(int64_t nv, int64_t nf);
  * scratch: 16-byte aligned. */
 int o2345_vertex_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, void* scratch,
                          int64_t scratch_bytes, float* normals, o2345_stream_t stream);
+
+/* Input-view projection (o2345/mesh_texture.py, run.py --project_input; csrc/project.cu).  The constants are not tuned on
+ * real outputs: no released checkpoint is available to the tests. */
+#define O2345_PROJECT_COS_LO 0.3f   /* facing weight 0 at or below this cosine ... */
+#define O2345_PROJECT_COS_HI 0.7f   /* ... and 1 at or above this one */
+#define O2345_PROJECT_TAU_PIX 2.0f  /* depth-test slack, in depth-buffer pixels of slope */
+/* For point i of points [n,3] with normal normals[i] (any length) and colour base[i] (fp32), the camera w2c [3,4] (device,
+ * OpenCV) with (fx, fy, cx, cy), the photo RGB uint8 [H,W,3], alpha uint8 [H,W] (or null: opaque) and the depth buffer
+ * [scale H, scale W] fp32 of the mesh rendered by o2345_raster with (scale fx, scale fy, scale (cx + 0.5), scale (cy + 0.5)),
+ * every operation in fp32 rounded to nearest in this order:
+ *   q_r = ((M[r][0] p.x + M[r][1] p.y) + M[r][2] p.z) + M[r][3]; weight 0 unless near < q.z <= FLT_MAX;
+ *   x = (fx q.x) / q.z + cx, y = (fy q.y) / q.z + cy (pixel i's centre at i); weight 0 unless 0 <= x <= W-1, 0 <= y <= H-1;
+ *   weight 0 unless 0 < |n| <= FLT_MAX, |a| = sqrt((a.x a.x + a.y a.y) + a.z a.z);
+ *   c_k = -((M[0][k] M[0][3] + M[1][k] M[1][3]) + M[2][k] M[2][3]), d = c - p,
+ *   cos = ((n.x/|n|)(d.x/|d|) + (n.y/|n|)(d.y/|d|)) + (n.z/|n|)(d.z/|d|);
+ *   w_a = t clamped to [0, 1] (NaN -> 0), t = (cos - COS_LO) / (COS_HI - COS_LO); weight 0 unless w_a > 0;
+ *   the buffer pixel (j, k) = (min(floor(scale (x + 0.5)), scale W - 1), min(floor(scale (y + 0.5)), scale H - 1)) holds D;
+ *   tau = ((TAU_PIX q.z) / (scale fx)) / max(cos, COS_LO); weight 0 unless D <= 0 (background) or q.z - D <= tau;
+ *   weight = w_a a, a = min(bilinear(alpha) / 255, 1) (1 without alpha);
+ *   out = base + weight (bilinear(photo) / 255 - base) per channel where weight > 0, else base bit for bit.
+ * bilinear(img) at (x, y): x0 = floor(x), x1 = x0 + 1 (y alike), taps nw, ne, sw, se with weights (x1 - x)(y1 - y),
+ * (x - x0)(y1 - y), (x1 - x)(y - y0), (x - x0)(y - y0), summed as ((v_nw w_nw + v_ne w_ne) + v_sw w_sw) + v_se w_se on the
+ * byte values; a tap past the last column or row has weight 0 and reads the last one.  weight [n] and out [n,3] fp32. */
+int o2345_project_view(const float* points, const float* normals, const float* base, int64_t n, const float* w2c,
+                       float fx, float fy, float cx, float cy, float near, const uint8_t* photo, const uint8_t* alpha,
+                       int W, int H, const float* depth, int scale, float* out, float* weight, o2345_stream_t stream);
+/* normals [n,3] fp32 := the unit normal of face face_index[i] of verts [nv,3], faces [nf,3]: (B - A) x (C - A) in fp64,
+ * divided by its length and rounded once; (0, 0, 0) for an index out of range or a face without area. */
+int o2345_face_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const int32_t* face_index,
+                       int64_t n, float* normals, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,4 @@
-// Shared pieces of the mesh kernels (metrics.cu, simplify.cu, texture.cu): fp64 vectors from the fp32 vertices with
+// Shared pieces of the mesh kernels (metrics.cu, simplify.cu, texture.cu, project.cu): fp64 vectors from the fp32 vertices with
 // explicit round-to-nearest operations in the order the numpy oracles repeat (no FMA contraction), the input check and
 // the vertex -> face adjacency.
 #pragma once
@@ -25,6 +25,14 @@ __device__ __forceinline__ D3 cross3(D3 a, D3 b, D3 c) {
   D3 e1 = sub3(b, a), e2 = sub3(c, a);
   return {__dsub_rn(__dmul_rn(e1.y, e2.z), __dmul_rn(e1.z, e2.y)), __dsub_rn(__dmul_rn(e1.z, e2.x), __dmul_rn(e1.x, e2.z)),
           __dsub_rn(__dmul_rn(e1.x, e2.y), __dmul_rn(e1.y, e2.x))};
+}
+
+// a / |a| in fp64; false when |a| is not a positive finite number
+__device__ __forceinline__ bool unit3(D3 a, D3& out) {
+  double l = __dsqrt_rn(dot3(a, a));
+  if (!(l > 0.0 && l < INFINITY)) return false;
+  out = {__ddiv_rn(a.x, l), __ddiv_rn(a.y, l), __ddiv_rn(a.z, l)};
+  return true;
 }
 
 // the three corner indices of a face lie in [0, nv)

@@ -380,14 +380,6 @@ __global__ void transfer_kernel(const float* __restrict__ V, int64_t nv, const i
 // ----------------------------------------------------------------------------- normal maps
 __device__ __forceinline__ D3 scale3(D3 a, double s) { return {__dmul_rn(a.x, s), __dmul_rn(a.y, s), __dmul_rn(a.z, s)}; }
 
-// a / |a| in fp64; false when |a| is not a positive finite number
-__device__ __forceinline__ bool unit3(D3 a, D3& out) {
-  double l = __dsqrt_rn(dot3(a, a));
-  if (!(l > 0.0 && l < INFINITY)) return false;
-  out = {__ddiv_rn(a.x, l), __ddiv_rn(a.y, l), __ddiv_rn(a.z, l)};
-  return true;
-}
-
 // One thread per texel: the tangent-space coordinates of world normal nw[i] in the frame of face texel_face[i] (rule in
 // include/o2345.h): T = dp/du, B = -dp/dv, N = e1 x e2, each normalised; (0, 0, 1) for a degenerate face or a zero or
 // non-finite normal, NaN for a face index out of range.  kDecoded: B = w (N x T), w = sign((N x T) . -dp/dv) (+1 on 0),

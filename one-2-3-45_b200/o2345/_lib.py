@@ -158,12 +158,15 @@ _SIGS = {
     "o2345_normal_quantise": (C.c_int, [c_fp, c_i64, c_fp, c_fp]),
     "o2345_vertex_normals_scratch_bytes": (c_i64, [c_i64, c_i64]),
     "o2345_vertex_normals": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp]),
+    "o2345_project_view": (C.c_int, [c_fp, c_fp, c_fp, c_i64, c_fp, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float,
+                                     c_fp, c_fp, C.c_int, C.c_int, c_fp, C.c_int, c_fp, c_fp, c_fp]),
+    "o2345_face_normals": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
 
 EXPORTED = tuple(_SIGS)
-ABI_VERSION = 13         # include/o2345.h: O2345_ABI_VERSION
+ABI_VERSION = 14         # include/o2345.h: O2345_ABI_VERSION
 _lib = None
 
 

@@ -8,7 +8,11 @@ vertices) or, for a mesh without a reconstruction, the colours of a source mesh 
 A normal map shares the atlas and the texel points: a normal function gives the world normal at every texel's point (the
 SDF gradient, or a source mesh's interpolated vertex normals: normal_transfer_fn), ops.tangent_normals codes it in the
 face's tangent frame (the rule of include/o2345.h, which mesh_io's writers and the rasterizer decode), the same push-pull
-fills the rest and ops.normal_quantise codes it to uint8."""
+fills the rest and ops.normal_quantise codes it to uint8.
+
+The input photo can be projected onto the mesh (view=, prepare_view, project_vertex_colors): ops.raster renders the
+mesh's depth from the photo's camera once, and ops.project_view blends the photo into the colours of every vertex
+(ops.vertex_normals) and texel (ops.face_normals of its face) that camera sees squarely."""
 from __future__ import annotations
 
 import numpy as np
@@ -20,6 +24,9 @@ MIN_SIZE, MAX_SIZE = 64, 8192
 ATLASES = ("faces", "charts")  # ops.texture_atlas (the default) and ops.chart_atlas
 TRANSFER_SEED = 0          # seed of the source surface samples of transfer_fn
 TRANSFER_SAMPLES = 4       # source samples per texel of the atlas
+DEPTH_SCALE = 4            # depth-buffer pixels per photo pixel and side (a 256^2 photo: 1024^2) ...
+DEPTH_MAX = 4096           # ... at most this many per side
+NEAR = 0.1                 # near plane of the depth buffer and of the projection
 
 
 def check_size(texture_size):
@@ -46,7 +53,68 @@ def check_atlas(atlas):
     return atlas
 
 
-def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False, normal_fn=None, atlas="faces"):
+def depth_scale(W, H):
+    """Depth-buffer pixels per photo pixel (per side) for a W x H photo: DEPTH_SCALE, less where the buffer would exceed
+    DEPTH_MAX on a side, at least 1."""
+    return max(1, min(DEPTH_SCALE, DEPTH_MAX // max(int(W), int(H))))
+
+
+def depth_intrinsics(intr, s):
+    """(fx, fy, cx, cy) of the depth buffer at s buffer pixels per photo pixel.  The rasterizer samples pixel j at
+    fx X / Z + cx = j + 0.5 and the photo puts pixel i's centre at i, so the buffer pixel under photo coordinate x is
+    floor(s (x + 0.5)) and photo pixel i covers buffer pixels s i .. s i + s - 1."""
+    fx, fy, cx, cy = (float(v) for v in intr)
+    return (s * fx, s * fy, s * (cx + 0.5), s * (cy + 0.5))
+
+
+def rescale_intrinsics(intr, from_wh, to_wh):
+    """(fx, fy, cx, cy) of a camera whose W x H image (from_wh) is resized to to_wh, with pixel i's centre at i (the
+    projector's convention; the image spans [-0.5, W - 0.5]): f' = f W' / W, c' = (c + 0.5) W' / W - 0.5 (y alike)."""
+    fx, fy, cx, cy = (float(v) for v in intr)
+    sx, sy = to_wh[0] / from_wh[0], to_wh[1] / from_wh[1]
+    return (fx * sx, fy * sy, (cx + 0.5) * sx - 0.5, (cy + 0.5) * sy - 0.5)
+
+
+def prepare_view(vt, ft, view):
+    """view: dict(photo uint8 [H,W,3] composited on white, alpha uint8 [H,W] or None, w2c [3,4] or [4,4] (OpenCV),
+    intr (fx, fy, cx, cy)) in the frame of the mesh vt [n,3] fp32, ft [m,3] int32 (device tensors).  Returns the view
+    with its arrays on the mesh's device and the mesh's depth buffer from that camera (ops.raster at depth_scale
+    pixels per photo pixel, depth_intrinsics); a view that already has its depth buffer is returned as it is, so one
+    buffer serves the vertices and the texels of the same mesh."""
+    if "depth" in view:
+        return view
+    dev = vt.device
+
+    def as_dev(a, dt):
+        return (a if torch.is_tensor(a) else torch.from_numpy(np.require(a, requirements="CW"))).to(dev, dt).contiguous()
+    photo = as_dev(view["photo"], torch.uint8)
+    alpha = None if view.get("alpha") is None else as_dev(view["alpha"], torch.uint8)
+    w2c = as_dev(view["w2c"], torch.float32)[:3, :4].contiguous()
+    intr = tuple(float(v) for v in view["intr"])
+    H, W = photo.shape[:2]
+    s = depth_scale(W, H)
+    with torch.cuda.device(dev):
+        depth = ops.raster(vt, ft, w2c[None], torch.tensor([depth_intrinsics(intr, s)], device=dev), s * W, s * H,
+                           near=NEAR)["depth"][0]
+    return {"photo": photo, "alpha": alpha, "w2c": w2c, "intr": intr, "depth": depth}
+
+
+def project(points, normals, rgb, view):
+    """ops.project_view of a prepared view (prepare_view) -> (colours [T,3], weight [T])."""
+    return ops.project_view(points, normals, rgb, view["w2c"], view["intr"], view["photo"], view["alpha"], view["depth"],
+                            near=NEAR)
+
+
+def project_vertex_colors(vt, ft, rgb, view):
+    """The photo of view (prepare_view's dict, or one it accepts) blended into vertex colours rgb [n,3] fp32 of the mesh
+    vt, ft (device tensors) with its vertex normals (ops.vertex_normals) -> (colours [n,3], weight [n])."""
+    view = prepare_view(vt, ft, view)
+    with torch.cuda.device(vt.device):
+        return project(vt, ops.vertex_normals(vt, ft), rgb, view)
+
+
+def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False, normal_fn=None, atlas="faces",
+         view=None):
     """vertices [n,3], faces [m,3] (numpy) -> (uv float32 [m,3,2], texture uint8 [N,N,3]); uv row k belongs to corner
     faces[f, k], in glTF's convention (v down the image, texel i's centre at (i + 0.5) / N).  colour_fn(points [T,3] fp32
     device tensor) -> rgb [T,3] in [0, 1] on the device, for the surface point behind every owned texel.  A texel whose
@@ -54,7 +122,9 @@ def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=Fal
     tangent-space normal map uint8 [N,N,3] in the same uv as a third result.  return_atlas: also the device tensors of the
     atlas and the texels (dict; with normal_fn also their tangent-space normals and the fp32 filled map).  atlas: "faces"
     (ops.texture_atlas, one isometric chart per face) or "charts" (ops.chart_atlas, multi-face projected charts: denser
-    and far fewer seams, stretch up to sqrt(3); its normal map is coded in the decoders' frame)."""
+    and far fewer seams, stretch up to sqrt(3); its normal map is coded in the decoders' frame).  view: the input photo
+    and its camera (prepare_view), blended into the texel colours with their faces' normals (ops.face_normals); with
+    return_atlas the dict then also holds the texels' project_weight [T]."""
     N = check_size(texture_size)
     check_atlas(atlas)
     dev = _device(device)
@@ -64,13 +134,15 @@ def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=Fal
         at = (ops.texture_atlas if atlas == "faces" else ops.chart_atlas)(vt, ft, N)
         index, points, face = ops.texel_points(vt, ft, at["uv"], at["owner"], N)
         rgb = colour_fn(points).float().contiguous()
-        tex = ops.texture_fill(index, rgb, at["owner"], N)
         extra = {}
+        if view is not None:
+            rgb, extra["project_weight"] = project(points, ops.face_normals(vt, ft, face), rgb, prepare_view(vt, ft, view))
+        tex = ops.texture_fill(index, rgb, at["owner"], N)
         if normal_fn is not None:
             code = ops.tangent_normals if atlas == "faces" else ops.tangent_normals_decoded
             tn = code(vt, ft, at["uv"], face, normal_fn(points).float().contiguous())
             nfill = ops.texture_fill(index, tn, at["owner"], N)
-            extra = {"tangent_normals": tn, "normal_fill": nfill, "normal_map": ops.normal_quantise(nfill)}
+            extra.update(tangent_normals=tn, normal_fill=nfill, normal_map=ops.normal_quantise(nfill))
     uv, texture = at["uv"].cpu().numpy(), quantise(tex)
     res = (uv, texture) if normal_fn is None else (uv, texture, extra["normal_map"].cpu().numpy())
     if return_atlas:

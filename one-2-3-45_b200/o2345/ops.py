@@ -647,3 +647,45 @@ def vertex_normals(verts, faces):
     out = torch.empty(nv, 3, dtype=_f32, device=dev)
     L.call("o2345_vertex_normals", _f(verts), nv, _p(faces, _i32), nf, _p(scratch), nbytes, _f(out), _stream())
     return out
+
+
+# ----------------------------------------------------------------------------- input-view projection
+def face_normals(verts, faces, face_index):
+    """Unit normals [n,3] fp32 of faces face_index [n] int32 of verts [nv,3], faces [nf,3] (csrc/project.cu): (B - A) x
+    (C - A) in fp64, normalised and rounded once; (0, 0, 0) for an index out of range or a face without area."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    n, dev = face_index.shape[0], verts.device
+    out = torch.empty(n, 3, dtype=_f32, device=dev)
+    if n == 0:
+        return out
+    L.call("o2345_face_normals", _f(verts), verts.shape[0], _p(faces, _i32), faces.shape[0], _p(face_index.contiguous(), _i32),
+           n, _f(out), _stream())
+    return out
+
+
+def project_view(points, normals, base, w2c, intr, photo, alpha, depth, near=0.1):
+    """The input photo blended into base colours (csrc/project.cu; the rule is in include/o2345.h): points [T,3], normals
+    [T,3] (any length; zero or non-finite: not seen), base [T,3] fp32; w2c [3,4] (OpenCV) and intr (fx, fy, cx, cy) of
+    the photo's camera; photo uint8 [H,W,3], alpha uint8 [H,W] or None; depth [s H, s W] fp32: the mesh's depth from
+    raster with (s fx, s fy, s (cx + 0.5), s (cy + 0.5)), s an integer >= 1.  -> (colours [T,3], weight [T]) fp32."""
+    points, normals, base = cf32(points).view(-1, 3), cf32(normals).view(-1, 3), cf32(base).view(-1, 3)
+    w2c, depth = cf32(w2c).view(3, 4), cf32(depth)
+    T, dev = points.shape[0], points.device
+    H, W = photo.shape[0], photo.shape[1]
+    if photo.shape != (H, W, 3) or (alpha is not None and alpha.shape != (H, W)):
+        raise ValueError(f"photo must be [H,W,3] and alpha [H,W], got {tuple(photo.shape)} and "
+                         f"{None if alpha is None else tuple(alpha.shape)}")
+    s = depth.shape[1] // W
+    if depth.dim() != 2 or s < 1 or depth.shape[1] != s * W or depth.shape[0] != s * H:
+        raise ValueError(f"depth {tuple(depth.shape)} is not an integer multiple of the photo's {H} x {W}")
+    if normals.shape[0] != T or base.shape[0] != T:
+        raise ValueError(f"{T} points, {normals.shape[0]} normals and {base.shape[0]} colours")
+    out = torch.empty(T, 3, dtype=_f32, device=dev)
+    weight = torch.empty(T, dtype=_f32, device=dev)
+    if T == 0:
+        return out, weight
+    fx, fy, cx, cy = (float(v) for v in intr)
+    L.call("o2345_project_view", _f(points), _f(normals), _f(base), T, _f(w2c), fx, fy, cx, cy, float(near),
+           _p(photo.contiguous(), _u8), None if alpha is None else _p(alpha.contiguous(), _u8), W, H, _f(depth), s, _f(out),
+           _f(weight), _stream())
+    return out, weight

@@ -68,7 +68,7 @@ class GenericTrainer(nn.Module):
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
                 alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None,
-                texture_size=None, normal_map=False, atlas="faces"):
+                texture_size=None, normal_map=False, atlas="faces", project_view=None):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
@@ -76,7 +76,7 @@ class GenericTrainer(nn.Module):
         if mode == 'export_mesh':
             return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution,
                                          target_faces=target_faces, texture_size=texture_size, normal_map=normal_map,
-                                         atlas=atlas)
+                                         atlas=atlas, **({} if project_view is None else {"project_view": project_view}))
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -200,14 +200,24 @@ class GenericTrainer(nn.Module):
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None,
-                         texture_size=None, normal_map=False, atlas="faces"):
+                         texture_size=None, normal_map=False, atlas="faces", project_view=None):
         """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
         after the vertex merge and before mesh.ply is written.  With texture_size N the final mesh's colours are also baked
         into an N x N texture (o2345/mesh_texture.py): the result gains uv [F,3,2] and texture uint8 [N,N,3]; mesh.ply is
         written as without it.  normal_map (needs texture_size) also bakes the SDF gradient into a tangent-space normal
         map in the same uv: the result gains normal_texture uint8 [N,N,3].  atlas selects mesh_texture.bake's atlas
-        ("faces" or "charts")."""
+        ("faces" or "charts").  project_view: dict(photo uint8 [H,W,3] on white, alpha uint8 [H,W] or None), the input
+        view (view 0) at any resolution: it is projected onto the final mesh from the query camera (sample['query_w2c'] and
+        the shared intrinsics, rescaled from img_wh to the photo's size by mesh_texture.rescale_intrinsics), into the
+        vertex colours and the baked texture (validate_colored_mesh)."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
+        kw = {}
+        if project_view is not None:
+            from .mesh_texture import rescale_intrinsics
+            K = sample['intrinsics'][0][0].cpu().numpy()           # every view of a scene shares K (synthetic.scene_cameras)
+            H, W = np.shape(project_view["photo"])[:2]
+            kw["project_view"] = dict(project_view, w2c=sample['query_w2c'][0][:3, :4],
+                                      intr=rescale_intrinsics((K[0, 0], K[1, 1], K[0, 2], K[1, 2]), (sizeW, sizeH), (W, H)))
         if self.num_lods > 1:
             # the lod-1 mesh is coloured with the lod-0 feature maps, as in the reference (:959-978)
             _, cond1 = self._lod1_volume(sample, imgs, cond, sizeW, sizeH)
@@ -219,7 +229,7 @@ class GenericTrainer(nn.Module):
                 w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
                 rendering_network=self.rendering_network_lod1, lod=1, threshold=0, query_c2w=sample['query_c2w'],
                 scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces,
-                texture_size=texture_size, normal_map=normal_map, atlas=atlas)
+                texture_size=texture_size, normal_map=normal_map, atlas=atlas, **kw)
         return self.validate_colored_mesh(
             density_or_sdf_network=self.sdf_network_lod0,
             func_extract_geometry=self.sdf_renderer_lod0.extract_geometry, resolution=resolution,
@@ -228,7 +238,7 @@ class GenericTrainer(nn.Module):
             w2cs=sample['w2cs'][0], intrinsics=sample['intrinsics'][0],
             rendering_network=self.rendering_network_lod0, lod=0, threshold=0, query_c2w=sample['query_c2w'],
             scale_mat=sample['scale_mat'], trans_mat=sample['trans_mat'], img_wh=[sizeW, sizeH], target_faces=target_faces,
-            texture_size=texture_size, normal_map=normal_map, atlas=atlas)
+            texture_size=texture_size, normal_map=normal_map, atlas=atlas, **kw)
 
     @torch.no_grad()
     def validate_colored_mesh(self, density_or_sdf_network, func_extract_geometry, world_space=True, resolution=360,
@@ -237,7 +247,10 @@ class GenericTrainer(nn.Module):
                               intrinsics=None, rendering_network=None, rendering_projector=None, query_c2w=None,
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
                               iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None,
-                              texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces"):
+                              texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces", project_view=None):
+        """project_view: dict(photo, alpha, w2c, intr) of a camera in the normalised frame (mesh_texture.prepare_view): the
+        photo is blended into the final mesh's vertex colours (its vertex normals) and baked texture (its face normals),
+        with one depth buffer of that mesh; the result gains project_weight [n] (the vertices' weights of the photo)."""
         if normal_map and texture_size is None:
             raise ValueError("normal_map needs texture_size")
         bmin = torch.tensor(bound_min, dtype=torch.float32)
@@ -271,11 +284,24 @@ class GenericTrainer(nn.Module):
         if target_faces is not None:
             from .mesh_simplify import simplify
             vertices, triangles, kept, _ = simplify(vertices, triangles, kept, target_faces, conditional_volume.device)
-        colors = colors[kept]
+        weight = None
+        if project_view is None:
+            colors = colors[kept]
+        else:
+            # the final mesh in the normalised frame, where the query camera is
+            from .mesh_texture import prepare_view, project_vertex_colors, quantise
+            dev = conditional_volume.device
+            vk = torch.from_numpy(np.ascontiguousarray(normalised[kept], np.float32)).to(dev)
+            fk = torch.from_numpy(np.ascontiguousarray(triangles, np.int32)).to(dev)
+            project_view = prepare_view(vk, fk, project_view)
+            rgb_k, weight = project_vertex_colors(vk, fk, rgb[torch.from_numpy(np.asarray(kept)).long().to(dev)], project_view)
+            colors = quantise(rgb_k)
         if self.base_exp_dir is not None:
             os.makedirs(self.base_exp_dir, exist_ok=True)
             write_ply(os.path.join(self.base_exp_dir, 'mesh.ply'), vertices, triangles, colors)
         out = {"vertices": vertices, "triangles": triangles, "colors": colors, "fields": fields}
+        if weight is not None:
+            out["project_weight"] = weight.cpu().numpy()           # each vertex's weight of the photo
         if texture_size is not None:
             # baked in the normalised frame, where blend_points evaluates (the charts only scale with scale_mat)
             from .mesh_texture import bake
@@ -284,7 +310,8 @@ class GenericTrainer(nn.Module):
             gradient = lambda p: (torch.cat([density_or_sdf_network.gradient(c, conditional_volume, lod)[:, 0]
                                              for c in p.split(colour_chunk)]) if len(p) else p)
             baked = bake(normalised[kept], triangles, texture_size, chunked, conditional_volume.device,
-                         **({"normal_fn": gradient} if normal_map else {}), **({} if atlas == "faces" else {"atlas": atlas}))
+                         **({"normal_fn": gradient} if normal_map else {}), **({} if atlas == "faces" else {"atlas": atlas}),
+                         **({} if project_view is None else {"view": project_view}))
             out["uv"], out["texture"] = baked[:2]
             if normal_map:
                 out["normal_texture"] = baked[2]

@@ -1,5 +1,6 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--target_faces N] [--texture_size N [--normal_map] [--atlas charts]] [--output_format .ply]`
+[--mesh_resolution R] [--target_faces N] [--texture_size N [--normal_map] [--atlas charts]] [--project_input]
+[--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -19,6 +20,9 @@ written as without it.  `--normal_map` (with `--texture_size`) also bakes the SD
 map in the same uv: the GLB gains NORMAL, TANGENT and a normalTexture, the OBJ `vn` and mesh_normal.png (`norm`).
 `--atlas charts` (with `--texture_size`) packs multi-face projected charts instead of one chart per face (the default
 `faces`): the full marching-cubes mesh then fits textures of practical size, and only chart borders are seams.
+`--project_input` (not in the reference) projects the input photo onto the final mesh from the input camera, so the side
+the photo shows keeps its colours (o2345/mesh_texture.py): into mesh.ply's vertex colours and, with `--texture_size`, the
+texture.  The photo is read at its own resolution (load_photo), not the 256 x 256 Zero123 input.
 
 Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
 calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
@@ -37,14 +41,36 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
 
 
-def load_input(path):
-    """256 x 256 RGB uint8 on white, like the output of the reference's preprocess() (utils/zero123_utils.py:180-202)."""
+PHOTO_MIN, PHOTO_MAX = 256, 2048   # side of the photo load_photo reads for --project_input
+
+
+def _on_white(im):
     from PIL import Image
-    im = Image.open(path)
     if im.mode == "RGBA":
         bg = Image.new("RGBA", im.size, (255, 255, 255, 255))
         im = Image.alpha_composite(bg, im)
-    return np.asarray(im.convert("RGB").resize((256, 256), Image.LANCZOS), np.uint8)
+    return im.convert("RGB")
+
+
+def load_input(path):
+    """256 x 256 RGB uint8 on white, like the output of the reference's preprocess() (utils/zero123_utils.py:180-202)."""
+    from PIL import Image
+    return np.asarray(_on_white(Image.open(path)).resize((256, 256), Image.LANCZOS), np.uint8)
+
+
+def photo_side(w, h):
+    """Side of the square photo --project_input reads from a w x h file: max(w, h) clamped to [PHOTO_MIN, PHOTO_MAX]."""
+    return min(max(int(w), int(h), PHOTO_MIN), PHOTO_MAX)
+
+
+def load_photo(path):
+    """The input photo for --project_input: the composite on white of load_input and the same non-uniform resize to a
+    square, at side photo_side(w, h) -> dict(photo uint8 [S,S,3], alpha uint8 [S,S] (RGBA files) or None)."""
+    from PIL import Image
+    im = Image.open(path)
+    S = photo_side(*im.size)
+    alpha = np.asarray(im.getchannel("A").resize((S, S), Image.LANCZOS), np.uint8) if im.mode == "RGBA" else None
+    return {"photo": np.asarray(_on_white(im).resize((S, S), Image.LANCZOS), np.uint8), "alpha": alpha}
 
 
 def parse_args(argv=None):
@@ -63,6 +89,8 @@ def parse_args(argv=None):
                     help='also bake a tangent-space normal map from the SDF gradient (needs --texture_size; .obj or .glb output)')
     ap.add_argument('--atlas', choices=("faces", "charts"), default="faces",
                     help='texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)')
+    ap.add_argument('--project_input', action='store_true',
+                    help='project the input photo onto the mesh from the input camera (vertex colours and texture)')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -164,7 +192,8 @@ def main(argv=None):
             torch.cuda.manual_seed(args.seed)
         mesh = image_to_mesh(model, trainer, load_input(args.img_path[0]), polar_angle=polars[0],
                              resolution=args.mesh_resolution, exp_dir=shape_dir, target_faces=args.target_faces,
-                             **_texture_kw(args))
+                             **_texture_kw(args),
+                             **({"project_view": load_photo(args.img_path[0])} if args.project_input else {}))
         mesh_path = _write_format(shape_dir, args.output_format, mesh)
         print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", mesh_path)
@@ -177,7 +206,9 @@ def main(argv=None):
     for i, mesh in images_to_meshes(model, trainer, [load_input(args.img_path[i]) for i in mine], [polars[i] for i in mine],
                                     seed=0 if args.seed is None else args.seed, resolution=args.mesh_resolution,
                                     exp_dirs=[shape_dirs[i] for i in mine], indices=mine, target_faces=args.target_faces,
-                                    **_texture_kw(args)):
+                                    **_texture_kw(args),
+                                    **({"project_views": [load_photo(args.img_path[i]) for i in mine]}
+                                       if args.project_input else {})):
         paths.append(_write_format(shape_dirs[i], args.output_format, mesh))
         print(f"{args.img_path[i]}: {len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", paths[-1])
