@@ -16,7 +16,8 @@
  *     o2345_lod_children and o2345_surface_sample read a device-side check, o2345_simplify reads
  *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial,
  *     o2345_vertex_normals reads its checks once, o2345_chart_atlas reads its checks, a flag per component pass,
- *     two values per chart round and a fit flag per trial);
+ *     two values per chart round and a fit flag per trial, o2345_clean_mesh reads its checks, a flag per
+ *     component pass, the component count and its counts);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -51,7 +52,9 @@ extern "C" {
                                 12: normal maps: o2345_tangent_normals, o2345_normal_quantise, o2345_vertex_normals(_scratch_bytes);
                                     o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info)
                                 13: multi-face charts: o2345_chart_atlas(_scratch_bytes), o2345_tangent_normals_decoded
-                                14: input-view projection: o2345_project_view, o2345_face_normals */
+                                14: input-view projection: o2345_project_view, o2345_face_normals; mesh cleaning:
+                                    o2345_clean_mesh(_scratch_bytes) (added entry points only: the binding resolves every
+                                    entry point by name, so a library without them fails to load) */
 
 typedef void* o2345_stream_t;
 
@@ -728,6 +731,29 @@ int o2345_project_view(const float* points, const float* normals, const float* b
  * divided by its length and rounded once; (0, 0, 0) for an index out of range or a face without area. */
 int o2345_face_normals(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const int32_t* face_index,
                        int64_t n, float* normals, o2345_stream_t stream);
+
+/* Mesh cleaning (o2345/mesh_clean.py, run.py / simplify_mesh.py --min_component; csrc/clean.cu).  For verts [nv,3] fp32
+ * and faces [nf,3] int32 (welded first: components follow vertex indices) and 0 < min_component <= 1:
+ *   components  two faces belong to one component when they share a vertex index (a bowtie vertex joins its fans);
+ *               components are numbered by their least face: label [nf] int32 := the component of each face, nc of them;
+ *   area        of a face: 0.5 sqrt(n . n), n = (B - A) x (C - A) in fp64 from the fp32 positions; of component c (area [nc]
+ *               fp64): its faces' areas in ascending face order, summed sequentially inside chunks of 1024 faces and then
+ *               sequentially over the chunk totals, each sum from +0.0;
+ *   largest     L: the greatest area, the least component on ties;
+ *   winding     of c != L (winding [nc] fp64, 0 at L): at the centroid p = ((A + B) + C) / 3 (fp64) of c's least face,
+ *               (the sum of the solid angles of L's faces, in ascending face order and chunked as the area) / (4 pi); the
+ *               solid angle of ABC is 2 atan2(a . (b x c), ((|a||b|)|c| + (a . b)|c| + (a . c)|b|) + (b . c)|a|), a = A - p
+ *               etc., |a| = sqrt((a.x a.x + a.y a.y) + a.z a.z), with the atan2 of csrc/clean.cu (+, -, *, /, sqrt only);
+ *               c is enclosed when |winding| >= 0.5 (either face orientation);
+ *   keep        keep [nc] uint8 := c == L, or c is not enclosed and area[c] >= min_component area[L] (fp64 product);
+ *   output      vertex_index [nv'] := the input indices of the vertices a kept face references, ascending; faces_out
+ *               [nf',3] := the kept faces in input order, renumbered into vertex_index.
+ * counts_host [6] := (nc, L, kept components, enclosed components, nv', nf').  Every float operation rounds to nearest
+ * in the stated order, so the outputs do not depend on scheduling.  Synchronises (see the conventions above). */
+int64_t o2345_clean_mesh_scratch_bytes(int64_t nv, int64_t nf);
+int o2345_clean_mesh(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, double min_component, void* scratch,
+                     int64_t scratch_bytes, int32_t* label, double* area, double* winding, uint8_t* keep,
+                     int32_t* vertex_index, int32_t* faces_out, int32_t* counts_host, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,5 @@
-// The input check and the vertex -> face adjacency of the mesh calls (simplify.cu, texture.cu); see mesh_common.cuh.
+// The input check, the vertex -> face adjacency and the union-find passes of the mesh calls (simplify.cu, texture.cu,
+// clean.cu); see mesh_common.cuh.
 #include "mesh_common.cuh"
 
 namespace o2345 {
@@ -45,7 +46,34 @@ __global__ void sort_kernel(const int32_t* __restrict__ off, int64_t nv, int32_t
   }
 }
 
+__global__ void iota_kernel(int32_t* __restrict__ p, int64_t n) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) p[i] = (int32_t)i;
+}
+
+__global__ void compress_kernel(int32_t* parent, int64_t n) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) parent[i] = find_root(parent, (int)i);
+}
+
 }  // namespace
+
+int iota_i32(int32_t* p, int64_t n, cudaStream_t stream) {
+  iota_kernel<<<cdiv(n, 256), 256, 0, stream>>>(p, n);
+  O2345_LAUNCH_CHECK();
+  return O2345_OK;
+}
+
+int union_find_settle(int32_t* parent, int64_t n, int32_t* changed, bool& again, cudaStream_t stream) {
+  compress_kernel<<<cdiv(n, 256), 256, 0, stream>>>(parent, n);
+  O2345_LAUNCH_CHECK();
+  int32_t h = 0;
+  O2345_CUDA(cudaMemcpyAsync(&h, changed, 4, cudaMemcpyDeviceToHost, stream));
+  O2345_CUDA(cudaStreamSynchronize(stream));
+  O2345_CUDA(cudaMemsetAsync(changed, 0, 4, stream));
+  again = h != 0;
+  return O2345_OK;
+}
 
 int vertex_faces(const int32_t* faces, int64_t nf, int64_t nv, int32_t* off, int32_t* sums, int32_t* cursor, int32_t* adj,
                  cudaStream_t stream) {

@@ -54,4 +54,39 @@ int mesh_check_status(int32_t err, const char* func);
 int vertex_faces(const int32_t* faces, int64_t nf, int64_t nv, int32_t* off, int32_t* sums, int32_t* cursor, int32_t* adj,
                  cudaStream_t stream);
 
+// Union-find over n elements (texture.cu's chart components, clean.cu's vertex components).  Parents only ever point at
+// lower indices, so every set ends rooted at its least element.
+__device__ __forceinline__ int find_root(const int32_t* parent, int x) {
+  for (int p = parent[x]; p != x; p = parent[x]) x = p;
+  return x;
+}
+
+// Hooks the larger of the roots of a and b under the smaller (atomicMin); *changed := 1 when the roots differed.
+__device__ __forceinline__ void unite(int32_t* parent, int a, int b, int32_t* changed) {
+  int ra = find_root(parent, a), rb = find_root(parent, b);
+  if (ra != rb) {
+    atomicMin(parent + max(ra, rb), min(ra, rb));
+    *changed = 1;
+  }
+}
+
+// mesh_common.cu.  p[i] := i for i in [0, n).
+int iota_i32(int32_t* p, int64_t n, cudaStream_t stream);
+// mesh_common.cu.  One pass's tail: every parent[i] := its root, then *again := *changed (read on the host), *changed := 0.
+int union_find_settle(int32_t* parent, int64_t n, int32_t* changed, bool& again, cudaStream_t stream);
+
+// parent[0, n) := the sets joined by hook(), each element pointing at its set's least element: parent := identity, then
+// passes of hook() (which launches the caller's kernel of unite() calls on `changed`) each followed by one compression,
+// until a pass joins nothing.  Synchronises once per pass.
+template <class Hook>
+int union_find(int32_t* parent, int64_t n, int32_t* changed, Hook hook, cudaStream_t stream) {
+  O2345_TRY(iota_i32(parent, n, stream));
+  O2345_CUDA(cudaMemsetAsync(changed, 0, 4, stream));
+  for (bool again = true; again;) {
+    O2345_TRY(hook());
+    O2345_TRY(union_find_settle(parent, n, changed, again, stream));
+  }
+  return O2345_OK;
+}
+
 }  // namespace o2345

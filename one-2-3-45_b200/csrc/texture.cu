@@ -558,18 +558,8 @@ __global__ void edge_kernel(const int32_t* __restrict__ F, int64_t nf, const int
   nbr[i] = uses == 2 && other >= 0 ? other : -1;
 }
 
-__global__ void iota_kernel(int32_t* __restrict__ p, int64_t n) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) p[i] = (int32_t)i;
-}
-
-__device__ __forceinline__ int find_root(const int32_t* parent, int x) {
-  for (int p = parent[x]; p != x; p = parent[x]) x = p;
-  return x;
-}
-
-// One thread per face: every neighbour g > f with the same key hooks the larger of the two roots under the smaller
-// (atomicMin; parents only ever point at lower indices, so each component ends rooted at its least face).
+// One thread per face: every neighbour g > f with the same key is joined with f (unite, mesh_common.cuh: each component
+// ends rooted at its least face).
 __global__ void hook_kernel(const int32_t* __restrict__ nbr, const int32_t* __restrict__ key, int64_t nf,
                             int32_t* parent, int32_t* __restrict__ changed) {
   int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
@@ -578,17 +568,8 @@ __global__ void hook_kernel(const int32_t* __restrict__ nbr, const int32_t* __re
   for (int k = 0; k < 3; ++k) {
     int g = nbr[3 * f + k];
     if (g <= f || key[g] != kf) continue;
-    int rf = find_root(parent, (int)f), rg = find_root(parent, g);
-    if (rf != rg) {
-      atomicMin(parent + max(rf, rg), min(rf, rg));
-      *changed = 1;
-    }
+    unite(parent, (int)f, g, changed);
   }
-}
-
-__global__ void compress_kernel(int32_t* parent, int64_t nf) {
-  int64_t f = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (f < nf) parent[f] = find_root(parent, (int)f);
 }
 
 // Chart buckets: cnt[root] counts its faces, then (after the scan) list[off[root] ..) holds them in scheduling order;
@@ -1044,14 +1025,11 @@ extern "C" int o2345_chart_atlas(const float* verts, int64_t nv, const int32_t* 
   int32_t rounds = 0, nc = 0;
   for (;;) {
     // connected components of the faces joined by an edge of two uses and the same key, rooted at their least face
-    iota_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.parent, nf);
-    for (int32_t changed = 1; changed;) {
-      O2345_CUDA(cudaMemsetAsync(S.ctr + kChanged, 0, 4, s));
+    O2345_TRY(union_find(S.parent, nf, S.ctr + kChanged, [&] {
       hook_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.nbr, S.key, nf, S.parent, S.ctr + kChanged);
-      compress_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.parent, nf);
       O2345_LAUNCH_CHECK();
-      O2345_TRY(read(S.ctr + kChanged, changed));
-    }
+      return O2345_OK;
+    }, s));
     O2345_CUDA(cudaMemsetAsync(S.off, 0, 4 * (nf + 1), s));
     O2345_CUDA(cudaMemsetAsync(S.cursor, 0, 4 * nf, s));
     bucket_count_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.parent, nf, S.off, S.is_root);

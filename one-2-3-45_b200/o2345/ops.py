@@ -689,3 +689,41 @@ def project_view(points, normals, base, w2c, intr, photo, alpha, depth, near=0.1
            _p(photo.contiguous(), _u8), None if alpha is None else _p(alpha.contiguous(), _u8), W, H, _f(depth), s, _f(out),
            _f(weight), _stream())
     return out, weight
+
+
+# ----------------------------------------------------------------------------- mesh cleaning
+def clean_mesh(verts, faces, min_component):
+    """Drops the components that are small next to the largest one or enclosed by it (csrc/clean.cu; the rules are in
+    include/o2345.h): verts [nv,3] fp32, faces [nf,3] int32 (welded: faces sharing a vertex index form one component),
+    0 < min_component <= 1 -> (vertex_index [nv'] int32, the input indices of the kept vertices (those a kept face
+    references), ascending; faces [nf',3] int32, the kept faces in input order renumbered into vertex_index; stats).
+    stats: components, largest, dropped (components), dropped_faces, enclosed (components) as ints, and the tensors
+    label [nf] int32 (each face's component, numbered by least face), area [nc] fp64, winding [nc] fp64 (0 at the largest)
+    and keep [nc] uint8.  Deterministic.  Synchronises once per union-find pass and three more times; raises O2345Error
+    for min_component outside (0, 1], an index outside [0, nv) or a non-finite coordinate."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    if not 0.0 < float(min_component) <= 1.0:
+        raise L.O2345Error(f"min_component must lie in (0, 1], got {min_component}")
+    if nf == 0:                      # no face: no component, and every vertex is unreferenced
+        empty = torch.empty(0, dtype=_i32, device=dev)
+        return empty, torch.empty(0, 3, dtype=_i32, device=dev), {
+            "components": 0, "largest": -1, "dropped": 0, "dropped_faces": 0, "enclosed": 0, "label": empty,
+            "area": torch.empty(0, dtype=torch.float64, device=dev), "winding": torch.empty(0, dtype=torch.float64, device=dev),
+            "keep": torch.empty(0, dtype=_u8, device=dev)}
+    nbytes = L.load().o2345_clean_mesh_scratch_bytes(nv, nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    label = torch.empty(nf, dtype=_i32, device=dev)
+    area = torch.empty(nf, dtype=torch.float64, device=dev)
+    winding = torch.empty(nf, dtype=torch.float64, device=dev)
+    keep = torch.empty(nf, dtype=_u8, device=dev)
+    vertex_index = torch.empty(max(nv, 1), dtype=_i32, device=dev)
+    out = torch.empty(nf, 3, dtype=_i32, device=dev)
+    counts = (C.c_int32 * 6)()
+    L.call("o2345_clean_mesh", _f(verts), nv, _p(faces, _i32), nf, float(min_component), _p(scratch), nbytes,
+           _p(label, _i32), _p(area, torch.float64), _p(winding, torch.float64), _p(keep, _u8), _p(vertex_index, _i32),
+           _p(out, _i32), counts, _stream())
+    nc, largest, kept, enclosed, n_v, n_f = list(counts)
+    stats = {"components": nc, "largest": largest, "dropped": nc - kept, "dropped_faces": nf - n_f, "enclosed": enclosed,
+             "label": label, "area": area[:nc], "winding": winding[:nc], "keep": keep[:nc]}
+    return vertex_index[:n_v], out[:n_f], stats

@@ -68,7 +68,7 @@ class GenericTrainer(nn.Module):
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
                 alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None,
-                texture_size=None, normal_map=False, atlas="faces", project_view=None):
+                texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
@@ -76,7 +76,8 @@ class GenericTrainer(nn.Module):
         if mode == 'export_mesh':
             return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution,
                                          target_faces=target_faces, texture_size=texture_size, normal_map=normal_map,
-                                         atlas=atlas, **({} if project_view is None else {"project_view": project_view}))
+                                         atlas=atlas, **({} if project_view is None else {"project_view": project_view}),
+                                         **({} if min_component is None else {"min_component": min_component}))
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -200,7 +201,7 @@ class GenericTrainer(nn.Module):
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None,
-                         texture_size=None, normal_map=False, atlas="faces", project_view=None):
+                         texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None):
         """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
         after the vertex merge and before mesh.ply is written.  With texture_size N the final mesh's colours are also baked
         into an N x N texture (o2345/mesh_texture.py): the result gains uv [F,3,2] and texture uint8 [N,N,3]; mesh.ply is
@@ -209,9 +210,11 @@ class GenericTrainer(nn.Module):
         ("faces" or "charts").  project_view: dict(photo uint8 [H,W,3] on white, alpha uint8 [H,W] or None), the input
         view (view 0) at any resolution: it is projected onto the final mesh from the query camera (sample['query_w2c'] and
         the shared intrinsics, rescaled from img_wh to the photo's size by mesh_texture.rescale_intrinsics), into the
-        vertex colours and the baked texture (validate_colored_mesh)."""
+        vertex colours and the baked texture (validate_colored_mesh).  min_component F: the components smaller than F times
+        the largest one's area, or enclosed by it, are dropped after the vertex merge (o2345/mesh_clean.py), before
+        target_faces, the projection and the bake; the result gains clean (its counts)."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
-        kw = {}
+        kw = {} if min_component is None else {"min_component": min_component}
         if project_view is not None:
             from .mesh_texture import rescale_intrinsics
             K = sample['intrinsics'][0][0].cpu().numpy()           # every view of a scene shares K (synthetic.scene_cameras)
@@ -247,10 +250,13 @@ class GenericTrainer(nn.Module):
                               intrinsics=None, rendering_network=None, rendering_projector=None, query_c2w=None,
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
                               iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None,
-                              texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces", project_view=None):
+                              texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces", project_view=None,
+                              min_component=None):
         """project_view: dict(photo, alpha, w2c, intr) of a camera in the normalised frame (mesh_texture.prepare_view): the
         photo is blended into the final mesh's vertex colours (its vertex normals) and baked texture (its face normals),
-        with one depth buffer of that mesh; the result gains project_weight [n] (the vertices' weights of the photo)."""
+        with one depth buffer of that mesh; the result gains project_weight [n] (the vertices' weights of the photo).
+        min_component: 0 < F <= 1, the welded mesh is cleaned (o2345/mesh_clean.py) before everything that follows; the
+        result gains clean, the counts of mesh_clean.clean."""
         if normal_map and texture_size is None:
             raise ValueError("normal_map needs texture_size")
         bmin = torch.tensor(bound_min, dtype=torch.float32)
@@ -281,6 +287,11 @@ class GenericTrainer(nn.Module):
         # each kept vertex's index into the extraction's arrays rides along with the colours (merge and simplify gather)
         vertices, triangles, kept = merge_vertices(vertices, triangles, np.arange(len(colors)),
                                                    candidates=getattr(renderer, "mc_lattice_candidates", None))
+        cleaned = None
+        if min_component is not None:
+            # floating fragments and inner shells go before they take faces, texels or colours from the object
+            from .mesh_clean import clean
+            vertices, triangles, kept, cleaned = clean(vertices, triangles, kept, min_component, conditional_volume.device)
         if target_faces is not None:
             from .mesh_simplify import simplify
             vertices, triangles, kept, _ = simplify(vertices, triangles, kept, target_faces, conditional_volume.device)
@@ -300,6 +311,8 @@ class GenericTrainer(nn.Module):
             os.makedirs(self.base_exp_dir, exist_ok=True)
             write_ply(os.path.join(self.base_exp_dir, 'mesh.ply'), vertices, triangles, colors)
         out = {"vertices": vertices, "triangles": triangles, "colors": colors, "fields": fields}
+        if cleaned is not None:
+            out["clean"] = cleaned
         if weight is not None:
             out["project_weight"] = weight.cpu().numpy()           # each vertex's weight of the photo
         if texture_size is not None:

@@ -1,6 +1,6 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--target_faces N] [--texture_size N [--normal_map] [--atlas charts]] [--project_input]
-[--output_format .ply]`
+[--mesh_resolution R] [--min_component F] [--target_faces N] [--texture_size N [--normal_map] [--atlas charts]]
+[--project_input] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
 (8 + 32 views, DDIM 75 / 50 steps, CFG 3) and the cost-volume reconstruction, writing the same artefacts under
@@ -23,6 +23,9 @@ map in the same uv: the GLB gains NORMAL, TANGENT and a normalTexture, the OBJ `
 `--project_input` (not in the reference) projects the input photo onto the final mesh from the input camera, so the side
 the photo shows keeps its colours (o2345/mesh_texture.py): into mesh.ply's vertex colours and, with `--texture_size`, the
 texture.  The photo is read at its own resolution (load_photo), not the 256 x 256 Zero123 input.
+`--min_component F` (0 < F <= 1, not in the reference) drops the mesh's floating fragments and enclosed inner shells right
+after the vertex merge (o2345/mesh_clean.py): every component whose area is below F times the largest one's, and every
+component inside the largest one, goes before simplification, projection and baking.  The counts are printed.
 
 Several images: `--img_path a.png b.png ...` writes exp/<basename>/ for each (basenames must differ); their Zero123
 calls run packed into shared sampler batches (o2345.pipeline.images_to_meshes) and image i's noise is seeded with
@@ -91,6 +94,8 @@ def parse_args(argv=None):
                     help='texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)')
     ap.add_argument('--project_input', action='store_true',
                     help='project the input photo onto the mesh from the input camera (vertex colours and texture)')
+    ap.add_argument('--min_component', type=float, default=None,
+                    help='drop mesh components smaller than F times the largest one\'s area or enclosed by it (0 < F <= 1)')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -101,6 +106,8 @@ def parse_args(argv=None):
     args = ap.parse_args(argv)
     if args.target_faces is not None and args.target_faces < 0:
         ap.error("--target_faces must be >= 0")
+    if args.min_component is not None and not 0.0 < args.min_component <= 1.0:
+        ap.error("--min_component must lie in (0, 1]")
     if args.texture_size is not None:
         n = args.texture_size
         if n < 64 or n > 8192 or n & (n - 1):
@@ -146,7 +153,8 @@ def _write_format(shape_dir, output_format, mesh=None):
 
 
 def _texture_kw(args):
-    kw = {} if args.texture_size is None else {"texture_size": args.texture_size}
+    kw = {} if args.min_component is None else {"min_component": args.min_component}
+    kw = kw if args.texture_size is None else dict(kw, texture_size=args.texture_size)
     kw = kw if args.atlas == "faces" else dict(kw, atlas=args.atlas)
     return dict(kw, normal_map=True) if args.normal_map else kw
 
@@ -157,6 +165,7 @@ def main(argv=None):
     if not torch.cuda.is_available():
         raise SystemExit("run.py needs a CUDA device: the o2345 path has no CPU fallback")
     from o2345 import sharding, synthetic as S
+    from o2345.mesh_clean import describe
     from o2345.pipeline import build_networks, image_to_mesh, images_to_meshes
     from o2345.zero123 import build_zero123
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -195,6 +204,8 @@ def main(argv=None):
                              **_texture_kw(args),
                              **({"project_view": load_photo(args.img_path[0])} if args.project_input else {}))
         mesh_path = _write_format(shape_dir, args.output_format, mesh)
+        if "clean" in mesh:
+            print(describe(mesh["clean"]))
         print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", mesh_path)
         return mesh_path
@@ -210,6 +221,8 @@ def main(argv=None):
                                     **({"project_views": [load_photo(args.img_path[i]) for i in mine]}
                                        if args.project_input else {})):
         paths.append(_write_format(shape_dirs[i], args.output_format, mesh))
+        if "clean" in mesh:
+            print(f"{args.img_path[i]}: {describe(mesh['clean'])}")
         print(f"{args.img_path[i]}: {len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", paths[-1])
     if world > 1:

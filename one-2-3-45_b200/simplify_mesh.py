@@ -23,7 +23,13 @@ normalTexture, the .obj `vn` lines and <stem>_normal.png (`norm` in the MTL).
     python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out full.glb --target_faces 1000000 --texture_size 1024 --atlas charts
 
 --atlas charts (with --texture_size) bakes into multi-face projected charts instead of one chart per face: meshes with
-far more faces fit the texture, and only chart borders are seams."""
+far more faces fit the texture, and only chart borders are seams.
+
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out small.glb --target_faces 5000 --min_component 0.05
+
+--min_component F (0 < F <= 1) cleans the welded input first (o2345/mesh_clean.py): components whose area is below F
+times the largest one's, and components enclosed by the largest one, are dropped.  The cleaned mesh is what is simplified
+and what the texture and normal map are transferred from, so a dropped fragment gives no texel its colour."""
 from __future__ import annotations
 
 import argparse
@@ -50,6 +56,8 @@ def parse_args(argv=None):
                     help="also bake the input's normals into a tangent-space normal map (needs --texture_size)")
     ap.add_argument("--atlas", choices=("faces", "charts"), default="faces",
                     help="texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)")
+    ap.add_argument("--min_component", type=float, default=None,
+                    help="first drop components smaller than F times the largest one's area or enclosed by it (0 < F <= 1)")
     args = ap.parse_args(argv)
     if os.path.splitext(args.inp)[1].lower() not in INPUTS:
         ap.error(f"{args.inp}: unsupported input format (only {', '.join(INPUTS)})")
@@ -57,6 +65,8 @@ def parse_args(argv=None):
         ap.error(f"{args.out}: unsupported output format (only {', '.join(OUTPUTS)})")
     if args.target_faces < 0:
         ap.error("--target_faces must be >= 0")
+    if args.min_component is not None and not 0.0 < args.min_component <= 1.0:
+        ap.error("--min_component must lie in (0, 1]")
     if args.texture_size is not None:
         n = args.texture_size
         if n < 64 or n > 8192 or n & (n - 1):
@@ -96,6 +106,10 @@ def main(argv=None):
     print(f"read {args.inp}: {len(v)} vertices, {len(f)} faces")
     v, f, c = mesh_io.merge_vertices(v, f, c)
     print(f"welded: {len(v)} vertices, {len(f)} faces")
+    if args.min_component is not None:
+        from o2345.mesh_clean import clean, describe
+        v, f, c, stats = clean(v, f, c, args.min_component)
+        print(f"cleaned: {describe(stats)}: {len(v)} vertices, {len(f)} faces")
     src = (v, f, c)
     v, f, c, rounds = simplify(v, f, c, args.target_faces)
     print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
