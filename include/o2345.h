@@ -17,7 +17,7 @@
  *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial,
  *     o2345_vertex_normals reads its checks once, o2345_chart_atlas reads its checks, a flag per component pass,
  *     two values per chart round and a fit flag per trial, o2345_clean_mesh reads its checks, a flag per
- *     component pass, the component count and its counts);
+ *     component pass, the component count and its counts, o2345_ambient_occlusion reads its checks once);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -53,8 +53,9 @@ extern "C" {
                                     o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info)
                                 13: multi-face charts: o2345_chart_atlas(_scratch_bytes), o2345_tangent_normals_decoded
                                 14: input-view projection: o2345_project_view, o2345_face_normals; mesh cleaning:
-                                    o2345_clean_mesh(_scratch_bytes) (added entry points only: the binding resolves every
-                                    entry point by name, so a library without them fails to load) */
+                                    o2345_clean_mesh(_scratch_bytes); ambient occlusion: o2345_ambient_occlusion(_scratch_bytes)
+                                    (added entry points only: the binding resolves every entry point by name, so a library
+                                    without them fails to load) */
 
 typedef void* o2345_stream_t;
 
@@ -754,6 +755,50 @@ int64_t o2345_clean_mesh_scratch_bytes(int64_t nv, int64_t nf);
 int o2345_clean_mesh(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, double min_component, void* scratch,
                      int64_t scratch_bytes, int32_t* label, double* area, double* winding, uint8_t* keep,
                      int32_t* vertex_index, int32_t* faces_out, int32_t* counts_host, o2345_stream_t stream);
+
+/* Ambient occlusion (o2345/mesh_texture.py, run.py / simplify_mesh.py --ambient_occlusion; csrc/ao.cu).  For point p with
+ * normal n and the occluder mesh verts [nv,3] fp32, faces [nf,3] int32, AO(p) is the share of the k directions of dirs
+ * [k,3] (fp32, turned into n's frame) for which the segment p + t w, t in [t_min, t_max], hits no face.  The library's
+ * callers pass K = 256 points of a golden-angle spiral on the unit disk lifted to the hemisphere (Malley's method, so they
+ * are cosine-distributed): d_k = (r cos phi, r sin phi, sqrt(1 - r^2)), r = sqrt((k + 1/2) / K), phi = k pi (3 - sqrt 5),
+ * computed in fp64 and rounded once to fp32 on the host (no device sin / cos), the same table at every point: the result
+ * moves in steps of 1/256, below one 8-bit code, so there is no per-point rotation.  t_min = 1e-3 D and t_max = 0.1 D,
+ * D the diagonal of the box of the nv vertices (fp64, rounded once); t_min drops the hits at t = 0 on the faces around
+ * a vertex the ray starts from.  Every fp32 operation is rounded to nearest in this order, without FMA contraction:
+ *   frame     |n| = sqrt((n.x n.x + n.y n.y) + n.z n.z), u = n / |n| per component; s = copysign(1, u.z),
+ *             a = -1 / (s + u.z), b = (u.x u.y) a, T = (1 + ((s u.x) u.x) a, s b, -(s u.x)), B = (b, s + (u.y u.y) a, -u.y)
+ *             (Duff et al. 2017), w = (d.x T + d.y B) + d.z u per component.  A normal of zero or non-finite length, or a
+ *             point with a non-finite coordinate, gives AO = 1;
+ *   box test  of a box [lo, hi] on the segment [0, t_max]: per axis c, when 1 / w_c rounds to a finite i_c the slab gives
+ *             t1 = (lo_c - p_c) i_c, t2 = (hi_c - p_c) i_c and the interval [min(t1, t2), max(t1, t2)]; otherwise the axis
+ *             passes when lo_c <= p_c <= hi_c and gives no interval.  The box passes when every axis passes and
+ *             max(0, the interval starts) <= min(t_max, the interval ends);
+ *   face      the face's box is the min / max of its corners' coordinates grown by pad = D' 2^-13 on every side (D' the
+ *             diagonal above, rounded to fp32; lo - pad, hi + pad rounded), and a face is hit when its box passes and the
+ *             watertight test (Woop, Benthin and Wald, JCGT 2013; no culling) accepts:
+ *               kz = the axis of the largest |w_c| (the lower on ties), kx = kz + 1, ky = kx + 1 (mod 3), kx and ky
+ *               swapped when w_kz < 0; Sx = w_kx / w_kz, Sy = w_ky / w_kz, Sz = 1 / w_kz;
+ *               per corner V (A, B, C in face order): P = V - p, x = P_kx - Sx P_kz, y = P_ky - Sy P_kz;
+ *               U = Cx By - Cy Bx, V = Ax Cy - Ay Cx, W = Bx Ay - By Ax; if any of them is 0 all three are recomputed as
+ *               fp32(fp64 product - fp64 product) of the same terms;
+ *               no hit if one of U, V, W is < 0 and one is > 0; det = (U + V) + W, no hit if det = 0;
+ *               T = ((U Sz A_kz + V Sz B_kz) + W Sz C_kz) with each Sz P_kz rounded first, T' and |det| the values with
+ *               det's sign taken off both; hit when t_min |det| <= T' <= t_max |det|.
+ *             The box stops the fp32 edge functions of a nearly degenerate face from accepting rays that pass far from
+ *             it; a ray through a shared edge or vertex is decided the same way by both faces' edge functions, so a
+ *             closed mesh lets none through.
+ *   result    out[i] = (number of directions without a hit) / k in fp32.  The count is a count of any-hits, so it does not
+ *             depend on which face is found first.
+ * The faces are searched through an LBVH built on the device (30-bit Morton codes of face-box centres, ties by face index;
+ * Karras 2012); a node's box is the exact min / max of the padded face boxes below it, and the box test only moves
+ * with its bounds through rounded subtractions and products, so a node never rejects a ray one of its faces passes and
+ * the result equals the brute-force search over all faces bit for bit.  Returns O2345_EINVAL for a face index outside
+ * [0, nv) or a non-finite vertex: the call synchronises the stream once to read that check.  nf = 0 gives AO = 1
+ * everywhere; n = 0 does nothing.  scratch: 16-byte aligned. */
+int64_t o2345_ambient_occlusion_scratch_bytes(int64_t nv, int64_t nf);
+int o2345_ambient_occlusion(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* points,
+                            const float* normals, int64_t n, const float* dirs, int k, float t_min, float t_max,
+                            void* scratch, int64_t scratch_bytes, float* out, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

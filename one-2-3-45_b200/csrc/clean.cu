@@ -5,7 +5,7 @@
 //               least face by atomicMin; the component heads (faces that are their component's least face) compacted in
 //               ascending order (o2345_compact), so component c is the c-th head;
 //   buckets     per component its face count (scan_i32: offsets), and the faces sorted by component, ascending inside each
-//               one, by a stable least-significant-bit-first split per bit of the label (scan_i32 of the one bits);
+//               one, by a stable least-significant-bit-first split per bit of the label (radix_sort_i32);
 //   area        one thread per face: its area in fp64; one block per component: the ordered sum of its faces' areas;
 //   largest     one block: the greatest area, the least component on ties;
 //   winding     one block per other component: the ordered sum of the largest component's solid angles at the centroid
@@ -123,23 +123,6 @@ __global__ void label_kernel(const float* __restrict__ V, const int32_t* __restr
   atomicAdd(cnt + lab, 1);
   D3 n = cross3(vert(V, c[0]), vert(V, c[1]), vert(V, c[2]));
   face_area[f] = __dmul_rn(0.5, __dsqrt_rn(dot3(n, n)));
-}
-
-// One pass of the stable split: ones[i] := bit b of the label of order[i]
-__global__ void bit_kernel(const int32_t* __restrict__ order, const int32_t* __restrict__ label, int64_t nf, int b,
-                           int32_t* __restrict__ ones) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < nf) ones[i] = (label[order[i]] >> b) & 1;
-}
-
-// ... and after the scan of ones (total *n_ones), the zeros keep their order at the front, the ones at the back
-__global__ void split_kernel(const int32_t* __restrict__ order, const int32_t* __restrict__ label, int64_t nf, int b,
-                             const int32_t* __restrict__ ones_before, const int32_t* __restrict__ n_ones,
-                             int32_t* __restrict__ next) {
-  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= nf) return;
-  const int32_t f = order[i], o = ones_before[i];
-  next[(label[f] >> b) & 1 ? nf - *n_ones + o : i - o] = f;
 }
 
 // One block per component: its area, the ordered sum of its faces' areas in ascending face order.
@@ -306,16 +289,9 @@ extern "C" int o2345_clean_mesh(const float* verts, int64_t nv, const int32_t* f
 
   // buckets: offsets, and the faces sorted by component (stable, so ascending inside each)
   O2345_TRY(scan_i32(S.off, nc + 1, S.sums, nullptr, s));
-  O2345_TRY(iota_i32(S.order, nf, s));
-  for (int b = 0; (1ll << b) < nc; ++b) {
-    bit_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.order, label, nf, b, S.ones);
-    O2345_LAUNCH_CHECK();
-    O2345_TRY(scan_i32(S.ones, nf, S.sums, S.ctr + kOnes, s));
-    split_kernel<<<cdiv(nf, 256), 256, 0, s>>>(S.order, label, nf, b, S.ones, S.ctr + kOnes, S.next);
-    O2345_LAUNCH_CHECK();
-    int32_t* t = S.order;
-    S.order = S.next, S.next = t;
-  }
+  int bits = 0;
+  while ((1ll << bits) < nc) ++bits;
+  O2345_TRY(radix_sort_i32(S.order, S.next, label, nf, bits, S.ones, S.sums, S.ctr + kOnes, s));
 
   area_kernel<<<nc, kSumThreads, 0, s>>>(S.off, S.order, S.face_area, area);
   largest_kernel<<<1, 1024, 0, s>>>(area, nc, S.ctr + kLargest);

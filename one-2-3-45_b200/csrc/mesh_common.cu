@@ -1,5 +1,5 @@
-// The input check, the vertex -> face adjacency and the union-find passes of the mesh calls (simplify.cu, texture.cu,
-// clean.cu); see mesh_common.cuh.
+// The input check, the vertex -> face adjacency, the union-find passes and the stable radix sort of the mesh calls
+// (simplify.cu, texture.cu, clean.cu, ao.cu); see mesh_common.cuh.
 #include "mesh_common.cuh"
 
 namespace o2345 {
@@ -56,6 +56,23 @@ __global__ void compress_kernel(int32_t* parent, int64_t n) {
   if (i < n) parent[i] = find_root(parent, (int)i);
 }
 
+// One pass of the stable split: ones[i] := bit b of the key of order[i]
+__global__ void bit_kernel(const int32_t* __restrict__ order, const int32_t* __restrict__ key, int64_t n, int b,
+                           int32_t* __restrict__ ones) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) ones[i] = (key[order[i]] >> b) & 1;
+}
+
+// ... and after the scan of ones (total *n_ones), the zeros keep their order at the front, the ones at the back
+__global__ void split_kernel(const int32_t* __restrict__ order, const int32_t* __restrict__ key, int64_t n, int b,
+                             const int32_t* __restrict__ ones_before, const int32_t* __restrict__ n_ones,
+                             int32_t* __restrict__ next) {
+  int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const int32_t f = order[i], o = ones_before[i];
+  next[(key[f] >> b) & 1 ? n - *n_ones + o : i - o] = f;
+}
+
 }  // namespace
 
 int iota_i32(int32_t* p, int64_t n, cudaStream_t stream) {
@@ -72,6 +89,21 @@ int union_find_settle(int32_t* parent, int64_t n, int32_t* changed, bool& again,
   O2345_CUDA(cudaStreamSynchronize(stream));
   O2345_CUDA(cudaMemsetAsync(changed, 0, 4, stream));
   again = h != 0;
+  return O2345_OK;
+}
+
+int radix_sort_i32(int32_t*& order, int32_t*& next, const int32_t* key, int64_t n, int bits, int32_t* ones, int32_t* sums,
+                   int32_t* n_ones, cudaStream_t stream) {
+  O2345_TRY(iota_i32(order, n, stream));
+  for (int b = 0; b < bits; ++b) {
+    bit_kernel<<<cdiv(n, 256), 256, 0, stream>>>(order, key, n, b, ones);
+    O2345_LAUNCH_CHECK();
+    O2345_TRY(scan_i32(ones, n, sums, n_ones, stream));
+    split_kernel<<<cdiv(n, 256), 256, 0, stream>>>(order, key, n, b, ones, n_ones, next);
+    O2345_LAUNCH_CHECK();
+    int32_t* t = order;
+    order = next, next = t;
+  }
   return O2345_OK;
 }
 

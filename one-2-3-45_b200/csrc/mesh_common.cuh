@@ -1,4 +1,4 @@
-// Shared pieces of the mesh kernels (metrics.cu, simplify.cu, texture.cu, project.cu): fp64 vectors from the fp32 vertices with
+// Shared pieces of the mesh kernels (metrics.cu, simplify.cu, texture.cu, project.cu, clean.cu, ao.cu): fp64 vectors from the fp32 vertices with
 // explicit round-to-nearest operations in the order the numpy oracles repeat (no FMA contraction), the input check and
 // the vertex -> face adjacency.
 #pragma once
@@ -53,6 +53,13 @@ int mesh_check_status(int32_t err, const char* func);
 // thread per vertex sorts its list (the scatter's order depends on scheduling).
 int vertex_faces(const int32_t* faces, int64_t nf, int64_t nv, int32_t* off, int32_t* sums, int32_t* cursor, int32_t* adj,
                  cudaStream_t stream);
+
+// mesh_common.cu.  order[0, n) := 0 .. n-1 sorted stably by key[i] (>= 0) over the key's low `bits` bits: one stable
+// split per bit, least significant first, each on a scan_i32 of the one bits (clean.cu's faces by component, ao.cu's faces
+// by Morton code).  next, ones: n int32 each; sums: scan_blocks(n); n_ones: one int32.  order and next swap with every
+// pass, so the sorted list is wherever order points on return.
+int radix_sort_i32(int32_t*& order, int32_t*& next, const int32_t* key, int64_t n, int bits, int32_t* ones, int32_t* sums,
+                   int32_t* n_ones, cudaStream_t stream);
 
 // Union-find over n elements (texture.cu's chart components, clean.cu's vertex components).  Parents only ever point at
 // lower indices, so every set ends rooted at its least element.

@@ -164,6 +164,9 @@ _SIGS = {
     "o2345_clean_mesh_scratch_bytes": (c_i64, [c_i64, c_i64]),
     "o2345_clean_mesh": (C.c_int, [c_fp, c_i64, c_fp, c_i64, C.c_double, c_fp, c_i64, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp,
                                    c_fp, c_fp]),
+    "o2345_ambient_occlusion_scratch_bytes": (c_i64, [c_i64, c_i64]),
+    "o2345_ambient_occlusion": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, C.c_int, C.c_float, C.c_float,
+                                          c_fp, c_i64, c_fp, c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }

@@ -190,13 +190,15 @@ def tangent_frames(vertices, triangles, uv):
     return T, B, N
 
 
-def write_textured_glb(path, vertices, triangles, uv, texture, normal_texture=None):
+def write_textured_glb(path, vertices, triangles, uv, texture, normal_texture=None, occlusion_texture=None):
     """Binary glTF 2.0 of a textured mesh: vertices [n,3], triangles [m,3], uv [m,3,2] (row k for corner k, glTF's
     convention), texture uint8 [N,N,3].  Vertices are split per corner (3m of them: POSITION float32, TEXCOORD_0 float32,
     uint32 indices 0 .. 3m-1) and the material is unlit-friendly PBR: the texture as an embedded PNG baseColorTexture
     (CLAMP_TO_EDGE, LINEAR), metallic 0, roughness 1.  No COLOR_0.  With normal_texture uint8 [N,N,3] (tangent space, in
     the frame of tangent_frames) the corners also get NORMAL (the face normal of the written winding) and TANGENT (T, w)
-    with w = sign((N x T) . B) in this frame, and the material a normalTexture (a second PNG)."""
+    with w = sign((N x T) . B) in this frame, and the material a normalTexture (a second PNG).  With occlusion_texture
+    uint8 [N,N] (ambient occlusion, 255 = open) the material gains an occlusionTexture in TEXCOORD_0: a grey PNG, whose
+    R channel glTF reads."""
     f = np.asarray(triangles, np.int64).reshape(-1, 3)
     v = np.ascontiguousarray(np.asarray(vertices, np.float32)[f.reshape(-1)])
     t = np.ascontiguousarray(np.asarray(uv, np.float32).reshape(-1, 2))
@@ -210,6 +212,8 @@ def write_textured_glb(path, vertices, triangles, uv, texture, normal_texture=No
         nrm = np.ascontiguousarray(np.repeat(N, 3, 0).astype(np.float32))
         tan = np.ascontiguousarray(np.repeat(np.concatenate([T, w[:, None]], 1), 3, 0).astype(np.float32))
         blobs += [_png_bytes(normal_texture), nrm.tobytes(), tan.tobytes()]
+    if occlusion_texture is not None:
+        blobs.append(_png_bytes(occlusion_texture))
     offs, total = [], 0
     for b in blobs:
         offs.append(total)
@@ -245,6 +249,11 @@ def write_textured_glb(path, vertices, triangles, uv, texture, normal_texture=No
                                {"buffer": 0, "byteOffset": offs[6], "byteLength": len(blobs[6]), "target": 34962}]
         doc["accessors"] += [{"bufferView": 5, "componentType": 5126, "count": int(len(v)), "type": "VEC3"},
                              {"bufferView": 6, "componentType": 5126, "count": int(len(v)), "type": "VEC4"}]
+    if occlusion_texture is not None:
+        doc["materials"][0]["occlusionTexture"] = {"index": len(doc["textures"])}
+        doc["textures"].append({"sampler": 0, "source": len(doc["images"])})
+        doc["images"].append({"bufferView": len(blobs) - 1, "mimeType": "image/png"})
+        doc["bufferViews"].append({"buffer": 0, "byteOffset": offs[-1], "byteLength": len(blobs[-1])})
     js = json.dumps(doc, separators=(",", ":")).encode("utf-8")
     js += b" " * ((4 - len(js) % 4) % 4)
     with open(path, "wb") as fh:
@@ -255,11 +264,13 @@ def write_textured_glb(path, vertices, triangles, uv, texture, normal_texture=No
         fh.write(bytes(bin_chunk))
 
 
-def write_textured_obj(path, vertices, triangles, uv, texture, normal_texture=None):
+def write_textured_obj(path, vertices, triangles, uv, texture, normal_texture=None, occlusion_texture=None):
     """Wavefront OBJ of a textured mesh beside its material: `v x y z`, then one `vt u (1 - v)` per face corner (OBJ's v
     points up the image), then `f a/t b/t c/t`; <stem>.mtl (`map_Kd <stem>_albedo.png`) and the PNG next to it.  With
     normal_texture uint8 [N,N,3] (tangent space, the frame of tangent_frames) also one `vn` per face (its normal),
-    `f a/t/n ...`, <stem>_normal.png and `norm <stem>_normal.png` in the MTL."""
+    `f a/t/n ...`, <stem>_normal.png and `norm <stem>_normal.png` in the MTL.  With occlusion_texture uint8 [N,N]
+    also <stem>_occlusion.png and `map_ao <stem>_occlusion.png` in the MTL: map_ao is not part of the MTL standard, but
+    several importers read it as the ambient occlusion map."""
     import os
     stem = os.path.splitext(os.path.basename(path))[0]
     folder = os.path.dirname(os.path.abspath(path))
@@ -273,6 +284,10 @@ def write_textured_obj(path, vertices, triangles, uv, texture, normal_texture=No
         with open(os.path.join(folder, stem + "_normal.png"), "wb") as fh:
             fh.write(_png_bytes(normal_texture))
         mtl += "norm %s_normal.png\n" % stem
+    if occlusion_texture is not None:
+        with open(os.path.join(folder, stem + "_occlusion.png"), "wb") as fh:
+            fh.write(_png_bytes(occlusion_texture))
+        mtl += "map_ao %s_occlusion.png\n" % stem
     with open(os.path.join(folder, stem + ".mtl"), "w") as fh:
         fh.write(mtl)
     with open(path, "w") as fh:
@@ -292,12 +307,12 @@ def write_textured_obj(path, vertices, triangles, uv, texture, normal_texture=No
                 fh.write("f %d/%d/%d %d/%d/%d %d/%d/%d\n" % (q[0], 3 * i + 1, i + 1, q[1], 3 * i + 2, i + 1, q[2], 3 * i + 3, i + 1))
 
 
-def write_textured(path, vertices, triangles, uv, texture, normal_texture=None):
+def write_textured(path, vertices, triangles, uv, texture, normal_texture=None, occlusion_texture=None):
     """write_textured_glb or write_textured_obj by the extension of path."""
     if path.lower().endswith(".glb"):
-        return write_textured_glb(path, vertices, triangles, uv, texture, normal_texture)
+        return write_textured_glb(path, vertices, triangles, uv, texture, normal_texture, occlusion_texture)
     if path.lower().endswith(".obj"):
-        return write_textured_obj(path, vertices, triangles, uv, texture, normal_texture)
+        return write_textured_obj(path, vertices, triangles, uv, texture, normal_texture, occlusion_texture)
     raise ValueError(f"{path}: a textured mesh is written as .glb or .obj")
 
 
@@ -395,11 +410,12 @@ def read_glb(path):
                 [n,2] (TEXCOORD_0, or None), face_tex [m] (texture of the material's baseColorTexture, -1 without), normals
                 [n,3] (NORMAL, zeros for a primitive without, or None), tangents [n,4] (TANGENT alike), face_ntex [m]
                 (texture of the material's normalTexture where the primitive has TEXCOORD_0, NORMAL and TANGENT, -1
-                without), root (index into roots), local_to_root [4x4] (product of the node matrices below the root's
-                own);
+                without), face_otex [m] (texture of the material's occlusionTexture where the primitive has TEXCOORD_0, -1
+                without; glTF reads its R channel), root (index into roots), local_to_root [4x4] (product of the node
+                matrices below the root's own);
       textures  [(RGBA uint8 [h,w,4], wrap s, wrap t)] decoded with PIL.
-    All in glTF's own (Y-up) axes.  Primitives that are not triangle lists, alpha modes, occlusion / metallic-roughness
-    textures, the normal map's scale and texture transforms are ignored; a texture is sampled at TEXCOORD_0."""
+    All in glTF's own (Y-up) axes.  Primitives that are not triangle lists, alpha modes, metallic-roughness textures,
+    the occlusion strength, the normal map's scale and texture transforms are ignored; a texture is sampled at TEXCOORD_0."""
     import io
     raw = open(path, "rb").read()
     magic, version, _ = struct.unpack_from("<III", raw, 0)
@@ -438,7 +454,7 @@ def read_glb(path):
         return tex_of_image[key]
 
     def mesh(mi):
-        vs, fs, cs, us, ts, ns, gs, nts, n = [], [], [], [], [], [], [], [], 0
+        vs, fs, cs, us, ts, ns, gs, nts, ots, n = [], [], [], [], [], [], [], [], [], 0
         for prim in doc["meshes"][mi]["primitives"]:
             if prim.get("mode", 4) != 4:
                 continue
@@ -455,6 +471,8 @@ def read_glb(path):
             tex = texture(pbr["baseColorTexture"]["index"]) if "baseColorTexture" in pbr and "TEXCOORD_0" in att else -1
             mapped = "normalTexture" in mat and all(k in att for k in ("TEXCOORD_0", "NORMAL", "TANGENT"))
             nts.append(np.full(len(f), texture(mat["normalTexture"]["index"]) if mapped else -1, np.int64))
+            occluded = "occlusionTexture" in mat and "TEXCOORD_0" in att
+            ots.append(np.full(len(f), texture(mat["occlusionTexture"]["index"]) if occluded else -1, np.int64))
             ns.append(_glb_accessor(doc, binary, att["NORMAL"])[:, :3] if "NORMAL" in att else np.zeros((len(v), 3)))
             gs.append(_glb_accessor(doc, binary, att["TANGENT"])[:, :4] if "TANGENT" in att else np.zeros((len(v), 4)))
             vs.append(v[:, :3])
@@ -469,7 +487,8 @@ def read_glb(path):
         return {"verts": np.concatenate(vs), "faces": np.concatenate(fs), "colors": np.concatenate(cs),
                 "uvs": np.concatenate(us) if has("TEXCOORD_0") else None, "face_tex": np.concatenate(ts),
                 "normals": np.concatenate(ns) if has("NORMAL") else None,
-                "tangents": np.concatenate(gs) if has("TANGENT") else None, "face_ntex": np.concatenate(nts)}
+                "tangents": np.concatenate(gs) if has("TANGENT") else None, "face_ntex": np.concatenate(nts),
+                "face_otex": np.concatenate(ots)}
 
     roots, meshes = [], []
 

@@ -12,7 +12,11 @@ fills the rest and ops.normal_quantise codes it to uint8.
 
 The input photo can be projected onto the mesh (view=, prepare_view, project_vertex_colors): ops.raster renders the
 mesh's depth from the photo's camera once, and ops.project_view blends the photo into the colours of every vertex
-(ops.vertex_normals) and texel (ops.face_normals of its face) that camera sees squarely."""
+(ops.vertex_normals) and texel (ops.face_normals of its face) that camera sees squarely.
+
+An occlusion map (ao_fn=, vertex_ao, ao_transfer_fn) shares the atlas too: ops.ambient_occlusion gives the AO of every
+vertex of the full mesh, the texels take it interpolated on the face of their nearest source sample (as transfer_fn does
+colours), and the same push-pull fills the rest.  The glTF occlusionTexture reads it."""
 from __future__ import annotations
 
 import numpy as np
@@ -27,6 +31,9 @@ TRANSFER_SAMPLES = 4       # source samples per texel of the atlas
 DEPTH_SCALE = 4            # depth-buffer pixels per photo pixel and side (a 256^2 photo: 1024^2) ...
 DEPTH_MAX = 4096           # ... at most this many per side
 NEAR = 0.1                 # near plane of the depth buffer and of the projection
+AO_RAYS = 256              # ambient occlusion: directions per point (steps of 1/256, below one 8-bit code) ...
+AO_T_MIN = 1e-3            # ... on segments from AO_T_MIN to AO_T_MAX times the diagonal of the occluder's box;
+AO_T_MAX = 0.1             # AO_T_MIN drops the hits at t = 0 on the faces around the vertex a ray starts from
 
 
 def check_size(texture_size):
@@ -113,8 +120,53 @@ def project_vertex_colors(vt, ft, rgb, view):
         return project(vt, ops.vertex_normals(vt, ft), rgb, view)
 
 
+def ao_directions(k=AO_RAYS):
+    """The golden-angle spiral on the unit disk lifted to the hemisphere by Malley's method (cosine-distributed):
+    d_i = (r cos phi, r sin phi, sqrt(1 - r^2)), r = sqrt((i + 1/2) / k), phi = i pi (3 - sqrt 5), in fp64 and rounded
+    once -> float32 [k,3]."""
+    i = np.arange(k, dtype=np.float64)
+    r2 = (i + 0.5) / k
+    r, phi = np.sqrt(r2), i * (np.pi * (3.0 - np.sqrt(5.0)))
+    return np.stack([r * np.cos(phi), r * np.sin(phi), np.sqrt(1.0 - r2)], 1).astype(np.float32)
+
+
+def ao_distances(verts):
+    """(t_min, t_max) float32 of the occluder verts [n,3]: AO_T_MIN and AO_T_MAX times the diagonal of their box,
+    sqrt((dx dx + dy dy) + dz dz) in fp64, each rounded once (0 without vertices)."""
+    v = np.asarray(verts, np.float32).reshape(-1, 3)
+    if len(v) == 0:
+        return np.float32(0.0), np.float32(0.0)
+    e = v.max(0).astype(np.float64) - v.min(0).astype(np.float64)
+    d = np.sqrt((e[0] * e[0] + e[1] * e[1]) + e[2] * e[2])
+    return np.float32(AO_T_MIN * d), np.float32(AO_T_MAX * d)
+
+
+def vertex_ao(vt, ft):
+    """AO [n] fp32 at the vertices of the mesh vt [n,3], ft [m,3] int32 (device tensors) against the mesh itself, with
+    its vertex normals (ops.vertex_normals; a vertex without faces gets 1)."""
+    with torch.cuda.device(vt.device):
+        return ops.ambient_occlusion(vt, ft, vt, ops.vertex_normals(vt, ft))
+
+
+def ao_transfer_fn(src_v, src_f, texture_size=None, device=None, seed=TRANSFER_SEED):
+    """An ao_fn for bake from a source mesh src_v [n,3], src_f [m,3]: its vertex AO (vertex_ao, computed now),
+    interpolated at each point's closest point on the face of its nearest source sample, with the same seeded samples
+    and search as transfer_fn."""
+    dev = _device(device)
+    sv = torch.from_numpy(np.ascontiguousarray(src_v, np.float32).reshape(-1, 3)).to(dev)
+    sf = torch.from_numpy(np.ascontiguousarray(src_f, np.int32).reshape(-1, 3)).to(dev)
+    with torch.cuda.device(dev):
+        fn = _transfer(sv, sf, vertex_ao(sv, sf)[:, None].expand(-1, 3).contiguous(), texture_size, seed)
+    return lambda points: fn(points)[:, 0]
+
+
+def ao_quantise(ao):
+    """AO [N,N] fp32 -> uint8 [N,N]: round_half_even(ao * 255) in fp32."""
+    return np.rint(ao.cpu().numpy().astype(np.float32) * np.float32(255)).clip(0, 255).astype(np.uint8)
+
+
 def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=False, normal_fn=None, atlas="faces",
-         view=None):
+         view=None, ao_fn=None):
     """vertices [n,3], faces [m,3] (numpy) -> (uv float32 [m,3,2], texture uint8 [N,N,3]); uv row k belongs to corner
     faces[f, k], in glTF's convention (v down the image, texel i's centre at (i + 0.5) / N).  colour_fn(points [T,3] fp32
     device tensor) -> rgb [T,3] in [0, 1] on the device, for the surface point behind every owned texel.  A texel whose
@@ -124,7 +176,8 @@ def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=Fal
     (ops.texture_atlas, one isometric chart per face) or "charts" (ops.chart_atlas, multi-face projected charts: denser
     and far fewer seams, stretch up to sqrt(3); its normal map is coded in the decoders' frame).  view: the input photo
     and its camera (prepare_view), blended into the texel colours with their faces' normals (ops.face_normals); with
-    return_atlas the dict then also holds the texels' project_weight [T]."""
+    return_atlas the dict then also holds the texels' project_weight [T].  ao_fn(points) -> AO [T] in [0, 1] (e.g.
+    ao_transfer_fn) adds an occlusion map uint8 [N,N] (ao_quantise of the push-pull filled AO) as the last result."""
     N = check_size(texture_size)
     check_atlas(atlas)
     dev = _device(device)
@@ -143,8 +196,12 @@ def bake(vertices, faces, texture_size, colour_fn, device=None, return_atlas=Fal
             tn = code(vt, ft, at["uv"], face, normal_fn(points).float().contiguous())
             nfill = ops.texture_fill(index, tn, at["owner"], N)
             extra.update(tangent_normals=tn, normal_fill=nfill, normal_map=ops.normal_quantise(nfill))
+        if ao_fn is not None:
+            ao = ao_fn(points).float().reshape(-1, 1).expand(-1, 3).contiguous()
+            extra.update(ao=ao[:, 0], ao_fill=ops.texture_fill(index, ao, at["owner"], N)[..., 0])
     uv, texture = at["uv"].cpu().numpy(), quantise(tex)
     res = (uv, texture) if normal_fn is None else (uv, texture, extra["normal_map"].cpu().numpy())
+    res = res if ao_fn is None else (*res, ao_quantise(extra["ao_fill"]))
     if return_atlas:
         return (*res, dict(at, texel_index=index, points=points, texel_face=face, rgb=rgb, **extra))
     return res

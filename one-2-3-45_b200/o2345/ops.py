@@ -727,3 +727,26 @@ def clean_mesh(verts, faces, min_component):
     stats = {"components": nc, "largest": largest, "dropped": nc - kept, "dropped_faces": nf - n_f, "enclosed": enclosed,
              "label": label, "area": area[:nc], "winding": winding[:nc], "keep": keep[:nc]}
     return vertex_index[:n_v], out[:n_f], stats
+
+
+# ----------------------------------------------------------------------------- ambient occlusion
+def ambient_occlusion(verts, faces, points, normals):
+    """AO [n] fp32 of points [n,3] with normals [n,3] (any length; zero or non-finite: 1) against the mesh verts [nv,3],
+    faces [nf,3] int32 (csrc/ao.cu; the rule is in include/o2345.h): the share of the mesh_texture.AO_RAYS directions of
+    mesh_texture.ao_directions, turned into each normal's frame, whose segment [t_min, t_max] (mesh_texture.ao_distances)
+    hits no face.  Deterministic.  Synchronises once; raises O2345Error for an index outside [0, nv) or a non-finite
+    coordinate."""
+    from .mesh_texture import ao_directions, ao_distances
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    points, normals = cf32(points).view(-1, 3), cf32(normals).view(-1, 3)
+    nv, nf, n, dev = verts.shape[0], faces.shape[0], points.shape[0], points.device
+    if normals.shape[0] != n:
+        raise ValueError(f"{n} points and {normals.shape[0]} normals")
+    dirs = torch.from_numpy(ao_directions()).to(dev)
+    t_min, t_max = ao_distances(verts.cpu().numpy())
+    nbytes = L.load().o2345_ambient_occlusion_scratch_bytes(nv, nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    out = torch.empty(n, dtype=_f32, device=dev)
+    L.call("o2345_ambient_occlusion", _f(verts), nv, _p(faces, _i32), nf, _f(points), _f(normals), n, _f(dirs), dirs.shape[0],
+           float(t_min), float(t_max), _p(scratch), nbytes, _f(out), _stream())
+    return out

@@ -68,7 +68,8 @@ class GenericTrainer(nn.Module):
 
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
                 alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None,
-                texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None):
+                texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None,
+                ambient_occlusion=False):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
@@ -77,7 +78,8 @@ class GenericTrainer(nn.Module):
             return self.export_mesh_step(sample, iter_step=iter_step, save_vis=save_vis, resolution=resolution,
                                          target_faces=target_faces, texture_size=texture_size, normal_map=normal_map,
                                          atlas=atlas, **({} if project_view is None else {"project_view": project_view}),
-                                         **({} if min_component is None else {"min_component": min_component}))
+                                         **({} if min_component is None else {"min_component": min_component}),
+                                         **({"ambient_occlusion": True} if ambient_occlusion else {}))
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -201,7 +203,8 @@ class GenericTrainer(nn.Module):
     # ------------------------------------------------------------------ mode='export_mesh'
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None,
-                         texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None):
+                         texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None,
+                         ambient_occlusion=False):
         """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
         after the vertex merge and before mesh.ply is written.  With texture_size N the final mesh's colours are also baked
         into an N x N texture (o2345/mesh_texture.py): the result gains uv [F,3,2] and texture uint8 [N,N,3]; mesh.ply is
@@ -212,9 +215,11 @@ class GenericTrainer(nn.Module):
         the shared intrinsics, rescaled from img_wh to the photo's size by mesh_texture.rescale_intrinsics), into the
         vertex colours and the baked texture (validate_colored_mesh).  min_component F: the components smaller than F times
         the largest one's area, or enclosed by it, are dropped after the vertex merge (o2345/mesh_clean.py), before
-        target_faces, the projection and the bake; the result gains clean (its counts)."""
+        target_faces, the projection and the bake; the result gains clean (its counts).  ambient_occlusion (needs
+        texture_size) also bakes an occlusion map (validate_colored_mesh): the result gains occlusion_texture."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
         kw = {} if min_component is None else {"min_component": min_component}
+        kw = dict(kw, ambient_occlusion=True) if ambient_occlusion else kw
         if project_view is not None:
             from .mesh_texture import rescale_intrinsics
             K = sample['intrinsics'][0][0].cpu().numpy()           # every view of a scene shares K (synthetic.scene_cameras)
@@ -251,14 +256,19 @@ class GenericTrainer(nn.Module):
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
                               iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None,
                               texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces", project_view=None,
-                              min_component=None):
+                              min_component=None, ambient_occlusion=False):
         """project_view: dict(photo, alpha, w2c, intr) of a camera in the normalised frame (mesh_texture.prepare_view): the
         photo is blended into the final mesh's vertex colours (its vertex normals) and baked texture (its face normals),
         with one depth buffer of that mesh; the result gains project_weight [n] (the vertices' weights of the photo).
         min_component: 0 < F <= 1, the welded mesh is cleaned (o2345/mesh_clean.py) before everything that follows; the
-        result gains clean, the counts of mesh_clean.clean."""
+        result gains clean, the counts of mesh_clean.clean.  ambient_occlusion (needs texture_size): the AO of every
+        vertex of the welded (and cleaned) full mesh, before target_faces, is transferred onto the final mesh's texels
+        (mesh_texture.ao_transfer_fn) and baked into occlusion_texture uint8 [N,N]; mesh.ply and the colours are as
+        without it."""
         if normal_map and texture_size is None:
             raise ValueError("normal_map needs texture_size")
+        if ambient_occlusion and texture_size is None:
+            raise ValueError("ambient_occlusion needs texture_size")
         bmin = torch.tensor(bound_min, dtype=torch.float32)
         bmax = torch.tensor(bound_max, dtype=torch.float32)
         vertices, triangles, fields = func_extract_geometry(
@@ -292,6 +302,11 @@ class GenericTrainer(nn.Module):
             # floating fragments and inner shells go before they take faces, texels or colours from the object
             from .mesh_clean import clean
             vertices, triangles, kept, cleaned = clean(vertices, triangles, kept, min_component, conditional_volume.device)
+        ao_fn = None
+        if ambient_occlusion:
+            # the full surface's own cavities, in the normalised frame, before simplification takes them out
+            from .mesh_texture import ao_transfer_fn
+            ao_fn = ao_transfer_fn(normalised[kept], triangles, texture_size, conditional_volume.device)
         if target_faces is not None:
             from .mesh_simplify import simplify
             vertices, triangles, kept, _ = simplify(vertices, triangles, kept, target_faces, conditional_volume.device)
@@ -324,8 +339,11 @@ class GenericTrainer(nn.Module):
                                              for c in p.split(colour_chunk)]) if len(p) else p)
             baked = bake(normalised[kept], triangles, texture_size, chunked, conditional_volume.device,
                          **({"normal_fn": gradient} if normal_map else {}), **({} if atlas == "faces" else {"atlas": atlas}),
-                         **({} if project_view is None else {"view": project_view}))
+                         **({} if project_view is None else {"view": project_view}),
+                         **({} if ao_fn is None else {"ao_fn": ao_fn}))
             out["uv"], out["texture"] = baked[:2]
             if normal_map:
                 out["normal_texture"] = baked[2]
+            if ao_fn is not None:
+                out["occlusion_texture"] = baked[-1]
         return out

@@ -1,5 +1,6 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--min_component F] [--target_faces N] [--texture_size N [--normal_map] [--atlas charts]]
+[--mesh_resolution R] [--min_component F] [--target_faces N] [--texture_size N [--normal_map] [--ambient_occlusion]
+[--atlas charts]]
 [--project_input] [--output_format .ply]`
 
 Command-line mirror of the reference's run.py:99-119 for the two accelerated paths: Zero123 stage 1 + stage 2
@@ -18,6 +19,10 @@ mesh to N faces on the GPU before mesh.ply is written (o2345/mesh_simplify.py); 
 the GPU (o2345/mesh_texture.py) and writes mesh.glb, or mesh.obj + mesh.mtl + mesh_albedo.png, textured; mesh.ply is
 written as without it.  `--normal_map` (with `--texture_size`) also bakes the SDF's gradient into a tangent-space normal
 map in the same uv: the GLB gains NORMAL, TANGENT and a normalTexture, the OBJ `vn` and mesh_normal.png (`norm`).
+`--ambient_occlusion` (with `--texture_size`) bakes an ambient occlusion map in the same uv: the share of 256
+cosine-distributed directions along which the full mesh (before `--target_faces`) is open within a tenth of its box
+diagonal, at every vertex on the GPU (o2345/mesh_texture.py), transferred to the texels.  The GLB gains an
+occlusionTexture, the OBJ mesh_occlusion.png (`map_ao`).
 `--atlas charts` (with `--texture_size`) packs multi-face projected charts instead of one chart per face (the default
 `faces`): the full marching-cubes mesh then fits textures of practical size, and only chart borders are seams.
 `--project_input` (not in the reference) projects the input photo onto the final mesh from the input camera, so the side
@@ -90,6 +95,8 @@ def parse_args(argv=None):
                     help='bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output only)')
     ap.add_argument('--normal_map', action='store_true',
                     help='also bake a tangent-space normal map from the SDF gradient (needs --texture_size; .obj or .glb output)')
+    ap.add_argument('--ambient_occlusion', action='store_true',
+                    help='also bake an ambient occlusion map of the full mesh (needs --texture_size; .obj or .glb output)')
     ap.add_argument('--atlas', choices=("faces", "charts"), default="faces",
                     help='texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)')
     ap.add_argument('--project_input', action='store_true',
@@ -116,6 +123,8 @@ def parse_args(argv=None):
             ap.error("--texture_size needs --output_format .obj or .glb")
     if args.normal_map and args.texture_size is None:
         ap.error("--normal_map needs --texture_size")
+    if args.ambient_occlusion and args.texture_size is None:
+        ap.error("--ambient_occlusion needs --texture_size")
     if args.atlas != "faces" and args.texture_size is None:
         ap.error("--atlas needs --texture_size")
     return args
@@ -139,7 +148,7 @@ def _write_format(shape_dir, output_format, mesh=None):
         from o2345.mesh_io import to_viewer_frame, write_textured
         v, f, uv = to_viewer_frame(mesh["vertices"], mesh["triangles"], mesh["uv"])
         mesh_path = os.path.join(shape_dir, f"mesh{output_format}")
-        write_textured(mesh_path, v, f, uv, mesh["texture"], mesh.get("normal_texture"))
+        write_textured(mesh_path, v, f, uv, mesh["texture"], mesh.get("normal_texture"), mesh.get("occlusion_texture"))
         return mesh_path
     mesh_path = os.path.join(shape_dir, "mesh.ply")
     if output_format == ".ply":          # reference run.py:113-118
@@ -156,6 +165,7 @@ def _texture_kw(args):
     kw = {} if args.min_component is None else {"min_component": args.min_component}
     kw = kw if args.texture_size is None else dict(kw, texture_size=args.texture_size)
     kw = kw if args.atlas == "faces" else dict(kw, atlas=args.atlas)
+    kw = dict(kw, ambient_occlusion=True) if args.ambient_occlusion else kw
     return dict(kw, normal_map=True) if args.normal_map else kw
 
 

@@ -20,6 +20,12 @@ writes it textured: .glb with the texture embedded, .obj beside <stem>.mtl and <
 tangent-space normal map, so the simplified mesh shades like the full one: the .glb gains NORMAL, TANGENT and a
 normalTexture, the .obj `vn` lines and <stem>_normal.png (`norm` in the MTL).
 
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out small.glb --target_faces 5000 --texture_size 2048 --ambient_occlusion
+
+--ambient_occlusion (with --texture_size) also bakes the welded input's ambient occlusion (at its vertices, against the
+input itself, transferred like the colours) into an occlusion map: the .glb gains an occlusionTexture, the .obj
+<stem>_occlusion.png (`map_ao` in the MTL).
+
     python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out full.glb --target_faces 1000000 --texture_size 1024 --atlas charts
 
 --atlas charts (with --texture_size) bakes into multi-face projected charts instead of one chart per face: meshes with
@@ -29,7 +35,8 @@ far more faces fit the texture, and only chart borders are seams.
 
 --min_component F (0 < F <= 1) cleans the welded input first (o2345/mesh_clean.py): components whose area is below F
 times the largest one's, and components enclosed by the largest one, are dropped.  The cleaned mesh is what is simplified
-and what the texture and normal map are transferred from, so a dropped fragment gives no texel its colour."""
+and what the texture, normal map and occlusion map are transferred from, so a dropped fragment gives no texel its colour
+and occludes nothing."""
 from __future__ import annotations
 
 import argparse
@@ -54,6 +61,8 @@ def parse_args(argv=None):
                     help="bake the colours into an N x N texture (a power of two in [64, 8192]; .obj or .glb output)")
     ap.add_argument("--normal_map", action="store_true",
                     help="also bake the input's normals into a tangent-space normal map (needs --texture_size)")
+    ap.add_argument("--ambient_occlusion", action="store_true",
+                    help="also bake the input's ambient occlusion into an occlusion map (needs --texture_size)")
     ap.add_argument("--atlas", choices=("faces", "charts"), default="faces",
                     help="texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)")
     ap.add_argument("--min_component", type=float, default=None,
@@ -75,6 +84,8 @@ def parse_args(argv=None):
             ap.error(f"--texture_size needs a {' or '.join(TEXTURED)} output")
     if args.normal_map and args.texture_size is None:
         ap.error("--normal_map needs --texture_size")
+    if args.ambient_occlusion and args.texture_size is None:
+        ap.error("--ambient_occlusion needs --texture_size")
     if args.atlas != "faces" and args.texture_size is None:
         ap.error("--atlas needs --texture_size")
     return args
@@ -115,12 +126,15 @@ def main(argv=None):
     print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     if args.texture_size is not None:
-        from o2345.mesh_texture import bake, normal_transfer_fn, transfer_fn
+        from o2345.mesh_texture import ao_transfer_fn, bake, normal_transfer_fn, transfer_fn
         nfn = normal_transfer_fn(*src[:2], texture_size=args.texture_size) if args.normal_map else None
+        afn = ao_transfer_fn(*src[:2], texture_size=args.texture_size) if args.ambient_occlusion else None
         baked = bake(v, f, args.texture_size, transfer_fn(*src, texture_size=args.texture_size), normal_fn=nfn,
-                     atlas=args.atlas)
-        print(f"baked a {args.texture_size} x {args.texture_size} texture" + (" and normal map" if args.normal_map else ""))
-        mesh_io.write_textured(args.out, v, f, *baked)
+                     atlas=args.atlas, ao_fn=afn)
+        print(f"baked a {args.texture_size} x {args.texture_size} texture" + (" and normal map" if args.normal_map else "")
+              + (" and occlusion map" if args.ambient_occlusion else ""))
+        mesh_io.write_textured(args.out, v, f, *baked[:2], normal_texture=baked[2] if args.normal_map else None,
+                               occlusion_texture=baked[-1] if args.ambient_occlusion else None)
         print("wrote", args.out)
         return (v, f, c, rounds, *baked)
     write_mesh(args.out, v, f, c)
