@@ -17,7 +17,8 @@
  *     a count once per round, o2345_texture_atlas reads its checks once and a fit flag per trial,
  *     o2345_vertex_normals reads its checks once, o2345_chart_atlas reads its checks, a flag per component pass,
  *     two values per chart round and a fit flag per trial, o2345_clean_mesh reads its checks, a flag per
- *     component pass, the component count and its counts, o2345_ambient_occlusion reads its checks once);
+ *     component pass, the component count and its counts, o2345_ambient_occlusion and o2345_closest_points read their
+ *     checks once, o2345_remesh reads its checks, its counts once per round and the output count);
  *   - `stream` is a cudaStream_t passed as void*; all work is enqueued on it;
  *   - return value 0 on success, negative O2345_E* otherwise; o2345_last_error() returns a
  *     thread-local description of the most recent failure.
@@ -36,6 +37,7 @@ extern "C" {
 #define O2345_EINVAL (-1)
 #define O2345_ECUDA (-2)
 #define O2345_EUNSUPPORTED (-3)
+#define O2345_ENOSPC (-4) /* o2345_remesh: the caller's capacities are too small (the counts it needs are returned) */
 
 #define O2345_ABI_VERSION 14 /* 2: o2345_epilogue, precision arguments of sdf_query / render_blend, GroupNorm as affine
                                  3: split-K inside the GEMM kernel (cluster per tile, private planes in the workspace), o2345_last_trap, o2345_debug_gemm_force
@@ -53,7 +55,8 @@ extern "C" {
                                     o2345_raster_mesh gained normals, tangents and face_ntex (after tex_info)
                                 13: multi-face charts: o2345_chart_atlas(_scratch_bytes), o2345_tangent_normals_decoded
                                 14: input-view projection: o2345_project_view, o2345_face_normals; mesh cleaning:
-                                    o2345_clean_mesh(_scratch_bytes); ambient occlusion: o2345_ambient_occlusion(_scratch_bytes)
+                                    o2345_clean_mesh(_scratch_bytes); ambient occlusion: o2345_ambient_occlusion(_scratch_bytes);
+                                    remeshing: o2345_closest_points(_scratch_bytes), o2345_remesh(_scratch_bytes), O2345_ENOSPC
                                     (added entry points only: the binding resolves every entry point by name, so a library
                                     without them fails to load) */
 
@@ -799,6 +802,66 @@ int64_t o2345_ambient_occlusion_scratch_bytes(int64_t nv, int64_t nf);
 int o2345_ambient_occlusion(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* points,
                             const float* normals, int64_t n, const float* dirs, int k, float t_min, float t_max,
                             void* scratch, int64_t scratch_bytes, float* out, o2345_stream_t stream);
+
+/* Closest points and isotropic remeshing (o2345/mesh_remesh.py, simplify_mesh.py --remesh; csrc/remesh.cu).
+ *
+ * Closest point.  For a point p (fp32, taken to fp64) and the reference mesh verts [nv,3], faces [nf,3]: over every face,
+ * the barycentrics (la, lb, lc) of the 7-region test of o2345_texel_points (corners A, B, C in face order, fp64), the
+ * point q = (la A + lb B) + lc C per component in fp64, d = q - p, d2 = (d.x d.x + d.y d.y) + d.z d.z; the face with the
+ * least (d2, face index) wins (so of duplicated faces the lowest index), and the point is q rounded to fp32.  The faces
+ * are searched through the LBVH of o2345_ambient_occlusion (padded face boxes, exact node boxes).  A node is skipped when
+ * its lower bound b > the best d2 so far, where per axis g = (lo - p) or (p - hi) outside the box (0 inside), minus the
+ * slack s = M 2^-44 (M the largest |coordinate| of the vertex box), floored at 0, and b = (gx gx + gy gy) + gz gz, every
+ * operation of g and b rounded downward.  Why this skips no face the brute force would pick: the computed q of a face
+ * lies within a few fp64 ulps of M of the face's box (the weights are in [0, 1] and sum to 1 within 2^-51), far inside
+ * s; the face's box is inside the node's; so the real |q_c - p_c| >= g_c per axis, rounding to nearest is monotone, and
+ * the face's computed d2 >= b > best.  Nodes with b = best are visited, so ties are decided by the face index as in the
+ * brute force, and the result equals it bit for bit.  A point with a non-finite coordinate, or nf = 0, gives NaN and
+ * face -1.  Returns O2345_EINVAL for a face index outside [0, nv) or a non-finite vertex (one synchronisation). */
+int64_t o2345_closest_points_scratch_bytes(int64_t nv, int64_t nf);
+int o2345_closest_points(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, const float* points, int64_t n,
+                         void* scratch, int64_t scratch_bytes, float* out_points, int32_t* out_face, o2345_stream_t stream);
+
+/* Remesh.  verts [nv,3] fp32, faces [nf,3] int32 (faces with a repeated index are dropped; an index outside [0, nv) or a
+ * non-finite coordinate is refused), target edge length L (fp32; the library's callers pass L = sqrt(4 A / (sqrt(3) N))
+ * rounded once to fp32, A the input's area summed in fp64 in ascending face order, N the target face count).  In fp64:
+ * hi = L (4/3), lo = L 0.8, hi2 = hi hi, lo2 = lo lo; len2(a, b) = (d.x d.x + d.y d.y) + d.z d.z, d = b - a from the fp32
+ * positions; an edge is long when len2 > hi2 and short when len2 < lo2.  Locks are the simplifier's (o2345_simplify),
+ * recomputed from the current faces at every round; a vertex without faces is locked.  The edge id of an edge is 3 g + k,
+ * its half-edge in its least face g.  Each of `iterations` iterations runs, on the mesh as the previous step left it:
+ *   split     rounds (at most 64 per iteration, fewer when a round splits nothing): each face's key is the greatest of
+ *             (bits(fp32(len2)) << 32) | edge id over its long edges with one or two faces; an edge splits when it is the
+ *             key of each of its faces.  The new vertices, numbered nv + i in edge-id order, are the fp32 midpoints
+ *             (a + b) * 0.5f (so a boundary edge's new vertex lies on it and is locked); a split face (p, q, r) on edge pq
+ *             (corners k, k + 1) becomes (p, m, r) and the face appended in face order is (m, q, r).  A round that would
+ *             exceed the capacities returns O2345_ENOSPC with counts_host[0..1] = the vertices and faces it needs;
+ *   collapse  rounds until none is accepted (each removes two faces per collapse: at most nf / 2 rounds): every unlocked
+ *             u proposes the neighbour v with the least (bits(fp32(len2(u, v))), v) among its short neighbours where u -> v
+ *             is the simplifier's legal collapse and every other neighbour x of u has len2(v, x) <= hi2; the key is
+ *             (bits << 32) | u, claims and acceptance are the simplifier's, and every accepted u -> v applies (u's faces
+ *             take v, the two faces of uv are deleted, the rest keep their order);
+ *   flip      rounds until none is accepted (every flip lowers the integer sum of (val - t)^2 over the mesh, t = 4 for a
+ *             locked vertex and 6 otherwise, so the rounds end): for the edge ab of a face f = (a, b, c) that is its
+ *             least face, with exactly two faces, the other holding b -> a with third vertex d: legal when d != c, cd is
+ *             not an edge, val(a), val(b) > 3 and the new faces (a, d, c), (d, b, c) have normals (B - A) x (C - A) whose
+ *             dot with both old faces' normals is > 0 (fp64, so no new face is degenerate or folded); the gain is the drop
+ *             of the sum over a, b, c, d, and a flip with gain > 0 claims its four vertices with the least key
+ *             ((2^30 - gain) << 32) | edge id; flips holding all four apply together: f := (a, d, c), the other := (d, b, c);
+ *   relax     every unlocked vertex p moves to p + (e - n (e . n)), e = c - p, c = (the sum of its neighbours' positions in
+ *             ascending index order, fp64, from 0) / their count, n its o2345_vertex_normals normal (fp32, taken to fp64),
+ *             e . n = (e.x n.x + e.y n.y) + e.z n.z, each component p + (e - n t) rounded to fp32; all from the positions
+ *             before the step (Jacobi);
+ *   project   every unlocked vertex moves to its closest point on the input mesh (as given, repeated-index faces included).
+ * Every floating-point operation is rounded to nearest in that order, without FMA contraction.  Outputs: out_verts
+ * [vertex_capacity,3] (the first counts_host[0] are the referenced vertices in index order: the input's, then the split
+ * vertices in creation order), out_faces [face_capacity,3] (the first counts_host[1], in their final order, renumbered),
+ * counts_host [5] (int64: vertices, faces, split rounds, collapse rounds, flip rounds).  The result does not depend on the
+ * capacities; capacities below nv, nf give O2345_ENOSPC at once.  L must be >= 2^-60 (+inf: no edge is long, every edge
+ * short: the mesh collapses as far as the rules allow).  scratch: 16-byte aligned. */
+int64_t o2345_remesh_scratch_bytes(int64_t nv, int64_t nf, int64_t vertex_capacity, int64_t face_capacity);
+int o2345_remesh(const float* verts, int64_t nv, const int32_t* faces, int64_t nf, float target_length, int iterations,
+                 int64_t vertex_capacity, int64_t face_capacity, void* scratch, int64_t scratch_bytes, float* out_verts,
+                 int32_t* out_faces, int64_t* counts_host, o2345_stream_t stream);
 
 #ifdef __cplusplus
 }

@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(HERE, "build")
 LIB = os.path.join(LIBDIR, "libo2345_sm90.so")
-SOURCES = ["api.cu", "sdf_mlp.cu", "costvol.cu", "spconv.cu", "mcubes.cu", "featnet.cu", "render.cu", "render_tc.cu", "sdf_mlp_tc.cu", "gemm_tc.cu", "unet_ops.cu", "attention.cu", "raster.cu", "metrics.cu", "simplify.cu", "texture.cu", "project.cu", "clean.cu", "ao.cu", "scan.cu", "mesh_common.cu"]
+SOURCES = ["api.cu", "sdf_mlp.cu", "costvol.cu", "spconv.cu", "mcubes.cu", "featnet.cu", "render.cu", "render_tc.cu", "sdf_mlp_tc.cu", "gemm_tc.cu", "unet_ops.cu", "attention.cu", "raster.cu", "metrics.cu", "simplify.cu", "texture.cu", "project.cu", "clean.cu", "ao.cu", "lbvh.cu", "remesh.cu", "scan.cu", "mesh_common.cu"]
 # no --use_fast_math: parity with the fp32 reference comes first
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [*ARCH, "-O3", "-lineinfo", "-std=c++17",

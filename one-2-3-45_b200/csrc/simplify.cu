@@ -23,18 +23,6 @@ constexpr int kSelect = 1024;                 // threads of the k-th key search
 constexpr uint64_t kNone = ~0ull;             // no proposal / no claim
 enum { kErr = 0, kFaces = 1, kAccepted = 2, kAlive = 3, kUsed = 4, kCtr = 8 };
 
-// the two other corners of face f (in corner order after u)
-__device__ __forceinline__ void others(const int32_t* __restrict__ F, int f, int u, int& a, int& b) {
-  int c0 = F[3 * f], c1 = F[3 * f + 1], c2 = F[3 * f + 2];
-  if (c0 == u) a = c1, b = c2;
-  else if (c1 == u) a = c2, b = c0;
-  else a = c0, b = c1;
-}
-
-__device__ __forceinline__ bool has(const int32_t* __restrict__ F, int f, int x) {
-  return F[3 * f] == x || F[3 * f + 1] == x || F[3 * f + 2] == x;
-}
-
 // ----------------------------------------------------------------------------- input
 // dst[i] = src[rows[i]] (faces)
 __global__ void gather_faces_kernel(const int32_t* __restrict__ src, const int32_t* __restrict__ rows, int64_t n,
@@ -47,47 +35,12 @@ __global__ void gather_faces_kernel(const int32_t* __restrict__ src, const int32
 
 // ----------------------------------------------------------------------------- adjacency (vertex_faces, mesh_common.cu)
 // One thread per vertex: counts its distinct neighbours and locks it unless every edge at it has exactly two faces and
-// its faces form one closed fan.
+// its faces form one closed fan (vertex_lock, mesh_common.cuh).
 __global__ void vertex_kernel(const int32_t* __restrict__ F, const int32_t* __restrict__ off, const int32_t* __restrict__ adj,
                               int nv, uint8_t* __restrict__ locked, int32_t* __restrict__ val) {
   int u = blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= nv) return;
-  const int32_t* L = adj + off[u];
-  int d = off[u + 1] - off[u];
-  int nval = 0;
-  bool ok = d > 0;
-  for (int j = 0; j < d; ++j) {
-    int ab[2];
-    others(F, L[j], u, ab[0], ab[1]);
-    for (int t = 0; t < 2; ++t) {
-      int cnt = 0;
-      bool before = false;
-      for (int i = 0; i < d; ++i)
-        if (has(F, L[i], ab[t])) ++cnt, before |= i < j;
-      nval += !before;
-      ok &= cnt == 2;
-    }
-  }
-  if (ok) {   // walk across the edges from face 0 until the walk returns to it
-    int a, b, x, prev = 0, seen = 1;
-    others(F, L[0], u, a, b);
-    x = b;
-    for (int step = 0; step < d; ++step) {
-      int j = -1, nx = -1;
-      for (int i = 0; i < d && j < 0; ++i) {
-        if (i == prev) continue;
-        int p, q;
-        others(F, L[i], u, p, q);
-        if (p == x) j = i, nx = q;
-        else if (q == x) j = i, nx = p;
-      }
-      if (j <= 0) break;
-      ++seen, x = nx, prev = j;
-    }
-    ok = seen == d;
-  }
-  locked[u] = !ok;
-  val[u] = nval;
+  locked[u] = vertex_lock(F, adj + off[u], off[u + 1] - off[u], u, val + u);
 }
 
 // Q[u] = sum over u's faces, in ascending face order, of w (p p^T) (10 entries, i <= j)
@@ -136,43 +89,6 @@ __device__ __forceinline__ float collapse_cost(const double* __restrict__ Q, con
   return c > 0.f ? c : 0.f;
 }
 
-// u -> v for an unlocked u (every edge at u has two faces): link condition, valences, no flipped or collapsed face
-__device__ bool legal(const float* __restrict__ V, const int32_t* __restrict__ F, const int32_t* __restrict__ off,
-                      const int32_t* __restrict__ adj, const int32_t* __restrict__ val, int u, int v) {
-  const int32_t* Lu = adj + off[u];
-  const int32_t* Lv = adj + off[v];
-  int du = off[u + 1] - off[u], dv = off[v + 1] - off[v];
-  int o[2] = {-1, -1}, no = 0;
-  for (int i = 0; i < du; ++i) {
-    int p, q;
-    others(F, Lu[i], u, p, q);
-    if (p == v || q == v) o[no++ & 1] = p == v ? q : p;
-  }
-  if (o[0] == o[1] || val[o[0]] < 4 || val[o[1]] < 4 || val[u] + val[v] - 4 < 3) return false;
-  for (int i = 0; i < du; ++i) {
-    int x[2];
-    others(F, Lu[i], u, x[0], x[1]);
-    for (int t = 0; t < 2; ++t) {
-      if (x[t] == v || x[t] == o[0] || x[t] == o[1]) continue;
-      for (int j = 0; j < dv; ++j)
-        if (has(F, Lv[j], x[t])) return false;
-    }
-  }
-  D3 pv = vert(V, v);
-  for (int i = 0; i < du; ++i) {
-    int f = Lu[i];
-    if (has(F, f, v)) continue;
-    int c[3] = {F[3 * f], F[3 * f + 1], F[3 * f + 2]};
-    D3 P[3] = {vert(V, c[0]), vert(V, c[1]), vert(V, c[2])};
-    D3 n0 = cross3(P[0], P[1], P[2]);
-#pragma unroll
-    for (int k = 0; k < 3; ++k)
-      if (c[k] == u) P[k] = pv;
-    if (!(dot3(cross3(P[0], P[1], P[2]), n0) > 0.0)) return false;
-  }
-  return true;
-}
-
 __device__ __forceinline__ void claim_ring(const int32_t* __restrict__ F, const int32_t* __restrict__ off,
                                            const int32_t* __restrict__ adj, int x, uint64_t key, uint64_t* __restrict__ claim) {
   for (int j = off[x]; j < off[x + 1]; ++j) {
@@ -212,7 +128,7 @@ __global__ void propose_kernel(const float* __restrict__ V, const int32_t* __res
     for (int t = 0; t < 2; ++t) {
       bool before = false;
       for (int i = 0; i < j && !before; ++i) before = has(F, L[i], x[t]);
-      if (before || !legal(V, F, off, adj, val, u, x[t])) continue;
+      if (before || !legal_collapse(V, F, off, adj, val, u, x[t])) continue;
       uint64_t c = ((uint64_t)__float_as_uint(collapse_cost(Q, V, u, x[t])) << 32) | (uint32_t)x[t];
       best = c < best ? c : best;
     }

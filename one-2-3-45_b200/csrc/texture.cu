@@ -55,44 +55,6 @@ __device__ __forceinline__ int base_corner(const float* __restrict__ V, const in
   return k0;
 }
 
-// Barycentrics (of a, b, c) of the point of triangle abc closest to p: the 7-region test (three corners, three edges,
-// the interior), in fp64.  A zero-length edge or a zero-area interior cannot divide by zero: the corner a is taken.
-struct Bary {
-  double a, b, c;
-};
-
-__device__ __forceinline__ Bary closest_point(D3 p, D3 a, D3 b, D3 c) {
-  D3 ab = sub3(b, a), ac = sub3(c, a), ap = sub3(p, a);
-  double d1 = dot3(ab, ap), d2 = dot3(ac, ap);
-  if (d1 <= 0.0 && d2 <= 0.0) return {1.0, 0.0, 0.0};
-  D3 bp = sub3(p, b);
-  double d3 = dot3(ab, bp), d4 = dot3(ac, bp);
-  if (d3 >= 0.0 && d4 <= d3) return {0.0, 1.0, 0.0};
-  double vc = __dsub_rn(__dmul_rn(d1, d4), __dmul_rn(d3, d2));
-  if (vc <= 0.0 && d1 >= 0.0 && d3 <= 0.0) {
-    double t = __dsub_rn(d1, d3), v = t > 0.0 ? __ddiv_rn(d1, t) : 0.0;
-    return {__dsub_rn(1.0, v), v, 0.0};
-  }
-  D3 cp = sub3(p, c);
-  double d5 = dot3(ab, cp), d6 = dot3(ac, cp);
-  if (d6 >= 0.0 && d5 <= d6) return {0.0, 0.0, 1.0};
-  double vb = __dsub_rn(__dmul_rn(d5, d2), __dmul_rn(d1, d6));
-  if (vb <= 0.0 && d2 >= 0.0 && d6 <= 0.0) {
-    double t = __dsub_rn(d2, d6), w = t > 0.0 ? __ddiv_rn(d2, t) : 0.0;
-    return {__dsub_rn(1.0, w), 0.0, w};
-  }
-  double va = __dsub_rn(__dmul_rn(d3, d6), __dmul_rn(d5, d4));
-  double e43 = __dsub_rn(d4, d3), e56 = __dsub_rn(d5, d6);
-  if (va <= 0.0 && e43 >= 0.0 && e56 >= 0.0) {
-    double t = __dadd_rn(e43, e56), w = t > 0.0 ? __ddiv_rn(e43, t) : 0.0;
-    return {0.0, __dsub_rn(1.0, w), w};
-  }
-  double den = __dadd_rn(__dadd_rn(va, vb), vc);
-  if (!(den > 0.0)) return {1.0, 0.0, 0.0};
-  double v = __ddiv_rn(vb, den), w = __ddiv_rn(vc, den);
-  return {__dsub_rn(__dsub_rn(1.0, v), w), v, w};
-}
-
 // (la * A + lb * B) + lc * C per component in fp32, the weights rounded to fp32 first
 __device__ __forceinline__ void blend3(const Bary& l, const float* A, const float* B, const float* C, float* out) {
   float la = __double2float_rn(l.a), lb = __double2float_rn(l.b), lc = __double2float_rn(l.c);
@@ -447,14 +409,7 @@ __global__ void vertex_normal_kernel(const float* __restrict__ V, const int32_t*
                                      float* __restrict__ out) {
   int64_t u = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (u >= nv) return;
-  D3 s = {0.0, 0.0, 0.0};
-  for (int j = off[u]; j < off[u + 1]; ++j) {
-    int64_t f = adj[j];
-    D3 n = cross3(vert(V, F[3 * f]), vert(V, F[3 * f + 1]), vert(V, F[3 * f + 2]));
-    s = {__dadd_rn(s.x, n.x), __dadd_rn(s.y, n.y), __dadd_rn(s.z, n.z)};
-  }
-  D3 r = {0.0, 0.0, 0.0};
-  unit3(s, r);
+  D3 r = vertex_normal(V, F, adj + off[u], off[u + 1] - off[u]);
   out[3 * u] = __double2float_rn(r.x), out[3 * u + 1] = __double2float_rn(r.y), out[3 * u + 2] = __double2float_rn(r.z);
 }
 

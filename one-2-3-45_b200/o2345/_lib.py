@@ -167,6 +167,11 @@ _SIGS = {
     "o2345_ambient_occlusion_scratch_bytes": (c_i64, [c_i64, c_i64]),
     "o2345_ambient_occlusion": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_i64, c_fp, C.c_int, C.c_float, C.c_float,
                                           c_fp, c_i64, c_fp, c_fp]),
+    "o2345_closest_points_scratch_bytes": (c_i64, [c_i64, c_i64]),
+    "o2345_closest_points": (C.c_int, [c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp]),
+    "o2345_remesh_scratch_bytes": (c_i64, [c_i64, c_i64, c_i64, c_i64]),
+    "o2345_remesh": (C.c_int, [c_fp, c_i64, c_fp, c_i64, C.c_float, C.c_int, c_i64, c_i64, c_fp, c_i64, c_fp, c_fp, c_fp,
+                               c_fp]),
     "o2345_ray_composite": (C.c_int, [c_fp, c_i64, C.c_int, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, C.c_float,
                                       C.c_float, C.c_int, C.c_float, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp, c_fp]),
 }
@@ -174,6 +179,9 @@ _SIGS = {
 EXPORTED = tuple(_SIGS)
 ABI_VERSION = 14         # include/o2345.h: O2345_ABI_VERSION
 _lib = None
+
+
+ENOSPC = -4              # include/o2345.h: O2345_ENOSPC
 
 
 class O2345Error(RuntimeError):

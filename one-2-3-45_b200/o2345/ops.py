@@ -750,3 +750,53 @@ def ambient_occlusion(verts, faces, points, normals):
     L.call("o2345_ambient_occlusion", _f(verts), nv, _p(faces, _i32), nf, _f(points), _f(normals), n, _f(dirs), dirs.shape[0],
            float(t_min), float(t_max), _p(scratch), nbytes, _f(out), _stream())
     return out
+
+
+# ----------------------------------------------------------------------------- remeshing
+def closest_points(verts, faces, points):
+    """Closest points of points [n,3] on the mesh verts [nv,3] fp32, faces [nf,3] int32 (csrc/remesh.cu; the rule is in
+    include/o2345.h): per point the least (squared distance, face index) of the 7-region closest point over all faces in
+    fp64, searched through an LBVH and equal to the search over all faces bit for bit -> (points [n,3] fp32, face [n]
+    int32); NaN and -1 for a non-finite point or no faces.  Synchronises once; raises O2345Error for an index outside
+    [0, nv) or a non-finite vertex."""
+    verts, faces, points = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3), cf32(points).view(-1, 3)
+    nv, nf, n, dev = verts.shape[0], faces.shape[0], points.shape[0], points.device
+    nbytes = L.load().o2345_closest_points_scratch_bytes(nv, nf)
+    scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+    out = torch.empty(n, 3, dtype=_f32, device=dev)
+    face = torch.empty(n, dtype=_i32, device=dev)
+    L.call("o2345_closest_points", _f(verts), nv, _p(faces, _i32), nf, _f(points), n, _p(scratch), nbytes, _f(out),
+           _p(face, _i32), _stream())
+    return out, face
+
+
+def remesh_mesh(verts, faces, target_length, iterations, vertex_capacity=None, face_capacity=None):
+    """Isotropic remesh of verts [nv,3] fp32, faces [nf,3] int32 (nf >= 1) at target edge length target_length (fp32)
+    for `iterations` iterations of split, collapse, flip, tangential relaxation and projection onto the input (csrc/
+    remesh.cu; the rules are in include/o2345.h) -> (verts [nv',3] fp32, faces [nf',3] int32, (split, collapse, flip
+    rounds)).  The buffers start at the given capacities (default: twice the input, at least 1024) and are regrown to
+    what a run reports it needs (O2345_ENOSPC) until it fits; the result does not depend on them.  Deterministic.
+    Synchronises once per round; raises O2345Error for an index outside [0, nv) or a non-finite coordinate."""
+    verts, faces = cf32(verts).view(-1, 3), faces.contiguous().view(-1, 3)
+    nv, nf, dev = verts.shape[0], faces.shape[0], verts.device
+    vcap = max(nv, int(vertex_capacity) if vertex_capacity is not None else max(2 * nv, 1024))
+    fcap = max(nf, int(face_capacity) if face_capacity is not None else max(2 * nf, 1024))
+    lib = L.load()
+    counts = (C.c_int64 * 5)()
+    while True:
+        nbytes = lib.o2345_remesh_scratch_bytes(nv, nf, vcap, fcap)
+        if nbytes < 0:
+            raise L.O2345Error(f"o2345_remesh_scratch_bytes: sizes out of range (nv {nv}, nf {nf}, capacities {vcap}, {fcap})")
+        scratch = torch.empty(max(nbytes, 1), dtype=_u8, device=dev)
+        out_v = torch.empty(vcap, 3, dtype=_f32, device=dev)
+        out_f = torch.empty(fcap, 3, dtype=_i32, device=dev)
+        rc = lib.o2345_remesh(_f(verts), nv, _p(faces, _i32), nf, float(target_length), int(iterations), vcap, fcap,
+                              _p(scratch), nbytes, _f(out_v), _p(out_f, _i32), counts, _stream())
+        if rc == L.ENOSPC:
+            vcap, fcap = max(int(counts[0]), 2 * vcap), max(int(counts[1]), 2 * fcap)
+            del scratch, out_v, out_f
+            continue
+        if rc != 0:
+            raise L.O2345Error(f"o2345_remesh failed with {rc}: {L.last_error()}")
+        L.add_launches(1)
+        return out_v[:counts[0]], out_f[:counts[1]], (int(counts[2]), int(counts[3]), int(counts[4]))

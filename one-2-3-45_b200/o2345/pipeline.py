@@ -219,23 +219,26 @@ def sample_from_views(stage1, stage2, pose, device, pin=False):
 
 
 def _simplify_kw(target_faces, texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None,
-                 ambient_occlusion=False):
+                 ambient_occlusion=False, remesh=False):
     # the keywords only when they are set: a trainer without mesh simplification or texture baking is called as before
     if atlas != "faces" and texture_size is None:
         raise ValueError("atlas needs texture_size")
+    if remesh and target_faces is None:
+        raise ValueError("remesh needs target_faces")
     kw = {} if target_faces is None else {"target_faces": target_faces}
     kw = kw if texture_size is None else dict(kw, texture_size=texture_size)
     kw = kw if atlas == "faces" else dict(kw, atlas=atlas)
     kw = kw if project_view is None else dict(kw, project_view=project_view)
     kw = kw if min_component is None else dict(kw, min_component=min_component)
     kw = dict(kw, ambient_occlusion=True) if ambient_occlusion else kw
+    kw = dict(kw, remesh=True) if remesh else kw
     return dict(kw, normal_map=True) if normal_map else kw
 
 
 @torch.no_grad()
 def image_to_mesh(zero123, trainer, input_u8, polar_angle=60, resolution=256, ddim_steps=75, stage2_steps=50, scale=3.0,
                   exp_dir=None, batched=True, target_faces=None, texture_size=None, normal_map=False, atlas="faces",
-                  project_view=None, min_component=None, ambient_occlusion=False):
+                  project_view=None, min_component=None, ambient_occlusion=False, remesh=False):
     """`python run.py --img_path X --half_precision` without SAM / elevation estimation: Zero123 stage 1 + stage 2
     (the reference's 10 DDIM sampler calls, run as two batched ones unless batched=False), camera set-up, cost volume, SDF grid, marching cubes, vertex colours.
     Returns dict(vertices, triangles, colors) as host numpy arrays (and writes mesh.ply when exp_dir is given); with
@@ -247,7 +250,9 @@ def image_to_mesh(zero123, trainer, input_u8, polar_angle=60, resolution=256, dd
     mesh from the input camera (GenericTrainer.export_mesh_step); the dict gains project_weight.  min_component: 0 < F
     <= 1, the components smaller than F times the largest one's area, or enclosed by it, are dropped after the vertex
     merge and before everything else (o2345/mesh_clean.py); the dict gains clean (the counts).  ambient_occlusion (needs
-    texture_size): the full mesh's vertex AO baked into an occlusion map in the same uv (occlusion_texture)."""
+    texture_size): the full mesh's vertex AO baked into an occlusion map in the same uv (occlusion_texture).  remesh (needs
+    target_faces): an isotropic remesh to about target_faces faces replaces the simplification (o2345/mesh_remesh.py);
+    everything after it, colours included, is taken on the remeshed mesh."""
     from .zero123 import generate_views
     dev = next(trainer.parameters()).device
     stage1, stage2, pose = generate_views(zero123, input_u8, polar_angle, ddim_steps, stage2_steps, scale, exp_dir, dev, batched=batched,
@@ -256,7 +261,7 @@ def image_to_mesh(zero123, trainer, input_u8, polar_angle=60, resolution=256, dd
     trainer.base_exp_dir = exp_dir
     return trainer(sample, mode="export_mesh", resolution=resolution,
                    **_simplify_kw(target_faces, texture_size, normal_map, atlas, project_view, min_component,
-                                  ambient_occlusion))
+                                  ambient_occlusion, remesh))
 
 
 # --------------------------------------------------------------------------------------
@@ -278,7 +283,8 @@ def pack_slices(n, max_pack):
 @torch.no_grad()
 def images_to_meshes(zero123, trainer, inputs_u8, polar_angles, seed=0, resolution=256, exp_dirs=None, *, max_pack=None,
                      indices=None, ddim_steps=75, stage2_steps=50, scale=3.0, target_faces=None, texture_size=None,
-                     normal_map=False, atlas="faces", project_views=None, min_component=None, ambient_occlusion=False):
+                     normal_map=False, atlas="faces", project_views=None, min_component=None, ambient_occlusion=False,
+                     remesh=False):
     """image_to_mesh for a list of images: a generator of (index, mesh) in input order.  The images go through Zero123 in
     packs of at most MAX_PACK (zero123.generate_views_multi: two sampler calls per pack), then each is reconstructed on its
     own (sample_from_views + trainer(..., mode="export_mesh")).
@@ -287,7 +293,7 @@ def images_to_meshes(zero123, trainer, inputs_u8, polar_angles, seed=0, resoluti
     positions in the caller's full list, default 0..n-1; a process that renders a share of a list passes the share's
     positions), so a mesh does not depend on the pack size, the number of processes or which one renders it; `index` is
     indices[i].  exp_dirs (one per image): stage1_8/, stage2_8/, pose.json and mesh.ply are written there.  max_pack
-    overrides MAX_PACK.  target_faces, texture_size, normal_map, atlas, min_component, ambient_occlusion: as in
+    overrides MAX_PACK.  target_faces, texture_size, normal_map, atlas, min_component, ambient_occlusion, remesh: as in
     image_to_mesh.
     project_views: one image_to_mesh project_view per image."""
     from .zero123 import generate_views_multi
@@ -309,5 +315,5 @@ def images_to_meshes(zero123, trainer, inputs_u8, polar_angles, seed=0, resoluti
             yield indices[a + i], trainer(sample, mode="export_mesh", resolution=resolution,
                                           **_simplify_kw(target_faces, texture_size, normal_map, atlas,
                                                          None if project_views is None else project_views[a + i],
-                                                         min_component, ambient_occlusion))
+                                                         min_component, ambient_occlusion, remesh))
         del views

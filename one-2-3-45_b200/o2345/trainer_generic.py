@@ -69,7 +69,7 @@ class GenericTrainer(nn.Module):
     def forward(self, sample, perturb_overwrite=-1, background_rgb=None, alpha_inter_ratio_lod0=0.0,
                 alpha_inter_ratio_lod1=0.0, iter_step=0, mode='train', save_vis=False, resolution=360, target_faces=None,
                 texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None,
-                ambient_occlusion=False):
+                ambient_occlusion=False, remesh=False):
         if mode == 'val':
             return self.val_step(sample, perturb_overwrite=perturb_overwrite, background_rgb=background_rgb,
                                  alpha_inter_ratio_lod0=alpha_inter_ratio_lod0, alpha_inter_ratio_lod1=alpha_inter_ratio_lod1,
@@ -79,7 +79,8 @@ class GenericTrainer(nn.Module):
                                          target_faces=target_faces, texture_size=texture_size, normal_map=normal_map,
                                          atlas=atlas, **({} if project_view is None else {"project_view": project_view}),
                                          **({} if min_component is None else {"min_component": min_component}),
-                                         **({"ambient_occlusion": True} if ambient_occlusion else {}))
+                                         **({"ambient_occlusion": True} if ambient_occlusion else {}),
+                                         **({"remesh": True} if remesh else {}))
         raise NotImplementedError(f"mode={mode!r}: only 'val' and 'export_mesh' run on the o2345 path")
 
     # ------------------------------------------------------------------ shared front end
@@ -204,7 +205,7 @@ class GenericTrainer(nn.Module):
     @torch.no_grad()
     def export_mesh_step(self, sample, iter_step=0, chunk_size=512, resolution=360, save_vis=False, target_faces=None,
                          texture_size=None, normal_map=False, atlas="faces", project_view=None, min_component=None,
-                         ambient_occlusion=False):
+                         ambient_occlusion=False, remesh=False):
         """The coloured marching-cubes mesh; with target_faces it is simplified to that many faces (o2345/mesh_simplify.py)
         after the vertex merge and before mesh.ply is written.  With texture_size N the final mesh's colours are also baked
         into an N x N texture (o2345/mesh_texture.py): the result gains uv [F,3,2] and texture uint8 [N,N,3]; mesh.ply is
@@ -216,10 +217,12 @@ class GenericTrainer(nn.Module):
         vertex colours and the baked texture (validate_colored_mesh).  min_component F: the components smaller than F times
         the largest one's area, or enclosed by it, are dropped after the vertex merge (o2345/mesh_clean.py), before
         target_faces, the projection and the bake; the result gains clean (its counts).  ambient_occlusion (needs
-        texture_size) also bakes an occlusion map (validate_colored_mesh): the result gains occlusion_texture."""
+        texture_size) also bakes an occlusion map (validate_colored_mesh): the result gains occlusion_texture.  remesh
+        (needs target_faces) replaces the simplification by an isotropic remesh (validate_colored_mesh)."""
         imgs, fmaps, cond, sizeW, sizeH = self._conditional_features(sample)
         kw = {} if min_component is None else {"min_component": min_component}
         kw = dict(kw, ambient_occlusion=True) if ambient_occlusion else kw
+        kw = dict(kw, remesh=True) if remesh else kw
         if project_view is not None:
             from .mesh_texture import rescale_intrinsics
             K = sample['intrinsics'][0][0].cpu().numpy()           # every view of a scene shares K (synthetic.scene_cameras)
@@ -256,7 +259,7 @@ class GenericTrainer(nn.Module):
                               lod=None, occupancy_mask=None, bound_min=[-1, -1, -1], bound_max=[1, 1, 1], meta='',
                               iter_step=0, scale_mat=None, trans_mat=None, img_wh=(256, 256), target_faces=None,
                               texture_size=None, colour_chunk=1 << 20, normal_map=False, atlas="faces", project_view=None,
-                              min_component=None, ambient_occlusion=False):
+                              min_component=None, ambient_occlusion=False, remesh=False):
         """project_view: dict(photo, alpha, w2c, intr) of a camera in the normalised frame (mesh_texture.prepare_view): the
         photo is blended into the final mesh's vertex colours (its vertex normals) and baked texture (its face normals),
         with one depth buffer of that mesh; the result gains project_weight [n] (the vertices' weights of the photo).
@@ -264,7 +267,12 @@ class GenericTrainer(nn.Module):
         result gains clean, the counts of mesh_clean.clean.  ambient_occlusion (needs texture_size): the AO of every
         vertex of the welded (and cleaned) full mesh, before target_faces, is transferred onto the final mesh's texels
         (mesh_texture.ao_transfer_fn) and baked into occlusion_texture uint8 [N,N]; mesh.ply and the colours are as
-        without it."""
+        without it.  remesh (needs target_faces): the welded (and cleaned) mesh in the normalised frame is remeshed
+        isotropically to about target_faces faces (o2345/mesh_remesh.py) instead of simplified; its vertices go to the
+        world frame by the same scale_mat / trans_mat formula, its colours are colour() at its own vertices (quantised as
+        above), and the projection and the bake read its arrays; the result gains remesh (mesh_remesh.remesh's stats)."""
+        if remesh and target_faces is None:
+            raise ValueError("remesh needs target_faces")
         if normal_map and texture_size is None:
             raise ValueError("normal_map needs texture_size")
         if ambient_occlusion and texture_size is None:
@@ -283,13 +291,17 @@ class GenericTrainer(nn.Module):
                                          conditional_valid_mask_volume, feature_maps, color_maps, w2cs, intrinsics, img_wh)[0]
         rgb = colour(vt)
         normalised = vertices
-        if scale_mat is not None:
-            sm = scale_mat.cpu().numpy()
-            vertices = vertices * sm[0][0, 0] + sm[0][:3, 3][None]
-        if trans_mat is not None:
-            tm = trans_mat.cpu().numpy().reshape(-1, 4, 4)[0]
-            vh = np.concatenate([vertices, np.ones_like(vertices[:, :1])], axis=1)
-            vertices = (vh @ tm.T)[:, :3]
+
+        def to_world(vertices):
+            if scale_mat is not None:
+                sm = scale_mat.cpu().numpy()
+                vertices = vertices * sm[0][0, 0] + sm[0][:3, 3][None]
+            if trans_mat is not None:
+                tm = trans_mat.cpu().numpy().reshape(-1, 4, 4)[0]
+                vh = np.concatenate([vertices, np.ones_like(vertices[:, :1])], axis=1)
+                vertices = (vh @ tm.T)[:, :3]
+            return vertices
+        vertices = to_world(vertices)
         colors = (rgb.cpu() * 255).numpy().astype(np.uint8)
         # trimesh.Trimesh(vertices, triangles, vertex_colors=...) with its default process=True merges coincident vertices
         # before the export (reference :1374-1380).  Marching-cubes vertices can only coincide on lattice points: the renderer
@@ -307,20 +319,32 @@ class GenericTrainer(nn.Module):
             # the full surface's own cavities, in the normalised frame, before simplification takes them out
             from .mesh_texture import ao_transfer_fn
             ao_fn = ao_transfer_fn(normalised[kept], triangles, texture_size, conditional_volume.device)
-        if target_faces is not None:
+        remeshed = None
+        if remesh:
+            # new vertices on the full surface: their own positions, world positions and colours
+            from .mesh_remesh import remesh as remesh_mesh
+            norm_k, triangles, remeshed = remesh_mesh(normalised[kept], triangles, None, target_faces,
+                                                      conditional_volume.device)
+            vertices = to_world(norm_k)
+            rgb_k0 = colour(torch.tensor(norm_k).to(conditional_volume)) if len(norm_k) else rgb[:0]
+            colors = (rgb_k0.cpu() * 255).numpy().astype(np.uint8)
+        elif target_faces is not None:
             from .mesh_simplify import simplify
             vertices, triangles, kept, _ = simplify(vertices, triangles, kept, target_faces, conditional_volume.device)
+        if not remesh:
+            norm_k = normalised[kept]
         weight = None
         if project_view is None:
-            colors = colors[kept]
+            colors = colors if remesh else colors[kept]
         else:
             # the final mesh in the normalised frame, where the query camera is
             from .mesh_texture import prepare_view, project_vertex_colors, quantise
             dev = conditional_volume.device
-            vk = torch.from_numpy(np.ascontiguousarray(normalised[kept], np.float32)).to(dev)
+            vk = torch.from_numpy(np.ascontiguousarray(norm_k, np.float32)).to(dev)
             fk = torch.from_numpy(np.ascontiguousarray(triangles, np.int32)).to(dev)
             project_view = prepare_view(vk, fk, project_view)
-            rgb_k, weight = project_vertex_colors(vk, fk, rgb[torch.from_numpy(np.asarray(kept)).long().to(dev)], project_view)
+            base = rgb_k0 if remesh else rgb[torch.from_numpy(np.asarray(kept)).long().to(dev)]
+            rgb_k, weight = project_vertex_colors(vk, fk, base, project_view)
             colors = quantise(rgb_k)
         if self.base_exp_dir is not None:
             os.makedirs(self.base_exp_dir, exist_ok=True)
@@ -328,6 +352,8 @@ class GenericTrainer(nn.Module):
         out = {"vertices": vertices, "triangles": triangles, "colors": colors, "fields": fields}
         if cleaned is not None:
             out["clean"] = cleaned
+        if remeshed is not None:
+            out["remesh"] = remeshed
         if weight is not None:
             out["project_weight"] = weight.cpu().numpy()           # each vertex's weight of the photo
         if texture_size is not None:
@@ -337,7 +363,7 @@ class GenericTrainer(nn.Module):
             # the normal map's source is the SDF gradient at the texel points: the reconstruction's own surface normal
             gradient = lambda p: (torch.cat([density_or_sdf_network.gradient(c, conditional_volume, lod)[:, 0]
                                              for c in p.split(colour_chunk)]) if len(p) else p)
-            baked = bake(normalised[kept], triangles, texture_size, chunked, conditional_volume.device,
+            baked = bake(norm_k, triangles, texture_size, chunked, conditional_volume.device,
                          **({"normal_fn": gradient} if normal_map else {}), **({} if atlas == "faces" else {"atlas": atlas}),
                          **({} if project_view is None else {"view": project_view}),
                          **({} if ao_fn is None else {"ao_fn": ao_fn}))

@@ -1,5 +1,5 @@
 """`python run.py --img_path P [P ...] [--polar_angle A [A ...]] [--seed S] [--gpu_idx N] [--half_precision]
-[--mesh_resolution R] [--min_component F] [--target_faces N] [--texture_size N [--normal_map] [--ambient_occlusion]
+[--mesh_resolution R] [--min_component F] [--target_faces N [--remesh]] [--texture_size N [--normal_map] [--ambient_occlusion]
 [--atlas charts]]
 [--project_input] [--output_format .ply]`
 
@@ -15,6 +15,8 @@ the EMA shadow (`model_ema.*`, reference ldm/modules/ema.py:14-21 + ddpm.py:180-
 attached and takes `cond_stage_model.*`; a file that lacks what the sampler needs is refused.  `--output_format .obj/.glb`
 follow reference utils/utils.py:31-45 (o2345/mesh_io.py).  `--target_faces N` (not in the reference) simplifies the
 mesh to N faces on the GPU before mesh.ply is written (o2345/mesh_simplify.py); .obj / .glb are converted from that mesh.
+`--remesh` (with `--target_faces N`) replaces that simplification by an isotropic remesh to about N near-equilateral faces
+whose vertices lie on the full mesh (o2345/mesh_remesh.py); colours, the projection and the bakes are taken on it.
 `--texture_size N` (not in the reference; .obj or .glb only) bakes the reconstruction's colours into an N x N texture on
 the GPU (o2345/mesh_texture.py) and writes mesh.glb, or mesh.obj + mesh.mtl + mesh_albedo.png, textured; mesh.ply is
 written as without it.  `--normal_map` (with `--texture_size`) also bakes the SDF's gradient into a tangent-space normal
@@ -103,6 +105,8 @@ def parse_args(argv=None):
                     help='project the input photo onto the mesh from the input camera (vertex colours and texture)')
     ap.add_argument('--min_component', type=float, default=None,
                     help='drop mesh components smaller than F times the largest one\'s area or enclosed by it (0 < F <= 1)')
+    ap.add_argument('--remesh', action='store_true',
+                    help='remesh isotropically to about --target_faces near-equilateral faces instead of simplifying')
     ap.add_argument('--no_ema', action='store_true', help='sample with model.* instead of the EMA shadow model_ema.* (the reference uses EMA)')
     ap.add_argument('--polar_angle', type=float, nargs='+', default=[60.0],
                     help='elevation of the input view in degrees (not estimated): one value, or one per image')
@@ -127,6 +131,8 @@ def parse_args(argv=None):
         ap.error("--ambient_occlusion needs --texture_size")
     if args.atlas != "faces" and args.texture_size is None:
         ap.error("--atlas needs --texture_size")
+    if args.remesh and args.target_faces is None:
+        ap.error("--remesh needs --target_faces")
     return args
 
 
@@ -166,6 +172,7 @@ def _texture_kw(args):
     kw = kw if args.texture_size is None else dict(kw, texture_size=args.texture_size)
     kw = kw if args.atlas == "faces" else dict(kw, atlas=args.atlas)
     kw = dict(kw, ambient_occlusion=True) if args.ambient_occlusion else kw
+    kw = dict(kw, remesh=True) if args.remesh else kw
     return dict(kw, normal_map=True) if args.normal_map else kw
 
 
@@ -176,6 +183,7 @@ def main(argv=None):
         raise SystemExit("run.py needs a CUDA device: the o2345 path has no CPU fallback")
     from o2345 import sharding, synthetic as S
     from o2345.mesh_clean import describe
+    from o2345.mesh_remesh import describe as describe_remesh
     from o2345.pipeline import build_networks, image_to_mesh, images_to_meshes
     from o2345.zero123 import build_zero123
     rank, world = int(os.environ.get("RANK", 0)), int(os.environ.get("WORLD_SIZE", 1))
@@ -216,6 +224,8 @@ def main(argv=None):
         mesh_path = _write_format(shape_dir, args.output_format, mesh)
         if "clean" in mesh:
             print(describe(mesh["clean"]))
+        if "remesh" in mesh:
+            print(describe_remesh(mesh["vertices"], mesh["triangles"], mesh["remesh"]))
         print(f"{len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", mesh_path)
         return mesh_path
@@ -233,6 +243,8 @@ def main(argv=None):
         paths.append(_write_format(shape_dirs[i], args.output_format, mesh))
         if "clean" in mesh:
             print(f"{args.img_path[i]}: {describe(mesh['clean'])}")
+        if "remesh" in mesh:
+            print(f"{args.img_path[i]}: {describe_remesh(mesh['vertices'], mesh['triangles'], mesh['remesh'])}")
         print(f"{args.img_path[i]}: {len(mesh['vertices'])} vertices, {len(mesh['triangles'])} triangles")
         print("Mesh saved to:", paths[-1])
     if world > 1:

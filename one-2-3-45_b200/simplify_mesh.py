@@ -33,6 +33,12 @@ far more faces fit the texture, and only chart borders are seams.
 
     python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out small.glb --target_faces 5000 --min_component 0.05
 
+--remesh replaces the simplification by an isotropic remesh to about --target_faces faces (o2345/mesh_remesh.py): long
+edges split, short ones collapse, edges flip towards valence 6 and the vertices relax and go back onto the input surface.
+Each vertex takes the input's colour at its closest point of the input.
+
+    python one-2-3-45_b200/simplify_mesh.py --in mesh.ply --out even.glb --target_faces 20000 --remesh
+
 --min_component F (0 < F <= 1) cleans the welded input first (o2345/mesh_clean.py): components whose area is below F
 times the largest one's, and components enclosed by the largest one, are dropped.  The cleaned mesh is what is simplified
 and what the texture, normal map and occlusion map are transferred from, so a dropped fragment gives no texel its colour
@@ -67,6 +73,8 @@ def parse_args(argv=None):
                     help="texture atlas: one chart per face (default) or multi-face projected charts (needs --texture_size)")
     ap.add_argument("--min_component", type=float, default=None,
                     help="first drop components smaller than F times the largest one's area or enclosed by it (0 < F <= 1)")
+    ap.add_argument("--remesh", action="store_true",
+                    help="remesh isotropically to about --target_faces near-equilateral faces instead of simplifying")
     args = ap.parse_args(argv)
     if os.path.splitext(args.inp)[1].lower() not in INPUTS:
         ap.error(f"{args.inp}: unsupported input format (only {', '.join(INPUTS)})")
@@ -122,8 +130,15 @@ def main(argv=None):
         v, f, c, stats = clean(v, f, c, args.min_component)
         print(f"cleaned: {describe(stats)}: {len(v)} vertices, {len(f)} faces")
     src = (v, f, c)
-    v, f, c, rounds = simplify(v, f, c, args.target_faces)
-    print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
+    if args.remesh:
+        from o2345.mesh_remesh import describe, remesh, surface_colors
+        v, f, stats = remesh(v, f, None, args.target_faces)
+        c = surface_colors(*src, v)
+        rounds = stats["rounds"]
+        print(describe(v, f, stats))
+    else:
+        v, f, c, rounds = simplify(v, f, c, args.target_faces)
+        print(f"simplified: {len(v)} vertices, {len(f)} faces in {rounds} rounds")
     os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
     if args.texture_size is not None:
         from o2345.mesh_texture import ao_transfer_fn, bake, normal_transfer_fn, transfer_fn
